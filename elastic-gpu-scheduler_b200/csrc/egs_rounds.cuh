@@ -395,6 +395,8 @@ struct MwArgs {
   int rke;                          // list entries per (shape, shard) held in shared memory
   int nw;                           // worker warps
   int use_hpay;                     // shared memory holds one prefetched candidate payload per shape
+  int pre_h, pre_cap;               // pre-install: the first pre_h merged candidates of every shape, at most pre_cap slots (0: off);
+                                    // shared memory then ends with int[NT]: the candidate entry each pre-installed slot comes from
 };
 
 template <int NS, int NT>
@@ -465,6 +467,11 @@ __device__ __forceinline__ void hset_add(SM &S, uint32_t node) {   // one lane, 
   unsigned i = hset_slot<SM>(node);
   while (S.hset[i] >= 0) i = (i + 1) & (unsigned)(SM::HS - 1);
   st_vol(&S.hset[i], (int)node);
+}
+template <class SM>
+__device__ __forceinline__ void hset_add_concurrent(SM &S, uint32_t node) {   // several lanes at once, distinct nodes
+  unsigned i = hset_slot<SM>(node);
+  while (atomicCAS(&S.hset[i], -1, (int)node) != -1) i = (i + 1) & (unsigned)(SM::HS - 1);
 }
 
 // The untracked candidate lists of shape s belong to its owner warp and are maintained LAZILY, outside the ticket:
@@ -757,9 +764,76 @@ __device__ __noinline__ int general_pod(SM &S, const MwArgs &a, const unsigned l
   return 0;
 }
 
+// ---- pre-install (DESIGN §3.1).  The winner rule max(best tracked option, best untracked head) does not depend on
+// WHICH nodes are tracked, so the prologue may track the round's likely winners before the first pod: their installs
+// then leave the ordered section.  Selection (one warp): rank r = 0..pre_h-1, shape s = 0..ns-1 in that order, the
+// entry of merged rank r of shape s over its D shard lists (a D-way merge on the lists' cursors), skipping nodes
+// already chosen, until pre_cap slots.  Slot numbers follow that order: a function of the lists only, so the
+// replicated resolvers of a sharded run make the same choice.  Returns the number of slots chosen.
+template <class SM>
+__device__ __noinline__ int preinstall_select(SM &S, const MwArgs &a, const unsigned long long *lk, int *psrc, int ns, int lane) {
+  const int D = a.n_shards, rke = a.rke, H = a.pre_h, cap = a.pre_cap;
+  int n = 0;
+  for (int r = 0; r < H && n < cap; r++) {
+    for (int g = 0; g < ns && n < cap; g += 32) {
+      const int s = g + lane;
+      int node = -1, src = 0;
+      if (s < ns) {
+        unsigned long long best = 0; int bd = 0, bc = 0;
+        for (int d = 0; d < D; d++) {
+          const int c = S.cur[s][d];
+          const unsigned long long k = c < S.len[s][d] ? lk[((size_t)s * D + d) * rke + c] : 0ull;
+          if (k > best) { best = k; bd = d; bc = c; }
+        }
+        if (best != 0) { S.cur[s][bd] = (uint8_t)(bc + 1); node = (int)key_node(best); src = (bd << 16) | (s * a.L.rkm + bc); }
+      }
+      bool take = node >= 0 && !hset_has(S, (uint32_t)node);
+      const unsigned same = __match_any_sync(0xffffffffu, take ? node : -1 - lane);
+      take = take && __ffs(same) - 1 == lane;                   // the lowest lane of a node chosen twice in this step
+      const unsigned tm = __ballot_sync(0xffffffffu, take);
+      const int t = n + __popc(tm & ((1u << lane) - 1u));
+      if (take && t < cap) { S.node[t] = node; psrc[t] = src; hset_add_concurrent(S, (uint32_t)node); }
+      n = min(cap, n + __popc(tm));
+      __syncwarp();
+    }
+  }
+  return n;
+}
+
+// Installs slots [0, nT) from their candidate entries, all threads.  install_slot without the ticket's parts: no
+// xbest (every owner scans all slots at its first pod) and no shape is observed yet, so OPT_NEW stays NEW (the first
+// pod of each shape turns it into CACHED).
+template <class SM>
+__device__ __noinline__ void preinstall_slots(SM &S, const MwArgs &a, const int *psrc, int nT, int ns) {
+  const int tid = threadIdx.x, nthreads = blockDim.x, nsc = a.L.nsc;
+  auto cand = [&](int t) -> const char * {
+    const int v = psrc[t];
+    return a.bufs + (size_t)(v >> 16) * a.L.bytes + a.L.off_cand + (size_t)(v & 0xFFFF) * a.L.cand_bytes;
+  };
+  for (int i = tid; i < nT * 2 * EGS_G; i += nthreads) {         // rc[8], rm[8] contiguous
+    const int t = i / (2 * EGS_G), f = i % (2 * EGS_G);
+    const int v = reinterpret_cast<const int *>(cand(t) + CD_RC)[f];
+    if (f < EGS_G) S.rc[t][f] = v; else S.rm[t][f - EGS_G] = v;
+  }
+  for (int t = tid; t < nT; t += nthreads) {
+    const char *cd = cand(t);
+    S.mt[t] = *reinterpret_cast<const int *>(cd + CD_MT); S.dirty[t] = 0; S.ver[t] = 0;
+    S.fterm[t] = *reinterpret_cast<const unsigned long long *>(cd + CD_FT);
+    S.sbase[t] = *reinterpret_cast<const unsigned long long *>(cd + CD_SB);
+  }
+  for (int i = tid; i < nT * ns; i += nthreads) {
+    const int t = i / ns, s2 = i - t * ns;
+    const char *cd = cand(t);
+    const uint8_t st = reinterpret_cast<const uint8_t *>(cd + CD_SC + 8 * nsc)[s2];
+    const unsigned long long k = (st == OPT_CACHED || st == OPT_NEW) ? cand_key(reinterpret_cast<const int *>(cd + CD_SC)[s2], (uint32_t)S.node[t]) : 0ull;
+    S.st[s2][t] = st; S.al[s2][t] = reinterpret_cast<const uint32_t *>(cd + CD_SC + 4 * nsc)[s2]; S.tkey[s2][t] = k;
+    if (st == OPT_ABSENT) { atomicOr(&S.pmask[s2][t >> 5], 1u << (t & 31)); S.pu[s2] = -2; }   // select leaves none; kept for safety
+  }
+}
+
 // ---- shared by the resolver kernels: round prologue (returns false when the batch is finished) and epilogue
 template <class SM>
-__device__ __noinline__ bool resolve_prologue(SM &S, const MwArgs &a, unsigned long long *lk) {
+__device__ __noinline__ bool resolve_prologue(SM &S, const MwArgs &a, unsigned long long *lk, int *psrc, int &n_pre) {
   constexpr int NS = (int)(sizeof(S.afit) / sizeof(int)), NT = SM::HS / 2;
   const int tid = threadIdx.x, nthreads = blockDim.x;
   const int D = a.n_shards, rke = a.rke;
@@ -803,6 +877,17 @@ __device__ __noinline__ bool resolve_prologue(SM &S, const MwArgs &a, unsigned l
     lk[e] = k < len ? *reinterpret_cast<const unsigned long long *>(a.bufs + (size_t)d * a.L.bytes + a.L.off_cand + ((size_t)s * a.L.rkm + k) * a.L.cand_bytes) : 0ull;
   }
   __syncthreads();
+  n_pre = 0;
+  if (NT > 128 && a.pre_cap > 0) {                               // the 128-slot resolver never pre-installs (preinstall_used)
+    if (tid < 32) {
+      const int n = preinstall_select(S, a, lk, psrc, ns, tid);
+      if (tid == 0) S.nT = n;
+    }
+    __syncthreads();
+    n_pre = S.nT;
+    preinstall_slots(S, a, psrc, n_pre, ns);
+    for (int i = tid; i < NS * RD; i += nthreads) (&S.cur[0][0])[i] = 0;   // the owners' list cursors start at the top
+  }
   if (tid == 0) {
     bool mono = true;                                            // all requests >= 0: rows only decrease in this round
     for (int s = 0; s < ns; s++) for (int c = 0; c < S.reqs[s].C; c++) mono &= S.reqs[s].core[c] >= 0 && S.reqs[s].mem[c] >= 0;
@@ -870,7 +955,9 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
   const int ns = a.rd->ns;
   unsigned long long *lk = reinterpret_cast<unsigned long long *>(smem_raw + ((sizeof(SM) + 15) & ~(size_t)15));   // [ns][D][rke]
   char *hpay = a.use_hpay ? reinterpret_cast<char *>(lk + (size_t)ns * D * rke) : nullptr;                        // [ns][cand_bytes]
-  if (!resolve_prologue(S, a, lk)) return;
+  int *psrc = reinterpret_cast<int *>(reinterpret_cast<char *>(lk + (size_t)ns * D * rke) + (a.use_hpay ? (size_t)ns * a.L.cand_bytes : 0));
+  int n_pre;
+  if (!resolve_prologue(S, a, lk, psrc, n_pre)) return;
   const int p0 = S.p0, p_end = S.p_end;
 #ifdef EGS_RESOLVE_PROF
   long long prof[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}; long long tprev = clock64();
@@ -1130,6 +1217,7 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
   __syncthreads();
   resolve_epilogue(S, a);
 #ifdef EGS_RESOLVE_PROF
+  if (warp == 0) prof[13] += n_pre;                             // pre-installed slots
   if (lane == 0 && warp < nw) for (int i = 0; i < 16; i++) atomicAdd((unsigned long long *)&a.ctl->prof[i], (unsigned long long)prof[i]);
 #endif
 }

@@ -106,6 +106,19 @@ static MwConfig mw_config(int ns) {
 }
 #define MW_SMEM_MAX 232448   // 227 KB opt-in limit per CTA on sm_90
 
+// Pre-install (DESIGN §3.1): the resolver's prologue fills 3/4 of the tracked table with the top NT / ns merged
+// candidates of every shape (at most half of a list held in shared memory, so no list runs dry at once); the last
+// quarter stays free for first pods and new winners.  Not in the 96-shape / 128-slot resolver: there (config 3:
+// multi-container shapes, nearly every pod a general pod whose in-ticket scans grow with the number of slots) it
+// measured slower.
+static bool preinstall_used(const MwConfig &cfg) { return cfg.inst != 2; }
+static void preinstall_geometry(const MwConfig &cfg, int ns, int rke, int &h, int &cap) {
+  h = 0; cap = 0;
+  if (!preinstall_used(cfg)) return;
+  h = std::max(1, std::min(cfg.nt / std::max(ns, 1), rke / 2));
+  cap = 3 * cfg.nt / 4;
+}
+
 // k_select grid: enough warps for one 128-node chunk each, at most two CTAs per SM (every CTA then runs in one wave)
 static int select_grid(const egs_handle *h) {
   const int chunks = (h->hi - h->lo + 127) / 128;
@@ -229,14 +242,15 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
   auto env_int = [](const char *k, int dflt) { const char *v = getenv(k); return v ? atoi(v) : dflt; };
   const int use_hpay = cfg.inst != 2 ? env_int("EGS_MW_HPAY", 2) : 0;   // prefetched candidate payload per shape (2: cp.async)
   const size_t hp_bytes = use_hpay ? (size_t)ns_cfg * L.cand_bytes : 0;
+  const size_t pre_bytes = preinstall_used(cfg) ? sizeof(int) * (size_t)cfg.nt : 0;   // after the payloads: see MwArgs::pre_h
   {
-    const size_t avail = MW_SMEM_MAX - cfg.smem_struct - hp_bytes;
+    const size_t avail = MW_SMEM_MAX - cfg.smem_struct - hp_bytes - pre_bytes;
     const size_t per = (size_t)ns_cfg * D * 8;
     if ((size_t)rke * per > avail) rke = (int)(avail / per) & ~1;   // even: what follows the lists stays 16-byte aligned
     if (rke < 4) return fail(h, EGS_ERR_BAD_ARG, "rounds: shape set too large for the resolver's shared memory");
   }
   const int nw = std::max(1, std::min(ns_cfg, env_int("EGS_MW_WARPS", MW_MAX_WARPS)));
-  const size_t smem = cfg.smem_struct + (size_t)ns_cfg * D * rke * 8 + hp_bytes;
+  const size_t smem = cfg.smem_struct + (size_t)ns_cfg * D * rke * 8 + hp_bytes + pre_bytes;
 
   SelectArgs sa; MergeArgs ma; MwArgs ra;
   sa.core = h->d_core; sa.mem = h->d_mem; sa.mem_total = h->d_mem_total;
@@ -248,6 +262,7 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
   ra.core = h->d_core; ra.mem = h->d_mem; ra.lo = h->lo; ra.hi = h->hi; ra.policy = h->policy; ra.n_shards = D;
   ra.rd = R.d_rd; ra.tb = tb; ra.obs_pending = R.d_obs; ra.bufs = R.d_bufs; ra.L = L; ra.pod_sidx = R.d_pod_sidx;
   ra.p0 = -1; ra.p_limit = 0; ra.out = out; ra.ctl = R.d_ctl; ra.rke = rke; ra.nw = nw; ra.use_hpay = use_hpay;
+  preinstall_geometry(cfg, ns_cfg, rke, ra.pre_h, ra.pre_cap);
 
   int ns_round = ns_cfg;                                        // grid of k_merge
   bool local_copied = false;

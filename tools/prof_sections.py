@@ -14,9 +14,9 @@ e.L.egs_debug_resolve_prof(e.h, out)
 v = [int(x) for x in out]
 print(e.rounds_stats(), "resolve ms", e.profile_get(3)[1], "select", e.profile_get(2)[1], "merge", e.profile_get(4)[1])
 fast, gen, hw = max(v[6], 1), max(v[9], 1), max(v[11], 1)
-print(f"pods: fast {v[6]} (head-wins {v[11]}), general {v[9]}")
+print(f"pods: fast {v[6]} (head-wins {v[11]}), general {v[9]}; slots pre-installed in the round prologues {v[13]}")
 print(f"  per-pod cycles (summed over owner warps / pods): prepare {v[0]/(fast+gen):.0f}  wait {v[1]/(fast+gen):.0f}  post {v[3]/fast:.0f}")
-print(f"  ticket: fast tracked-win {v[2]/max(fast-hw,1):.0f}  fast head-win {v[5]/hw:.0f} (install {v[12]/hw:.0f}, heads {v[13]/hw:.0f})  general {v[4]/gen:.0f}")
+print(f"  ticket: fast tracked-win {v[2]/max(fast-hw,1):.0f}  fast head-win {v[5]/hw:.0f}  general {v[4]/gen:.0f}")
 tw = max(fast - hw, 1)
 print(f"  tracked-win ticket split: rows+Trade {v[7]/tw:.0f}  winner {v[8]/tw:.0f}  transact reads {v[10]/tw:.0f}  stores+arrive {v[12]/tw:.0f}")
 print(f"  pending Trade redone inside the ticket (rows changed since the preparation): {v[14]} of {fast} fast pods")
