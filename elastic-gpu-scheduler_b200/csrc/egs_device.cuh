@@ -126,6 +126,24 @@ EGS_HD bool trade_single(const int (&c)[EGS_G], const int (&m)[EGS_G], int rc, i
   return bestkey >= 0;
 }
 
+// The same Trade as trade_single, one GPU per lane (the resolver's form: the lane holds the whole row, gl = its GPU).
+// Returns the lane's folded key -- (x >> 2) * 8 + gl under binpack, gl under spread, -1 when GPU gl does not fit;
+// the max over gl = 0..7 is trade_single's bestkey.  The max over the OTHER GPUs is a masked scan of the row.
+EGS_HD int trade_lane_key(const int (&c)[EGS_G], const int (&m)[EGS_G], int gl, int rq_c, int rq_m, int policy) {
+  unsigned ucmin = 0xFFFFFFFFu, ummin = 0xFFFFFFFFu;
+  int cex = INT32_MIN, mex = INT32_MIN, cg = 0, mg = 0;
+#pragma unroll
+  for (int g = 0; g < EGS_G; g++) {
+    ucmin = EGS_MIN(ucmin, (unsigned)c[g]); ummin = EGS_MIN(ummin, (unsigned)m[g]);
+    cex = EGS_MAX(cex, g == gl ? INT32_MIN : c[g]); mex = EGS_MAX(mex, g == gl ? INT32_MIN : m[g]);
+    cg = g == gl ? c[g] : cg; mg = g == gl ? m[g] : mg;
+  }
+  const bool ok = cg >= rq_c && mg >= rq_m;                      // CanAllocate gpu.go:55; PAD rows fail
+  const int nc = cg - rq_c, nm = mg - rq_m;                      // GPU.Add gpu.go:36-37
+  const int x = (EGS_MAX(mex, nm) + EGS_MAX(cex, nc)) - (EGS_MIN((int)ummin, nm) + EGS_MIN((int)ucmin, nc));
+  return !ok ? -1 : (policy == EGS_BINPACK ? (x >> 2) * 8 + gl : gl);
+}
+
 // ---------------------------------------------------------------------------------------------
 // General Trade: up to EGS_C containers, whole-GPU units, sentinel units.  Depth-first over
 // the containers exactly as gpu.go:72-123.  Cold path: rows live in local memory.

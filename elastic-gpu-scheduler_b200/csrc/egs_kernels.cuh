@@ -28,6 +28,18 @@ struct PodOut {              // per-pod outputs of the batch loop (device pointe
   unsigned long long *fit_digest, *score_digest;
 };
 
+// The six per-pod outputs of pod p; `masks` packs the EGS_C alloc bytes of the pod (one u8 GPU mask per container).
+__device__ __forceinline__ void write_pod_out(const PodOut &o, int p, int node, int status, int fit, unsigned long long fd,
+                                              unsigned long long sd, uint32_t masks) {
+  static_assert(EGS_C == 4, "alloc row == one 32-bit word");
+  if (o.node) o.node[p] = node;
+  if (o.status) o.status[p] = status;
+  if (o.fit_count) o.fit_count[p] = fit;
+  if (o.fit_digest) o.fit_digest[p] = fd;
+  if (o.score_digest) o.score_digest[p] = sd;
+  if (o.alloc) reinterpret_cast<uint32_t *>(o.alloc)[p] = masks;
+}
+
 struct PassArgs {
   const int32_t *core, *mem, *mem_total;   // rows are written by the bind in the last block
   int32_t *core_w, *mem_w;
@@ -153,13 +165,7 @@ __global__ void __launch_bounds__(PASS_THREADS) k_pass(PassArgs a) {
     } else if (key != 0) {
       node = (int)key_node(key); status = EGS_OK;
     }
-    const int p = a.pod;
-    if (a.out.node) a.out.node[p] = node;
-    if (a.out.status) a.out.status[p] = status;
-    if (a.out.alloc) for (int c = 0; c < EGS_C; c++) a.out.alloc[(size_t)p * EGS_C + c] = (uint8_t)(masks >> (8 * c));
-    if (a.out.fit_count) a.out.fit_count[p] = fit;
-    if (a.out.fit_digest) a.out.fit_digest[p] = fd;
-    if (a.out.score_digest) a.out.score_digest[p] = sd;
+    write_pod_out(a.out, a.pod, node, status, fit, fd, sd, masks);
   }
 }
 

@@ -88,6 +88,25 @@ static inline BufLayout make_layout(int ns, int rkm) {
 #define CD_FT 80
 #define CD_SB 88
 #define CD_SC 96
+#define CD_AL(nsc) (CD_SC + 4 * (nsc))
+#define CD_ST(nsc) (CD_SC + 8 * (nsc))
+
+// Read view of one candidate record (k_merge writes it).  Every reader goes through this view and cand_at.
+struct Cand {
+  const char *p; int nsc;
+  __device__ __forceinline__ unsigned long long key() const { return *reinterpret_cast<const unsigned long long *>(p + CD_KEY); }
+  __device__ __forceinline__ int row(int f) const { return reinterpret_cast<const int *>(p + CD_RC)[f]; }   // f < 16: rc[8], rm[8]
+  __device__ __forceinline__ int mt() const { return *reinterpret_cast<const int *>(p + CD_MT); }
+  __device__ __forceinline__ unsigned long long fterm() const { return *reinterpret_cast<const unsigned long long *>(p + CD_FT); }
+  __device__ __forceinline__ unsigned long long sbase() const { return *reinterpret_cast<const unsigned long long *>(p + CD_SB); }
+  __device__ __forceinline__ int sc(int s) const { return reinterpret_cast<const int *>(p + CD_SC)[s]; }
+  __device__ __forceinline__ uint32_t al(int s) const { return reinterpret_cast<const uint32_t *>(p + CD_AL(nsc))[s]; }
+  __device__ __forceinline__ uint8_t st(int s) const { return reinterpret_cast<const uint8_t *>(p + CD_ST(nsc))[s]; }
+};
+// entry k of the list of shape s in the candidate buffer of shard d
+__device__ __forceinline__ Cand cand_at(const char *bufs, const BufLayout &L, int d, int s, int k) {
+  return Cand{bufs + (size_t)d * L.bytes + L.off_cand + ((size_t)s * L.rkm + k) * L.cand_bytes, L.nsc};
+}
 
 struct AggPart { unsigned long long fd, sd; int fit, pad; };
 
@@ -345,8 +364,8 @@ __global__ void __launch_bounds__(256) k_merge(MergeArgs a) {
     if (f < EGS_G) reinterpret_cast<int *>(cd + CD_RC)[f] = a.core[node * EGS_G + f];
     else reinterpret_cast<int *>(cd + CD_RM)[f - EGS_G] = a.mem[node * EGS_G + f - EGS_G];
     int *csc = reinterpret_cast<int *>(cd + CD_SC);
-    uint32_t *cal = reinterpret_cast<uint32_t *>(cd + CD_SC + 4 * nsc);
-    uint8_t *cst = reinterpret_cast<uint8_t *>(cd + CD_SC + 8 * nsc);
+    uint32_t *cal = reinterpret_cast<uint32_t *>(cd + CD_AL(nsc));
+    uint8_t *cst = reinterpret_cast<uint8_t *>(cd + CD_ST(nsc));
     for (int s2 = f; s2 < nsc; s2 += 16) {
       uint8_t st = OPT_UNFIT; int32_t sc = 0; uint32_t al = 0;
       if (s2 < ns) {
@@ -394,9 +413,7 @@ struct MwArgs {
   RoundCtl *ctl;
   int rke;                          // list entries per (shape, shard) held in shared memory
   int nw;                           // worker warps
-  int use_hpay;                     // shared memory holds one prefetched candidate payload per shape
-  int pre_h, pre_cap;               // pre-install: the first pre_h merged candidates of every shape, at most pre_cap slots (0: off);
-                                    // shared memory then ends with int[NT]: the candidate entry each pre-installed slot comes from
+  int pre_h, pre_cap;               // pre-install: the first pre_h merged candidates of every shape, at most pre_cap slots
 };
 
 template <int NS, int NT>
@@ -428,6 +445,35 @@ struct MwSmem {
   int stop, stop_reason, stop_p, nT, n_observed, mono, p0, p_end;
 };
 #define MW_STOP 0x40000000
+
+// The resolver instances, by the size of the round's shape set: NS shapes, NT tracked slots, lists of RKM merged
+// candidates per shape and shard.  kHpay: shared memory holds one prefetched candidate payload per shape (cp.async).
+// kPreinstall: the prologue pre-installs the round's likely winners (DESIGN §3.1).  Neither is in the 96-shape /
+// 128-slot resolver: there (config 3: multi-container shapes, nearly every pod a general pod whose in-ticket scans grow
+// with the number of slots) pre-install measured slower.
+template <int NS_, int NT_, int RKM_, bool PRE_, bool HPAY_>
+struct MwInst {
+  static constexpr int NS = NS_, NT = NT_, RKM = RKM_;
+  static constexpr bool kPreinstall = PRE_, kHpay = HPAY_;
+  using Smem = MwSmem<NS, NT>;
+};
+using MwInst16 = MwInst<16, 512, 128, true, true>;
+using MwInst32 = MwInst<32, 256, 64, true, true>;
+using MwInst96 = MwInst<RSMAX, 128, 32, false, false>;
+
+// Dynamic shared memory of instance I: MwSmem, then the tail -- the lists lk (u64 [ns][D][rke]), the prefetched
+// payloads hpay (kHpay: [ns][cand_bytes]) and psrc (kPreinstall: int[NT], the candidate entry each pre-installed slot
+// comes from).  Byte offsets; `end` is the size.
+struct MwTail { size_t lk, hpay, psrc, end; };
+template <class I>
+__host__ __device__ __forceinline__ MwTail mw_tail(int ns, int D, int rke, int cand_bytes) {
+  MwTail t;
+  t.lk = (sizeof(typename I::Smem) + 15) & ~(size_t)15;
+  t.hpay = t.lk + (size_t)ns * D * rke * 8;
+  t.psrc = t.hpay + (I::kHpay ? (size_t)ns * cand_bytes : 0);
+  t.end = t.psrc + (I::kPreinstall ? sizeof(int) * I::NT : 0);
+  return t;
+}
 
 // Ticket hand-over: `turn` in shared memory names the pod whose ticket is open (bookkeeping, and the stop signal);
 // the owner of the next pod SLEEPS in hardware on its own mbarrier (try_wait suspends the warp) and is woken by ONE
@@ -509,55 +555,74 @@ __device__ __forceinline__ void maintain_heads(SM &S, const unsigned long long *
 // Trade of one fractional single-container request on a tracked node, one lane per GPU (lane & 7), every
 // lane holding the whole row: no shuffles until the final max.  Returns the folded key q*8+g (-1: no fit).
 __device__ __forceinline__ int trade_lanes(const int (&c)[EGS_G], const int (&m)[EGS_G], int gl, int rq_c, int rq_m, int policy) {
-  unsigned ucmin = 0xFFFFFFFFu, ummin = 0xFFFFFFFFu;
-  int cex = INT32_MIN, mex = INT32_MIN, cg = 0, mg = 0;
-#pragma unroll
-  for (int g = 0; g < EGS_G; g++) {
-    ucmin = min(ucmin, (unsigned)c[g]); ummin = min(ummin, (unsigned)m[g]);
-    cex = max(cex, g == gl ? INT32_MIN : c[g]); mex = max(mex, g == gl ? INT32_MIN : m[g]);
-    cg = g == gl ? c[g] : cg; mg = g == gl ? m[g] : mg;
-  }
-  const bool ok = cg >= rq_c && mg >= rq_m;                      // CanAllocate gpu.go:55; PAD rows fail
-  const int nc = cg - rq_c, nm = mg - rq_m;                      // GPU.Add gpu.go:36-37
-  const int x = (max(mex, nm) + max(cex, nc)) - (min((int)ummin, nm) + min((int)ucmin, nc));
-  const int key = !ok ? -1 : (policy == EGS_BINPACK ? (x >> 2) * 8 + gl : gl);
-  return __reduce_max_sync(0xffffffffu, key);
+  return __reduce_max_sync(0xffffffffu, trade_lane_key(c, m, gl, rq_c, rq_m, policy));
 }
 
-// A node becomes tracked: install the payload `cd` (node w) as slot t.  All lanes, inside the ticket of shape s_self.
+// ---- installing a tracked slot from its candidate record, in two parts shared by the ticket (install_slot, one warp)
+// and the prologue (preinstall_slots, the whole CTA).  The caller sets node[t] and enters the node in the tracked set.
+// Part f < 16 of the rows of slot t: rc[f] or rm[f - 8]; part 0 also writes the per-slot fields.
+template <class SM>
+__device__ __forceinline__ void install_rows(SM &S, const Cand &c, int t, int f) {
+  const int v = c.row(f);
+  if (f < EGS_G) S.rc[t][f] = v; else S.rm[t][f - EGS_G] = v;
+  if (f == 0) { S.mt[t] = c.mt(); S.dirty[t] = 0; S.ver[t] = 0; S.fterm[t] = c.fterm(); S.sbase[t] = c.sbase(); }
+}
+// The option of shape s2 on slot t (node w); an OPT_NEW option of an observed shape is an ordinary cached one.
+// Returns its key (0: not fit).
+template <class SM>
+__device__ __forceinline__ unsigned long long install_option(SM &S, const Cand &c, int t, uint32_t w, int s2, bool observed) {
+  uint8_t st = c.st(s2);
+  if (st == OPT_NEW && observed) st = OPT_CACHED;
+  const unsigned long long k = (st == OPT_CACHED || st == OPT_NEW) ? cand_key(c.sc(s2), w) : 0ull;
+  S.st[s2][t] = st; S.al[s2][t] = c.al(s2); S.tkey[s2][t] = k;
+  if (st == OPT_ABSENT) { atomicOr(&S.pmask[s2][t >> 5], 1u << (t & 31)); S.pu[s2] = -2; }   // select leaves none; kept for safety
+  return k;
+}
+
+// A node becomes tracked: install the record `c` (node w) as slot t.  All lanes, inside the ticket of shape s_self.
 // Other shapes learn about the slot through xbest (their owners scan only the slots they have seen).
 template <class SM>
-__device__ __noinline__ void install_slot(SM &S, const MwArgs &a, const char *cd, int t, uint32_t w, int ns, int s_self, int lane) {
-  const int nsc = a.L.nsc;
+__device__ __noinline__ void install_slot(SM &S, Cand c, int t, uint32_t w, int ns, int s_self, int lane) {
   if (lane < 2 * EGS_G) {
-    const int v = reinterpret_cast<const int *>(cd + CD_RC)[lane];          // rc[8], rm[8] contiguous
-    if (lane < EGS_G) S.rc[t][lane] = v; else S.rm[t][lane - EGS_G] = v;
+    install_rows(S, c, t, lane);
+    if (lane == 0) { S.node[t] = (int)w; hset_add(S, w); }
   }
-  if (lane == 0) {
-    S.node[t] = (int)w; S.mt[t] = *reinterpret_cast<const int *>(cd + CD_MT); S.dirty[t] = 0; S.ver[t] = 0;
-    S.fterm[t] = *reinterpret_cast<const unsigned long long *>(cd + CD_FT);
-    S.sbase[t] = *reinterpret_cast<const unsigned long long *>(cd + CD_SB);
-    hset_add(S, w);
-  }
-  const int *csc = reinterpret_cast<const int *>(cd + CD_SC);
-  const uint32_t *cal = reinterpret_cast<const uint32_t *>(cd + CD_SC + 4 * nsc);
-  const uint8_t *cst = reinterpret_cast<const uint8_t *>(cd + CD_SC + 8 * nsc);
   for (int s2 = lane; s2 < ns; s2 += 32) {
-    uint8_t st = cst[s2];
-    if (st == OPT_NEW && S.observed[s2]) st = OPT_CACHED;
-    const unsigned long long k = (st == OPT_CACHED || st == OPT_NEW) ? cand_key(csc[s2], w) : 0ull;
-    S.st[s2][t] = st; S.al[s2][t] = cal[s2]; S.tkey[s2][t] = k;
+    const unsigned long long k = install_option(S, c, t, w, s2, S.observed[s2] != 0);
     if (s2 != s_self && k > S.xbest[s2]) { S.xbest[s2] = k; S.xbest_t[s2] = t; }
-    if (st == OPT_ABSENT) { atomicOr(&S.pmask[s2][t >> 5], 1u << (t & 31)); S.pu[s2] = -2; }   // select leaves none; kept for safety
   }
 }
 
-// payload of the current best head of shape s: prefetched copy in shared memory, else the candidate buffer
+// record of the current best head of shape s: prefetched copy in shared memory, else the candidate buffer
 template <class SM>
-__device__ __forceinline__ const char *head_payload(const SM &S, const MwArgs &a, const char *hpay, int s, uint32_t w) {
-  if (hpay && S.hpay_node[s] == (int)w) return hpay + (size_t)s * a.L.cand_bytes;
+__device__ __forceinline__ Cand head_payload(const SM &S, const MwArgs &a, const char *hpay, int s, uint32_t w) {
+  if (hpay && S.hpay_node[s] == (int)w) return Cand{hpay + (size_t)s * a.L.cand_bytes, a.L.nsc};
   const int d = S.bh_d[s];
-  return a.bufs + (size_t)d * a.L.bytes + a.L.off_cand + ((size_t)s * a.L.rkm + S.cur[s][d]) * a.L.cand_bytes;
+  return cand_at(a.bufs, a.L, d, s, S.cur[s][d]);
+}
+
+// Single-container Transact (gpu.go:164-171) of GPU g of tracked slot t, all lanes, inside the ticket: the row is
+// written under the slot's seqlock.  Returns ok (the bind is recorded -- dirty -- either way).
+template <class SM>
+__device__ __forceinline__ int bind_single_slot(SM &S, int t, int g, int rq_c, int rq_m, int lane) {
+  const int c = S.rc[t][g], m = S.rm[t][g];
+  const int ok = (c >= rq_c && m >= rq_m) ? 1 : 0;
+  __syncwarp();                                                  // every lane has read the row
+  if (lane == 0) {
+    if (ok) { const int v = S.ver[t]; st_vol(&S.ver[t], v + 1); S.rc[t][g] = c - rq_c; S.rm[t][g] = m - rq_m; st_vol(&S.ver[t], v + 2); }
+    S.dirty[t] = 1;
+  }
+  return ok;
+}
+
+// node.go:90-92: the winning option (key win, slot t) of shape s is consumed; the aggregates (fit, fd, sd as this pod
+// saw them) lose its terms, and it is the shape's one pending option.  One lane.
+template <class SM>
+__device__ __forceinline__ void consume_option(SM &S, int s, int t, unsigned long long win, int fit, unsigned long long fd,
+                                               unsigned long long sd) {
+  S.st[s][t] = OPT_ABSENT; S.tkey[s][t] = 0; S.pmask[s][t >> 5] |= 1u << (t & 31);
+  S.afit[s] = fit - 1; S.afd[s] = fd - S.fterm[t]; S.asd[s] = sd - score_term_b(S.sbase[t], key_score(win));
+  S.pu[s] = t;
 }
 
 // General Trade of request r on the tracked slot whose rows are (rc, rm): the DFS leaves spread over the lanes
@@ -621,17 +686,11 @@ __device__ __noinline__ int general_pod(SM &S, const MwArgs &a, const unsigned l
           bool okl = false; int sc = 0; int t = 0;
           if (bsel >= 0) {                                       // group-uniform
             t = w * 32 + bsel;
-            const int c = S.rc[t][gl], m = S.rm[t][gl];
-            const int cmin = (int)__reduce_min_sync(gmask, (unsigned)c), mmin = (int)__reduce_min_sync(gmask, (unsigned)m);
-            const int c1 = __reduce_max_sync(gmask, c), m1 = __reduce_max_sync(gmask, m);
-            const int c2 = __reduce_max_sync(gmask, c == c1 ? INT32_MIN : c), m2 = __reduce_max_sync(gmask, m == m1 ? INT32_MIN : m);
-            const bool cu = __popc(__ballot_sync(gmask, c == c1)) == 1, mu = __popc(__ballot_sync(gmask, m == m1)) == 1;
-            const int cex = (c == c1 && cu) ? c2 : c1, mex = (m == m1 && mu) ? m2 : m1;   // max over the OTHER GPUs
-            const bool ok = c >= rq_c && m >= rq_m;                                         // gpu.go:55
-            const int nc = c - rq_c, nm = m - rq_m;
-            const int x = (max(mex, nm) + max(cex, nc)) - (min(mmin, nm) + min(cmin, nc));
-            const int key = !ok ? -1 : (a.policy == EGS_BINPACK ? (x >> 2) * 8 + gl : gl);
-            const int bk = __reduce_max_sync(gmask, key);
+            const int4 c0 = *reinterpret_cast<const int4 *>(&S.rc[t][0]), c1 = *reinterpret_cast<const int4 *>(&S.rc[t][4]);
+            const int4 m0 = *reinterpret_cast<const int4 *>(&S.rm[t][0]), m1 = *reinterpret_cast<const int4 *>(&S.rm[t][4]);
+            const int c[EGS_G] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+            const int m[EGS_G] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
+            const int bk = __reduce_max_sync(gmask, trade_lane_key(c, m, gl, rq_c, rq_m, a.policy));
             if (gl == 0) {
               if (bk >= 0) {
                 sc = a.policy == EGS_BINPACK ? (bk >> 3) * 100 : 0;
@@ -686,7 +745,6 @@ __device__ __noinline__ int general_pod(SM &S, const MwArgs &a, const unsigned l
   const unsigned long long ofd = S.afd[s], osd = S.asd[s];
   // ---- commit: NodeAllocator.Allocate (node.go:87-104) on the tracked copy, or NOFIT
   int o_node = -1, o_status = EGS_ERR_NOFIT; uint32_t o_masks = 0;
-  int pu_new = -1;
   if (win != 0) {
     int t = tw0;
     if (from_head) {
@@ -695,7 +753,7 @@ __device__ __noinline__ int general_pod(SM &S, const MwArgs &a, const unsigned l
       const uint32_t w = key_node(win);
       asm volatile("cp.async.wait_all;" ::: "memory");
       __syncwarp();
-      install_slot(S, a, head_payload(S, a, hpay, s, w), t, w, ns, s, lane);
+      install_slot(S, head_payload(S, a, hpay, s, w), t, w, ns, s, lane);
       __syncwarp();
       nT = t + 1;
       if (lane == 0) { __threadfence_block(); st_vol(&S.nT, nT); }
@@ -704,33 +762,22 @@ __device__ __noinline__ int general_pod(SM &S, const MwArgs &a, const unsigned l
     o_node = S.node[t];
     const uint32_t masks = S.al[s][t] & S.rq_cmask[s];
     const unsigned pbit = 1u << (t & 31);
+    // NodeAllocator.Allocate: Transact, then the deferred delete of the option (node.go:90-92)
     int ok = 0;
-    // deferred delete of the option (node.go:90-92) + aggregates
-    const int nfit = fitc - 1;
-    const unsigned long long nfd = ofd - S.fterm[t], nsd = osd - score_term_b(S.sbase[t], key_score(win));
-    const unsigned npm = S.pmask[s][t >> 5] | pbit;
-    if (single) {                                                 // GPUs.Transact gpu.go:164-171
-      const int g = __ffs(masks) - 1;
-      const int c = S.rc[t][g], m = S.rm[t][g], rc = S.rq_core[s], rm = S.rq_mem[s];
-      ok = (c >= rc && m >= rm) ? 1 : 0;
-      __syncwarp();                                               // all lanes have read before lane 0 writes
-      if (lane == 0) {
-        S.st[s][t] = OPT_ABSENT; S.tkey[s][t] = 0; S.pmask[s][t >> 5] = npm;
-        S.afit[s] = nfit; S.afd[s] = nfd; S.asd[s] = nsd; S.dirty[t] = 1;
-        if (ok) { const int v = S.ver[t]; st_vol(&S.ver[t], v + 1); S.rc[t][g] = c - rc; S.rm[t][g] = m - rm; st_vol(&S.ver[t], v + 2); }
-      }
+    if (single) {
+      ok = bind_single_slot(S, t, __ffs(masks) - 1, S.rq_core[s], S.rq_mem[s], lane);
+      if (lane == 0) consume_option(S, s, t, win, fitc, ofd, osd);
     } else {
       __syncwarp();
       if (lane == 0) {
-        S.st[s][t] = OPT_ABSENT; S.tkey[s][t] = 0; S.pmask[s][t >> 5] = npm;
-        S.afit[s] = nfit; S.afd[s] = nfd; S.asd[s] = nsd; S.dirty[t] = 1;
+        consume_option(S, s, t, win, fitc, ofd, osd);
+        S.dirty[t] = 1;
         const int v = S.ver[t]; st_vol(&S.ver[t], v + 1);
         ok = transact_row(S.rc[t], S.rm[t], S.mt[t], S.reqs[s], masks) ? 1 : 0;
         st_vol(&S.ver[t], v + 2);
       }
       ok = __shfl_sync(0xffffffffu, ok, 0);
     }
-    pu_new = t;
     // Rows changed.  (a) not-yet-observed NEW options of this node are void (only while some shape of the
     // round is unobserved); (b) UNFIT memos are void -- unless every request of the round is >= 0: rows
     // then only decrease and an option that did not fit can never fit (exact shortcut).
@@ -752,13 +799,8 @@ __device__ __noinline__ int general_pod(SM &S, const MwArgs &a, const unsigned l
     o_masks = ok ? masks : 0;
   }
   if (lane == 0) {
-    S.pu[s] = pu_new;                                           // every pending option of s was Traded above
-    if (a.out.node) a.out.node[p] = o_node;
-    if (a.out.status) a.out.status[p] = o_status;
-    if (a.out.fit_count) a.out.fit_count[p] = fitc;
-    if (a.out.fit_digest) a.out.fit_digest[p] = ofd;
-    if (a.out.score_digest) a.out.score_digest[p] = osd;
-    if (a.out.alloc) reinterpret_cast<uint32_t *>(a.out.alloc)[p] = o_masks;
+    if (win == 0) S.pu[s] = -1;                                 // every pending option of s was Traded above
+    write_pod_out(a.out, p, o_node, o_status, fitc, ofd, osd, o_masks);
   }
   __syncwarp();
   return 0;
@@ -785,7 +827,7 @@ __device__ __noinline__ int preinstall_select(SM &S, const MwArgs &a, const unsi
           const unsigned long long k = c < S.len[s][d] ? lk[((size_t)s * D + d) * rke + c] : 0ull;
           if (k > best) { best = k; bd = d; bc = c; }
         }
-        if (best != 0) { S.cur[s][bd] = (uint8_t)(bc + 1); node = (int)key_node(best); src = (bd << 16) | (s * a.L.rkm + bc); }
+        if (best != 0) { S.cur[s][bd] = (uint8_t)(bc + 1); node = (int)key_node(best); src = (bd << 16) | (s << 8) | bc; }
       }
       bool take = node >= 0 && !hset_has(S, (uint32_t)node);
       const unsigned same = __match_any_sync(0xffffffffu, take ? node : -1 - lane);
@@ -800,41 +842,25 @@ __device__ __noinline__ int preinstall_select(SM &S, const MwArgs &a, const unsi
   return n;
 }
 
-// Installs slots [0, nT) from their candidate entries, all threads.  install_slot without the ticket's parts: no
-// xbest (every owner scans all slots at its first pod) and no shape is observed yet, so OPT_NEW stays NEW (the first
-// pod of each shape turns it into CACHED).
+// Installs slots [0, nT) from their candidate entries (psrc: shard << 16 | shape << 8 | list position), all threads.
+// install_slot without the ticket's parts: no xbest (every owner scans all slots at its first pod) and no shape is
+// observed yet, so OPT_NEW stays NEW (the first pod of each shape turns it into CACHED).
 template <class SM>
 __device__ __noinline__ void preinstall_slots(SM &S, const MwArgs &a, const int *psrc, int nT, int ns) {
-  const int tid = threadIdx.x, nthreads = blockDim.x, nsc = a.L.nsc;
-  auto cand = [&](int t) -> const char * {
-    const int v = psrc[t];
-    return a.bufs + (size_t)(v >> 16) * a.L.bytes + a.L.off_cand + (size_t)(v & 0xFFFF) * a.L.cand_bytes;
-  };
-  for (int i = tid; i < nT * 2 * EGS_G; i += nthreads) {         // rc[8], rm[8] contiguous
-    const int t = i / (2 * EGS_G), f = i % (2 * EGS_G);
-    const int v = reinterpret_cast<const int *>(cand(t) + CD_RC)[f];
-    if (f < EGS_G) S.rc[t][f] = v; else S.rm[t][f - EGS_G] = v;
-  }
-  for (int t = tid; t < nT; t += nthreads) {
-    const char *cd = cand(t);
-    S.mt[t] = *reinterpret_cast<const int *>(cd + CD_MT); S.dirty[t] = 0; S.ver[t] = 0;
-    S.fterm[t] = *reinterpret_cast<const unsigned long long *>(cd + CD_FT);
-    S.sbase[t] = *reinterpret_cast<const unsigned long long *>(cd + CD_SB);
-  }
+  const int tid = threadIdx.x, nthreads = blockDim.x;
+  auto cand = [&](int t) { const int v = psrc[t]; return cand_at(a.bufs, a.L, v >> 16, (v >> 8) & 0xFF, v & 0xFF); };
+  for (int i = tid; i < nT * 2 * EGS_G; i += nthreads) install_rows(S, cand(i / (2 * EGS_G)), i / (2 * EGS_G), i % (2 * EGS_G));
   for (int i = tid; i < nT * ns; i += nthreads) {
     const int t = i / ns, s2 = i - t * ns;
-    const char *cd = cand(t);
-    const uint8_t st = reinterpret_cast<const uint8_t *>(cd + CD_SC + 8 * nsc)[s2];
-    const unsigned long long k = (st == OPT_CACHED || st == OPT_NEW) ? cand_key(reinterpret_cast<const int *>(cd + CD_SC)[s2], (uint32_t)S.node[t]) : 0ull;
-    S.st[s2][t] = st; S.al[s2][t] = reinterpret_cast<const uint32_t *>(cd + CD_SC + 4 * nsc)[s2]; S.tkey[s2][t] = k;
-    if (st == OPT_ABSENT) { atomicOr(&S.pmask[s2][t >> 5], 1u << (t & 31)); S.pu[s2] = -2; }   // select leaves none; kept for safety
+    install_option(S, cand(t), t, (uint32_t)S.node[t], s2, false);
   }
 }
 
 // ---- shared by the resolver kernels: round prologue (returns false when the batch is finished) and epilogue
-template <class SM>
-__device__ __noinline__ bool resolve_prologue(SM &S, const MwArgs &a, unsigned long long *lk, int *psrc, int &n_pre) {
-  constexpr int NS = (int)(sizeof(S.afit) / sizeof(int)), NT = SM::HS / 2;
+template <class I>
+__device__ __noinline__ bool resolve_prologue(typename I::Smem &S, const MwArgs &a, unsigned long long *lk, int *psrc, int &n_pre) {
+  using SM = typename I::Smem;
+  constexpr int NS = I::NS, NT = I::NT;
   const int tid = threadIdx.x, nthreads = blockDim.x;
   const int D = a.n_shards, rke = a.rke;
   const int ns = a.rd->ns;
@@ -874,11 +900,11 @@ __device__ __noinline__ bool resolve_prologue(SM &S, const MwArgs &a, unsigned l
   for (int e = tid; e < ns * D * rke; e += nthreads) {
     const int k = e % rke, sd = e / rke, d = sd % D, s = sd / D;
     const int len = reinterpret_cast<const int *>(a.bufs + (size_t)d * a.L.bytes + a.L.off_len)[s];
-    lk[e] = k < len ? *reinterpret_cast<const unsigned long long *>(a.bufs + (size_t)d * a.L.bytes + a.L.off_cand + ((size_t)s * a.L.rkm + k) * a.L.cand_bytes) : 0ull;
+    lk[e] = k < len ? cand_at(a.bufs, a.L, d, s, k).key() : 0ull;
   }
   __syncthreads();
   n_pre = 0;
-  if (NT > 128 && a.pre_cap > 0) {                               // the 128-slot resolver never pre-installs (preinstall_used)
+  if constexpr (I::kPreinstall) {
     if (tid < 32) {
       const int n = preinstall_select(S, a, lk, psrc, ns, tid);
       if (tid == 0) S.nT = n;
@@ -945,19 +971,20 @@ __device__ __noinline__ void resolve_epilogue(SM &S, const MwArgs &a) {
   }
 }
 
-template <int NS, int NT>
+template <class I>
 __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  using SM = MwSmem<NS, NT>;
+  using SM = typename I::Smem;
   SM &S = *reinterpret_cast<SM *>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int D = a.n_shards, rke = a.rke, nw = a.nw;
   const int ns = a.rd->ns;
-  unsigned long long *lk = reinterpret_cast<unsigned long long *>(smem_raw + ((sizeof(SM) + 15) & ~(size_t)15));   // [ns][D][rke]
-  char *hpay = a.use_hpay ? reinterpret_cast<char *>(lk + (size_t)ns * D * rke) : nullptr;                        // [ns][cand_bytes]
-  int *psrc = reinterpret_cast<int *>(reinterpret_cast<char *>(lk + (size_t)ns * D * rke) + (a.use_hpay ? (size_t)ns * a.L.cand_bytes : 0));
+  const MwTail tail = mw_tail<I>(ns, D, rke, a.L.cand_bytes);
+  unsigned long long *lk = reinterpret_cast<unsigned long long *>(smem_raw + tail.lk);
+  char *hpay = I::kHpay ? reinterpret_cast<char *>(smem_raw + tail.hpay) : nullptr;
+  int *psrc = reinterpret_cast<int *>(smem_raw + tail.psrc);
   int n_pre;
-  if (!resolve_prologue(S, a, lk, psrc, n_pre)) return;
+  if (!resolve_prologue<I>(S, a, lk, psrc, n_pre)) return;
   const int p0 = S.p0, p_end = S.p_end;
 #ifdef EGS_RESOLVE_PROF
   long long prof[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}; long long tprev = clock64();
@@ -1022,21 +1049,19 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
       // ======== preparation outside the ticket: only owner-private data and data that never changes
       maintain_heads(S, lk, D, rke, s, lane, false);
       const unsigned long long head = S.bh[s];
-      if (hpay && head != 0 && S.hpay_node[s] != (int)key_node(head)) {   // payload of the best head -> shared memory,
-        const int d = S.bh_d[s];                                          // asynchronously: only a head-win waits for it
-        const char *src = a.bufs + (size_t)d * a.L.bytes + a.L.off_cand + ((size_t)s * a.L.rkm + S.cur[s][d]) * a.L.cand_bytes;
-        char *dst = hpay + (size_t)s * a.L.cand_bytes;
-        if (a.use_hpay == 2) {
+      if constexpr (I::kHpay) {
+        if (head != 0 && S.hpay_node[s] != (int)key_node(head)) {         // payload of the best head -> shared memory,
+          const int d = S.bh_d[s];                                        // asynchronously: only a head-win waits for it
+          const char *src = cand_at(a.bufs, a.L, d, s, S.cur[s][d]).p;
+          char *dst = hpay + (size_t)s * a.L.cand_bytes;
           asm volatile("cp.async.wait_all;" ::: "memory");                // an older copy into this buffer has long landed
           for (int i = lane; i < a.L.cand_bytes / 16; i += 32)
             asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(dst + i * 16)), "l"(src + i * 16) : "memory");
           asm volatile("cp.async.commit_group;" ::: "memory");
-        } else {
-          for (int i = lane; i < a.L.cand_bytes / 16; i += 32) reinterpret_cast<int4 *>(dst)[i] = reinterpret_cast<const int4 *>(src)[i];
+          __syncwarp();                                                   // every lane has compared hpay_node
+          if (lane == 0) S.hpay_node[s] = (int)key_node(head);
+          __syncwarp();
         }
-        __syncwarp();                                                     // every lane has compared hpay_node
-        if (lane == 0) S.hpay_node[s] = (int)key_node(head);
-        __syncwarp();
       }
       // n_observed BEFORE pu: other warps write pu[s] / the aggregates of s (general_pod, inside their tickets) only while
       // some shape of the round is unobserved; once n_observed == ns was seen, everything read below is owner-private
@@ -1124,7 +1149,7 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
         const bool from_head = reason == 0 && hd > best;
         const unsigned long long win = from_head ? hd : best;
         int nT = 0;
-        if (from_head) { nT = S.nT; if (nT >= NT) reason = 2; }
+        if (from_head) { nT = S.nT; if (nT >= I::NT) reason = 2; }
 #ifdef EGS_RESOLVE_PROF
         long long q2_ = clock64() + (reason & 0) + ((int)win & 0);
         long long q3_ = q2_;
@@ -1137,30 +1162,23 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
               const uint32_t w = key_node(win);
               asm volatile("cp.async.wait_all;" ::: "memory");
               __syncwarp();
-              install_slot(S, a, head_payload(S, a, hpay, s, w), tw, w, ns, s, lane);
+              install_slot(S, head_payload(S, a, hpay, s, w), tw, w, ns, s, lane);
               __syncwarp();
               masks = S.al[s][tw] & 0xFFu;
               PROF_C(11, 1)
             } else if (masks == 0) {
               masks = S.al[s][tw] & 0xFFu;                        // a slot another shape installed
             }
-            const int g = __ffs(masks) - 1;
-            const int cc = S.rc[tw][g], mm = S.rm[tw][g];
-            const int ok = (cc >= rq_c && mm >= rq_m) ? 1 : 0;    // GPUs.Transact gpu.go:164-171
             o_node = S.node[tw];
+            const int ok = bind_single_slot(S, tw, __ffs(masks) - 1, rq_c, rq_m, lane);
 #ifdef EGS_RESOLVE_PROF
             q3_ = clock64() + (ok & 0) + (o_node & 0);
 #endif
-            __syncwarp();                                         // every lane has read the row
-            if (lane == 0) {
-              if (ok) { const int v = S.ver[tw]; st_vol(&S.ver[tw], v + 1); S.rc[tw][g] = cc - rq_c; S.rm[tw][g] = mm - rq_m; st_vol(&S.ver[tw], v + 2); }
-              S.dirty[tw] = 1;
-              if (from_head) { __threadfence_block(); st_vol(&S.nT, nT + 1); }
-            }
             o_status = ok ? EGS_OK : EGS_ERR_TRANSACT; o_masks = ok ? masks : 0;
           }
           // ---- hand the ticket on (arrive = release), then the owner-private part
           if (lane == 0) {
+            if (from_head) { __threadfence_block(); st_vol(&S.nT, nT + 1); }
             if (xb != 0) { S.xbest[s] = 0; S.xbest_t[s] = -1; }
             st_vol(&S.turn, p + 1);
             if (wake >= 0) mbar_arrive(&S.mbar[wake]);
@@ -1180,20 +1198,9 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
               else S.st[s][u] = OPT_UNFIT;
               S.pmask[s][u >> 5] &= ~(1u << (u & 31));
             }
-            if (win != 0) {                                       // node.go:90-92: the entry is consumed
-              S.st[s][tw] = OPT_ABSENT; S.tkey[s][tw] = 0; S.pmask[s][tw >> 5] |= 1u << (tw & 31);
-              S.afit[s] = fit - 1; S.afd[s] = fd - S.fterm[tw]; S.asd[s] = sd - score_term_b(S.sbase[tw], key_score(win));
-              S.pu[s] = tw;
-            } else {
-              S.afit[s] = fit; S.afd[s] = fd; S.asd[s] = sd;
-              S.pu[s] = -1;
-            }
-            if (a.out.node) a.out.node[p] = o_node;
-            if (a.out.status) a.out.status[p] = o_status;
-            if (a.out.fit_count) a.out.fit_count[p] = fit;
-            if (a.out.fit_digest) a.out.fit_digest[p] = fd;
-            if (a.out.score_digest) a.out.score_digest[p] = sd;
-            if (a.out.alloc) reinterpret_cast<uint32_t *>(a.out.alloc)[p] = o_masks;
+            if (win != 0) consume_option(S, s, tw, win, fit, fd, sd);
+            else { S.afit[s] = fit; S.afd[s] = fd; S.asd[s] = sd; S.pu[s] = -1; }
+            write_pod_out(a.out, p, o_node, o_status, fit, fd, sd, o_masks);
           }
           __syncwarp();
           PROF_T(3)

@@ -94,29 +94,24 @@ static int rounds_comm_init_local(egs_handle **handles, int world) {
   return EGS_OK;
 }
 
-// ---- resolver configuration by the size of the round's shape set
-struct MwConfig { int inst; int nt; int rkm; size_t smem_struct; };
-static MwConfig mw_config(int ns) {
-  MwConfig c;
-  if (ns <= 16) { c.inst = 0; c.nt = 512; c.rkm = 128; c.smem_struct = sizeof(MwSmem<16, 512>); }
-  else if (ns <= 32) { c.inst = 1; c.nt = 256; c.rkm = 64; c.smem_struct = sizeof(MwSmem<32, 256>); }
-  else { c.inst = 2; c.nt = 128; c.rkm = 32; c.smem_struct = sizeof(MwSmem<RSMAX, 128>); }
-  c.smem_struct = (c.smem_struct + 15) & ~(size_t)15;
-  return c;
+// ---- the resolver instance for a round set of ns shapes: f(MwInst16()), f(MwInst32()) or f(MwInst96())
+template <class F>
+static auto mw_dispatch(int ns, F &&f) {
+  if (ns <= MwInst16::NS) return f(MwInst16());
+  if (ns <= MwInst32::NS) return f(MwInst32());
+  return f(MwInst96());
 }
 #define MW_SMEM_MAX 232448   // 227 KB opt-in limit per CTA on sm_90
 
 // Pre-install (DESIGN §3.1): the resolver's prologue fills 3/4 of the tracked table with the top NT / ns merged
 // candidates of every shape (at most half of a list held in shared memory, so no list runs dry at once); the last
-// quarter stays free for first pods and new winners.  Not in the 96-shape / 128-slot resolver: there (config 3:
-// multi-container shapes, nearly every pod a general pod whose in-ticket scans grow with the number of slots) it
-// measured slower.
-static bool preinstall_used(const MwConfig &cfg) { return cfg.inst != 2; }
-static void preinstall_geometry(const MwConfig &cfg, int ns, int rke, int &h, int &cap) {
+// quarter stays free for first pods and new winners.  Only in the instances with kPreinstall.
+template <class I>
+static void preinstall_geometry(int ns, int rke, int &h, int &cap) {
   h = 0; cap = 0;
-  if (!preinstall_used(cfg)) return;
-  h = std::max(1, std::min(cfg.nt / std::max(ns, 1), rke / 2));
-  cap = 3 * cfg.nt / 4;
+  if (!I::kPreinstall) return;
+  h = std::max(1, std::min(I::NT / std::max(ns, 1), rke / 2));
+  cap = 3 * I::NT / 4;
 }
 
 // k_select grid: enough warps for one 128-node chunk each, at most two CTAs per SM (every CTA then runs in one wave)
@@ -132,9 +127,10 @@ static int rounds_ensure(egs_handle *h, int P, const BufLayout &L) {
     CK(h, cudaMallocHost(&R.h_ctl, sizeof(RoundCtl)));
     CK(h, cudaMalloc(&R.d_rd, sizeof(RoundDesc)));
     CK(h, cudaMallocHost(&R.h_rd, sizeof(RoundDesc)));
-    CK(h, cudaFuncSetAttribute(k_resolve_mw<16, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, MW_SMEM_MAX));
-    CK(h, cudaFuncSetAttribute(k_resolve_mw<32, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, MW_SMEM_MAX));
-    CK(h, cudaFuncSetAttribute(k_resolve_mw<RSMAX, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, MW_SMEM_MAX));
+    for (int ns : {MwInst16::NS, MwInst32::NS, MwInst96::NS})
+      CK(h, mw_dispatch(ns, [](auto i) {
+        return cudaFuncSetAttribute(k_resolve_mw<decltype(i)>, cudaFuncAttributeMaxDynamicSharedMemorySize, MW_SMEM_MAX);
+      }));
   }
   const size_t need = (size_t)L.bytes * RD;
   if (need > R.bufs_cap) {
@@ -192,11 +188,11 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
   }
   const bool one_set = (int)batch_shapes.size() <= RSMAX;
   const int ns_cfg = one_set ? (int)batch_shapes.size() : RSMAX;
-  MwConfig cfg = mw_config(ns_cfg);
+  int rkm = mw_dispatch(ns_cfg, [](auto i) { return decltype(i)::RKM; });
   // sharded: every shard contributes its own list; the resolver holds about the same number of candidates per
   // shape in total, so each shard gathers (and ships) fewer
-  if (h->world > 2) cfg.rkm = std::min(cfg.rkm, 64);          // (the resolver keeps what its shared memory holds: rke below)
-  const BufLayout L = make_layout(ns_cfg, cfg.rkm);
+  if (h->world > 2) rkm = std::min(rkm, 64);                  // (the resolver keeps what its shared memory holds: rke below)
+  const BufLayout L = make_layout(ns_cfg, rkm);
   TRY(rounds_ensure(h, P, L));
 
   TableSet tb; tb.st = h->d_st; tb.sc = h->d_sc; tb.al = h->d_al; tb.n_pad = (size_t)h->n_pad; tb.n_slots = (int)h->shapes.size();
@@ -238,19 +234,18 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
 
   // ---- resolver geometry
   const int D = h->world;
-  int rke = cfg.rkm;
-  auto env_int = [](const char *k, int dflt) { const char *v = getenv(k); return v ? atoi(v) : dflt; };
-  const int use_hpay = cfg.inst != 2 ? env_int("EGS_MW_HPAY", 2) : 0;   // prefetched candidate payload per shape (2: cp.async)
-  const size_t hp_bytes = use_hpay ? (size_t)ns_cfg * L.cand_bytes : 0;
-  const size_t pre_bytes = preinstall_used(cfg) ? sizeof(int) * (size_t)cfg.nt : 0;   // after the payloads: see MwArgs::pre_h
-  {
-    const size_t avail = MW_SMEM_MAX - cfg.smem_struct - hp_bytes - pre_bytes;
+  int rke = rkm, pre_h = 0, pre_cap = 0;
+  size_t smem = 0;
+  mw_dispatch(ns_cfg, [&](auto i) {
+    using I = decltype(i);
+    const size_t avail = MW_SMEM_MAX - mw_tail<I>(ns_cfg, D, 0, L.cand_bytes).end;   // all but the lists
     const size_t per = (size_t)ns_cfg * D * 8;
     if ((size_t)rke * per > avail) rke = (int)(avail / per) & ~1;   // even: what follows the lists stays 16-byte aligned
-    if (rke < 4) return fail(h, EGS_ERR_BAD_ARG, "rounds: shape set too large for the resolver's shared memory");
-  }
-  const int nw = std::max(1, std::min(ns_cfg, env_int("EGS_MW_WARPS", MW_MAX_WARPS)));
-  const size_t smem = cfg.smem_struct + (size_t)ns_cfg * D * rke * 8 + hp_bytes + pre_bytes;
+    smem = mw_tail<I>(ns_cfg, D, rke, L.cand_bytes).end;
+    preinstall_geometry<I>(ns_cfg, rke, pre_h, pre_cap);
+  });
+  if (rke < 4) return fail(h, EGS_ERR_BAD_ARG, "rounds: shape set too large for the resolver's shared memory");
+  const int nw = std::max(1, std::min(ns_cfg, MW_MAX_WARPS));
 
   SelectArgs sa; MergeArgs ma; MwArgs ra;
   sa.core = h->d_core; sa.mem = h->d_mem; sa.mem_total = h->d_mem_total;
@@ -261,8 +256,7 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
   ma.out = R.d_bufs + (size_t)h->rank * L.bytes; ma.L = L; ma.ctl = R.d_ctl;
   ra.core = h->d_core; ra.mem = h->d_mem; ra.lo = h->lo; ra.hi = h->hi; ra.policy = h->policy; ra.n_shards = D;
   ra.rd = R.d_rd; ra.tb = tb; ra.obs_pending = R.d_obs; ra.bufs = R.d_bufs; ra.L = L; ra.pod_sidx = R.d_pod_sidx;
-  ra.p0 = -1; ra.p_limit = 0; ra.out = out; ra.ctl = R.d_ctl; ra.rke = rke; ra.nw = nw; ra.use_hpay = use_hpay;
-  preinstall_geometry(cfg, ns_cfg, rke, ra.pre_h, ra.pre_cap);
+  ra.p0 = -1; ra.p_limit = 0; ra.out = out; ra.ctl = R.d_ctl; ra.rke = rke; ra.nw = nw; ra.pre_h = pre_h; ra.pre_cap = pre_cap;
 
   int ns_round = ns_cfg;                                        // grid of k_merge
   bool local_copied = false;
@@ -291,9 +285,7 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
     } else if (h->world > 1)
       NCK(h, nccl_api()->AllGather(R.d_bufs + (size_t)h->rank * L.bytes, R.d_bufs, (size_t)L.bytes, ncclChar, (ncclComm_t)R.comm, h->stream));
     if (h->timing) CK(h, cudaEventRecord(ev[2], h->stream));
-    if (cfg.inst == 0) k_resolve_mw<16, 512><<<1, 32 * nw, smem, h->stream>>>(ra);
-    else if (cfg.inst == 1) k_resolve_mw<32, 256><<<1, 32 * nw, smem, h->stream>>>(ra);
-    else k_resolve_mw<RSMAX, 128><<<1, 32 * nw, smem, h->stream>>>(ra);
+    mw_dispatch(ns_cfg, [&](auto i) { k_resolve_mw<decltype(i)><<<1, 32 * nw, smem, h->stream>>>(ra); });
     if (h->timing) CK(h, cudaEventRecord(ev[3], h->stream));
     h->k_launches[EGS_K_SELECT] += 1; h->k_launches[EGS_K_MERGE] += 1; h->k_launches[EGS_K_RESOLVE] += 1;
     return EGS_OK;

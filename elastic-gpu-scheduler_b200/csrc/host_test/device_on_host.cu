@@ -48,6 +48,18 @@ int egsdh_trade_leaves(const int32_t *core, const int32_t *mem, int mem_total, i
   *score = (int32_t)(best >> 20); *masks = bm;
   return 1;
 }
+// the resolver's one-GPU-per-lane single-container Trade (trade_lane_key), serially: max over the lanes gl = 0..7,
+// score and mask decoded from the winning key as the resolver does
+int egsdh_trade_lanes(const int32_t *core, const int32_t *mem, int rq_core, int rq_mem, int policy, int32_t *score,
+                      uint32_t *masks) {
+  int c[EGS_G], m[EGS_G];
+  rows(core, mem, c, m);
+  int bk = -1;
+  for (int gl = 0; gl < EGS_G; gl++) { const int k = trade_lane_key(c, m, gl, rq_core, rq_mem, policy); bk = k > bk ? k : bk; }
+  if (bk < 0) return 0;
+  *score = policy == EGS_BINPACK ? (bk >> 3) * 100 : 0; *masks = 1u << (bk & 7);
+  return 1;
+}
 int egsdh_transact(int32_t *core, int32_t *mem, int mem_total, int C, const egs_unit *units, uint32_t masks) {
   const Req r = make_req(C, units);
   return transact_row(core, mem, mem_total, r, masks) ? 1 : 0;

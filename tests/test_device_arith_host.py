@@ -1,5 +1,6 @@
 """The kernels' integer arithmetic -- csrc/egs_device.cuh: the Trade fast path (prefix/suffix maxima,
-unsigned-min PAD trick, packed q*8+g key), the general DFS Trade and Transact -- compiled for the host
+unsigned-min PAD trick, packed q*8+g key) and its one-GPU-per-lane form in the resolver, the general DFS Trade
+and Transact -- compiled for the host
 (csrc/host_test/device_on_host.cu) and checked against the oracle WITHOUT a GPU.  Same source the kernels
 inline; the device SASS is unaffected by the host build."""
 import ctypes as C
@@ -20,6 +21,7 @@ def DH():
     L.egsdh_trade.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     L.egsdh_trade_leaves.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     L.egsdh_transact.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint32]
+    L.egsdh_trade_lanes.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     L.egsdh_is_single.argtypes = [C.c_int, C.c_void_p]
     for f in ("egsdh_cand_key", "egsdh_fit_term", "egsdh_score_term"):
         getattr(L, f).restype = C.c_uint64
@@ -54,6 +56,16 @@ def _trade(DH, rows, mt, req, policy, path):
     return alloc, sc.value
 
 
+def _trade_lanes(DH, rows, req, policy):
+    """trade_lane_key, the one-GPU-per-lane Trade of the resolver's single-container pods, maxed over the lanes."""
+    core, mem = _pad(rows)
+    (rq_core, rq_mem, _), = req
+    sc, mk = C.c_int32(0), C.c_uint32(0)
+    if not DH.egsdh_trade_lanes(core.ctypes.data, mem.ctypes.data, rq_core, rq_mem, policy, C.byref(sc), C.byref(mk)):
+        return None
+    return [[g for g in range(8) if (mk.value >> g) & 1]], sc.value
+
+
 unit = st.one_of(
     st.tuples(st.integers(0, 100), st.integers(0, 40), st.just(0)).filter(lambda u: u[0] or u[1]),
     st.tuples(st.just(0), st.just(0), st.integers(1, 3)),
@@ -70,6 +82,8 @@ def test_kernel_trade_equals_oracle(DH, rows, req, policy, mt):
     want = None if opt is None else (opt.allocated, opt.score)
     assert _trade(DH, rows, mt, req, policy, 0) == want          # the dispatch the kernels use
     assert _trade(DH, rows, mt, req, policy, 1) == want          # general DFS on every request
+    if DH.egsdh_is_single(len(req), _units(req).ctypes.data):
+        assert _trade_lanes(DH, rows, req, policy) == want       # the resolver's per-lane form
 
 
 @settings(max_examples=800, deadline=None)
@@ -105,6 +119,7 @@ def test_fast_path_single_container_large_values(DH, rows, core, mem, policy):
     u = _units(req)
     assert DH.egsdh_is_single(1, u.ctypes.data) == 1
     assert _trade(DH, rows, mt, req, policy, 0) == want
+    assert _trade_lanes(DH, rows, req, policy) == want
 
 
 @settings(max_examples=400, deadline=None)

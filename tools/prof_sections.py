@@ -18,6 +18,6 @@ print(f"pods: fast {v[6]} (head-wins {v[11]}), general {v[9]}; slots pre-install
 print(f"  per-pod cycles (summed over owner warps / pods): prepare {v[0]/(fast+gen):.0f}  wait {v[1]/(fast+gen):.0f}  post {v[3]/fast:.0f}")
 print(f"  ticket: fast tracked-win {v[2]/max(fast-hw,1):.0f}  fast head-win {v[5]/hw:.0f}  general {v[4]/gen:.0f}")
 tw = max(fast - hw, 1)
-print(f"  tracked-win ticket split: rows+Trade {v[7]/tw:.0f}  winner {v[8]/tw:.0f}  transact reads {v[10]/tw:.0f}  stores+arrive {v[12]/tw:.0f}")
+print(f"  tracked-win ticket split: rows+Trade {v[7]/tw:.0f}  winner {v[8]/tw:.0f}  transact {v[10]/tw:.0f}  stores+arrive {v[12]/tw:.0f}")
 print(f"  pending Trade redone inside the ticket (rows changed since the preparation): {v[14]} of {fast} fast pods")
 print(f"  total ticket Mcyc {(v[2]+v[5]+v[4])/1e6:.1f} = {(v[2]+v[5]+v[4])/1.965e6:.1f} ms at 1.965 GHz")
