@@ -372,6 +372,9 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
       if (R.h_ctl->error || R.h_ctl->next_p <= p0) { rc = fail(h, EGS_ERR_CUDA, "rounds: resolver made no progress"); break; }
       R.rounds += 1; R.pods += R.h_ctl->next_p - p0; R.tracked += R.h_ctl->tracked;
       for (int i = 0; i < 4; i++) R.stops[i] += R.h_ctl->stops[i];
+      // the resolver counts a round that reached p_end as "pod limit"; when pod plim < P is the first pod of a
+      // shape outside this round's set, the round ended at its set boundary (egs.h: "shape outside the round set")
+      if (R.h_ctl->next_p == plim && plim < P) { R.stops[0] -= 1; R.stops[1] += 1; }
       p0 = R.h_ctl->next_p;
       resolved = p0;
     }
