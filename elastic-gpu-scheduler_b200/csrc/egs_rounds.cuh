@@ -779,8 +779,9 @@ __device__ __noinline__ int general_pod(SM &S, const MwArgs &a, const unsigned l
       ok = __shfl_sync(0xffffffffu, ok, 0);
     }
     // Rows changed.  (a) not-yet-observed NEW options of this node are void (only while some shape of the
-    // round is unobserved); (b) UNFIT memos are void -- unless every request of the round is >= 0: rows
-    // then only decrease and an option that did not fit can never fit (exact shortcut).
+    // round is unobserved); (b) UNFIT memos are void -- unless the round is monotone (every container
+    // fractional, every request >= 0; resolve_prologue): rows then only decrease and a fractional option
+    // that did not fit can never fit (exact shortcut).
     if (!mono || S.n_observed < ns) {
       for (int s2 = lane; s2 < ns; s2 += 32) {
         if (s2 == s) continue;
@@ -915,8 +916,13 @@ __device__ __noinline__ bool resolve_prologue(typename I::Smem &S, const MwArgs 
     for (int i = tid; i < NS * RD; i += nthreads) (&S.cur[0][0])[i] = 0;   // the owners' list cursors start at the top
   }
   if (tid == 0) {
-    bool mono = true;                                            // all requests >= 0: rows only decrease in this round
-    for (int s = 0; s < ns; s++) for (int c = 0; c < S.reqs[s].C; c++) mono &= S.reqs[s].core[c] >= 0 && S.reqs[s].mem[c] >= 0;
+    // Monotone round: every container fractional with requests >= 0.  Rows then only decrease, and fractional
+    // feasibility (avail >= request) is monotone in the rows.  A whole-GPU container tests EQUALITY with the totals
+    // (gpu.go:193-202): a GPU above its totals (a sidecar's +1, ForgetPod after a failed AddPod, a loaded row) is
+    // not free, and a bind that brings it down to its totals frees it -- so a round with one is never monotone.
+    bool mono = true;
+    for (int s = 0; s < ns; s++)
+      for (int c = 0; c < S.reqs[s].C; c++) mono &= S.reqs[s].core[c] >= 0 && S.reqs[s].mem[c] >= 0 && S.reqs[s].cnt[c] == 0;
     S.mono = mono ? 1 : 0;
   }
   __syncthreads();

@@ -27,6 +27,14 @@ def score_term(node: int, score: int) -> int:
     return po.score_digest_term(node, score)
 
 
+def monotone(shapes) -> bool:
+    """The round's UNFIT memos survive its binds: every container fractional with requests >= 0.  Rows then only
+    decrease and fractional feasibility (avail >= request) is monotone in them.  Whole-GPU feasibility tests equality
+    with the totals, so a GPU above them (sidecar +1, ForgetPod after a failed AddPod, a loaded row) turns free when a
+    bind brings it down: a round with a whole-GPU container is never monotone."""
+    return all(u[0] >= 0 and u[1] >= 0 and u[2] == 0 for s in shapes for u in s)
+
+
 class Entry:
     __slots__ = ("st", "score", "alloc")
 
@@ -87,7 +95,7 @@ class RoundsModel:
                 plim += 1
             for s in shapes:
                 self._table(s)
-            mono = all(u[0] >= 0 and u[1] >= 0 for s in shapes for u in s)
+            mono = monotone(shapes)
             # ---- k_select per shard: evaluate ABSENT, convert NEW when observed since, aggregates, top-K
             lists = {s: [] for s in shapes}                      # per shape: per shard (keys, more)
             agg = {}

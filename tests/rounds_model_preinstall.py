@@ -13,7 +13,7 @@ from __future__ import annotations
 from typing import Dict, List, Optional, Sequence
 
 import egs_oracle as po
-from rounds_model import ABSENT, CACHED, MASK64, NEW, UNFIT, RoundsModel, fit_term, score_term
+from rounds_model import ABSENT, CACHED, MASK64, NEW, UNFIT, RoundsModel, fit_term, monotone, score_term
 
 
 class PreinstallRoundsModel(RoundsModel):
@@ -41,7 +41,7 @@ class PreinstallRoundsModel(RoundsModel):
                 plim += 1
             for s in shapes:
                 self._table(s)
-            mono = all(u[0] >= 0 and u[1] >= 0 for s in shapes for u in s)
+            mono = monotone(shapes)
             # ---- k_select per shard: evaluate ABSENT, convert NEW when observed since, aggregates, top-K
             lists = {s: [] for s in shapes}                      # per shape: per shard (keys, more)
             agg = {}

@@ -144,6 +144,100 @@ def test_kernel_transact_equals_oracle(DH, rows, req, mt, stale):
     assert [(int(core[i]), int(mem[i])) for i in range(len(g))] == [(x.core_avail, x.mem_avail) for x in g]
 
 
+def _trade_leaves(DH, rows, mt, req, policy):
+    core, mem = _pad(rows)
+    u = _units(req)
+    sc, mk = C.c_int32(0), C.c_uint32(0)
+    if not DH.egsdh_trade_leaves(core.ctypes.data, mem.ctypes.data, mt, len(req), u.ctypes.data, policy, C.byref(sc), C.byref(mk)):
+        return None
+    return [[g for g in range(8) if (mk.value >> (8 * c + g)) & 1] for c in range(len(req))], sc.value
+
+
+def _every_trade_equals_oracle(DH, rows, mt, req, policy):
+    """The kernels' dispatch, the general DFS, the leaf-parallel Trade and (single-container shapes) the per-lane
+    form all return the oracle's option.  Returns it."""
+    g = [po.GPU(c, m, 100, mt) for c, m in rows]
+    opt = po.trade(g, po.RATERS[policy], list(req))
+    want = None if opt is None else (opt.allocated, opt.score)
+    assert _trade(DH, rows, mt, req, policy, 0) == want
+    assert _trade(DH, rows, mt, req, policy, 1) == want
+    assert _trade_leaves(DH, rows, mt, req, policy) == want
+    if DH.egsdh_is_single(len(req), _units(req).ctypes.data):
+        assert _trade_lanes(DH, rows, req, policy) == want
+    return want
+
+
+# ---- the int32 guard (DESIGN §1): free core <= 2^20 and free memory <= 2^25 per GPU, requests within the same
+# bounds.  The score comes closest to 2^31 with k = 0 (no container holds exactly one GPU: whole-GPU containers of
+# count >= 2 only): Range/1*100 with Range up to (2^25 + 2^20) / 2, about 1.73e9.
+MAX_CORE, MAX_MEM = 1 << 20, 1 << 25
+
+
+@st.composite
+def guard_rows(draw):
+    """(mem_total, rows): GPUs free at their totals (whole-GPU containers can take them), just above them, or
+    anywhere up to the guard."""
+    mt = draw(st.sampled_from([1, 81920, MAX_MEM - 1, MAX_MEM]))
+    gpu = st.one_of(
+        st.just((100, mt)),
+        st.tuples(st.integers(100, 103), st.integers(mt, mt + 3)).map(lambda r: (r[0], min(r[1], MAX_MEM))),
+        st.tuples(st.one_of(st.integers(0, MAX_CORE), st.sampled_from([0, MAX_CORE - 1, MAX_CORE])),
+                  st.one_of(st.integers(0, MAX_MEM), st.sampled_from([0, MAX_MEM - 1, MAX_MEM]))),
+    )
+    return mt, draw(st.lists(gpu, min_size=1, max_size=8))
+
+
+guard_unit = st.one_of(
+    st.tuples(st.one_of(st.integers(0, MAX_CORE), st.sampled_from([0, 1, 100, MAX_CORE])),
+              st.one_of(st.integers(0, MAX_MEM), st.sampled_from([0, 1, MAX_MEM])), st.just(0)).filter(lambda u: u[0] or u[1]),
+    st.tuples(st.just(0), st.just(0), st.integers(1, 3)),
+    st.just((-1, -1, 0)),
+)
+k0_req = st.lists(st.tuples(st.just(0), st.just(0), st.integers(2, 4)), min_size=1, max_size=2)
+
+
+@settings(max_examples=800, deadline=None)
+@given(mrows=guard_rows(), req=st.one_of(st.lists(guard_unit, min_size=1, max_size=4), k0_req), policy=st.integers(0, 1))
+def test_every_trade_at_the_int32_guard(DH, mrows, req, policy):
+    """Rows and requests up to the guard, whole-GPU containers on GPUs at, above and far from their totals, k = 0
+    shapes: every Trade the kernels run equals the oracle's (which computes in int64)."""
+    mt, rows = mrows
+    _every_trade_equals_oracle(DH, rows, mt, req, policy)
+
+
+@pytest.mark.parametrize("policy", [0, 1])
+def test_k0_score_near_the_int32_limit(DH, policy):
+    """The largest score the guard admits: the free GPUs taken by whole-GPU containers of count 2, the last GPU at
+    (2^20, 2^25)."""
+    for req in ([(0, 0, 2)], [(0, 0, 2), (0, 0, 2)]):
+        n = 2 * len(req)
+        rows = [(100, MAX_MEM)] * n + [(MAX_CORE, MAX_MEM)]
+        alloc, score = _every_trade_equals_oracle(DH, rows, MAX_MEM, req, policy)
+        assert sorted(sum(alloc, [])) == list(range(n))
+        assert score == (0 if policy else (MAX_MEM + MAX_CORE) // 2 * 100) and score < 2**31
+
+
+@settings(max_examples=600, deadline=None)
+@given(rows=st.lists(st.tuples(st.integers(97, 103), st.integers(13, 19)), min_size=1, max_size=8),
+       req=st.lists(st.one_of(st.tuples(st.integers(0, 3), st.integers(0, 3), st.just(0)).filter(lambda u: u[0] or u[1]),
+                              st.tuples(st.just(0), st.just(0), st.integers(1, 3)), st.just((-1, -1, 0))),
+                    min_size=1, max_size=4),
+       policy=st.integers(0, 1))
+def test_whole_gpu_trade_above_totals(DH, rows, req, policy):
+    """GPUs of 16 MiB around their totals (97..103 core, 13..19 MiB): only a GPU at exactly (100, 16) is free for a
+    whole-GPU container, also after the shape's own fractional and sidecar containers moved it there; Transact of the
+    resulting option agrees too."""
+    want = _every_trade_equals_oracle(DH, rows, 16, req, policy)
+    if want is None:
+        return
+    g = [po.GPU(c, m, 100, 16) for c, m in rows]
+    ok = po.transact(g, po.GPUOption(request=list(req), allocated=want[0], score=want[1]))
+    core, mem = _pad(rows)
+    masks = sum(1 << (8 * c + gi) for c, a in enumerate(want[0]) for gi in a)
+    assert bool(DH.egsdh_transact(core.ctypes.data, mem.ctypes.data, 16, len(req), _units(req).ctypes.data, masks)) == ok
+    assert [(int(core[i]), int(mem[i])) for i in range(len(g))] == [(x.core_avail, x.mem_avail) for x in g]
+
+
 def test_keys_and_digest_terms(DH):
     for node, score in [(0, 0), (5, 600), (99999, 2050500), (2**31 - 1, 0)]:
         assert DH.egsdh_fit_term(node) == po.fit_digest_term(node)

@@ -9,7 +9,7 @@ import pytest
 import egs_oracle as po
 from rounds_model import RoundsModel
 from rounds_model_preinstall import PreinstallRoundsModel
-from test_rounds_model import _cluster, _fast_regime, _shapes
+from test_rounds_model import MINIMAL, _cluster, _fast_regime, _shapes, load_over_totals, over_totals_scenario, replay
 
 PRE_H = (0, 1, 64)                                                # off, the top of every list, every list entry
 
@@ -94,6 +94,31 @@ def test_stops_fire_with_preinstalled_slots(pre_h):
         for k in tot:
             tot[k] += m.stats[k]
     assert all(v > 0 for v in tot.values()), tot
+
+
+@pytest.mark.parametrize("pre_h", PRE_H)
+@pytest.mark.parametrize("policy", [0, 1])
+def test_preinstall_whole_gpu_fits_again_after_bind_above_totals(policy, pre_h):
+    """test_rounds_model's minimal case with the node pre-installed: a GPU at (101, 17) of (100, 16) is not free for
+    the first whole-GPU pod, is after a (1, 1) bind, and the second whole-GPU pod takes it."""
+    o, m = po.Scheduler(policy), PreinstallRoundsModel(policy, pre_h=pre_h)
+    assert o.add_node(100, 16) == m.add_node(100, 16) == 0
+    assert replay(m, o, MINIMAL, ("minimal", policy, pre_h)) == 1
+    assert o.rows(0) == [(0, 0)]
+
+
+@pytest.mark.parametrize("cap", ["full", "half"])
+@pytest.mark.parametrize("pre_h", PRE_H)
+@pytest.mark.parametrize("seed", range(16))
+def test_preinstall_over_totals_equals_oracle(seed, pre_h, cap):
+    """GPUs at or just above their totals, whole-GPU and small fractional shapes only (every round's requests >= 0),
+    three batches on one state: outputs, rows, caches and UNFIT memos equal the oracle's."""
+    policy, K, T, RS, D, nodes, batches = over_totals_scenario(seed)
+    o = po.Scheduler(policy)
+    m = PreinstallRoundsModel(policy, K=K, T=T, RS=RS, shards=D, pre_h=pre_h, pre_cap=_cap(T, cap))
+    load_over_totals(m, o, nodes)
+    replay(m, o, batches, (seed, pre_h, cap, K, T, RS, D))
+    assert (m.stats["pre"] > 0) == (pre_h > 0)
 
 
 @pytest.mark.parametrize("seed", range(24))
