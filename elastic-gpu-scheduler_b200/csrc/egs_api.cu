@@ -1128,10 +1128,10 @@ extern "C" int egs_rounds_stats(egs_handle *h, int64_t out[8]) {
 }
 
 // debug: cycle counters of k_resolve sections (only filled when built with -DEGS_RESOLVE_PROF)
-extern "C" int egs_debug_resolve_prof(egs_handle *h, long long out[16]) {
+extern "C" int egs_debug_resolve_prof(egs_handle *h, long long out[RPROF]) {
   if (!h || !out) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  memcpy(out, h->rounds.prof, sizeof(long long) * 16);
+  memcpy(out, h->rounds.prof, sizeof(long long) * RPROF);
   return EGS_OK;
 }
 

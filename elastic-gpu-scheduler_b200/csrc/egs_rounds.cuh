@@ -44,6 +44,7 @@
 #define SEL_THREADS 128
 #define SEL_WARPS (SEL_THREADS / 32)
 #define MW_MAX_WARPS 16
+#define RPROF 32     // resolver cycle counters (-DEGS_RESOLVE_PROF; tools/prof_sections.py names them)
 
 struct RoundDesc {                  // device resident: the round's shape set
   int ns; int pad[3];
@@ -55,7 +56,7 @@ struct RoundCtl {                   // device resident: progress of the batch, w
   int next_p, p_end, error, rounds;
   long long pods, tracked;
   long long stops[4];               // pod limit, shape outside the set, tracked table full, list dry
-  long long prof[16];
+  long long prof[RPROF];
 };
 
 // One shard's candidate buffer (dynamic layout: shape capacity nsc, list depth rkm):
@@ -385,9 +386,11 @@ __global__ void __launch_bounds__(256) k_merge(MergeArgs a) {
 #ifdef EGS_RESOLVE_PROF
 #define PROF_T(i) { long long now_ = clock64(); prof[i] += now_ - tprev; tprev = now_; }
 #define PROF_C(i, v) { prof[i] += (v); }
+#define PROF_RELEASE() { *reinterpret_cast<volatile long long *>(&S.t_release) = clock64(); }   // lane 0, before the arrive
 #else
 #define PROF_T(i)
 #define PROF_C(i, v)
+#define PROF_RELEASE()
 #endif
 
 // max of a 64-bit key over the warp: two redux.sync steps on the halves; owner = lowest lane holding it
@@ -443,6 +446,9 @@ struct MwSmem {
   unsigned long long mbar[MW_MAX_WARPS];   // one per owner warp: "the ticket is yours"
   int turn;                                // the pod whose ticket is open; MW_STOP | p once the round was stopped before pod p
   int stop, stop_reason, stop_p, nT, n_observed, mono, p0, p_end;
+#ifdef EGS_RESOLVE_PROF
+  long long t_release;                     // clock64 at which the last ticket was handed on
+#endif
 };
 #define MW_STOP 0x40000000
 
@@ -544,6 +550,11 @@ __device__ __forceinline__ void maintain_heads(SM &S, const unsigned long long *
     if (c >= len) { k = 0; if (S.more[s][d] != 0 && len > 0) db = l[len - 1]; }
     S.cur[s][d] = (uint8_t)c;
     S.hkey[s][d] = k;
+  }
+  if (D == 1) {                                                  // one list (unsharded): lane 0 holds the maxima already
+    if (lane == 0) { S.bh[s] = k; S.bh_d[s] = 0; S.dbound[s] = db; S.hv_nT[s] = nT; }
+    __syncwarp();
+    return;
   }
   int owner, o2;
   const unsigned long long b = warp_max_key_fwd(k, owner);
@@ -989,11 +1000,16 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
   unsigned long long *lk = reinterpret_cast<unsigned long long *>(smem_raw + tail.lk);
   char *hpay = I::kHpay ? reinterpret_cast<char *>(smem_raw + tail.hpay) : nullptr;
   int *psrc = reinterpret_cast<int *>(smem_raw + tail.psrc);
+  // what the owner loop reads of `a`, in registers: `a` is passed by reference to the non-inlined helpers, so its
+  // fields otherwise live in a stack copy and every use is a local-memory load on the ordered chain
+  const int policy = a.policy;
+  const uint8_t *const pod_sidx = a.pod_sidx;
   int n_pre;
   if (!resolve_prologue<I>(S, a, lk, psrc, n_pre)) return;
   const int p0 = S.p0, p_end = S.p_end;
 #ifdef EGS_RESOLVE_PROF
-  long long prof[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}; long long tprev = clock64();
+  long long prof[RPROF]; for (int i = 0; i < RPROF; i++) prof[i] = 0;
+  long long tprev = clock64();
 #endif
   // ---- the owner loop.  Pods of shapes si with si % nw == warp, in pod order.
   if (warp < nw) {
@@ -1006,11 +1022,11 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
     auto load_chunk = [&](int base) {
       const int q = base + 4 * lane;
       uint32_t wd = 0xFFFFFFFFu;
-      if (q < p_end) wd = *reinterpret_cast<const uint32_t *>(a.pod_sidx + q);   // padded allocation: reads up to 3 past the end
+      if (q < p_end) wd = *reinterpret_cast<const uint32_t *>(pod_sidx + q);   // padded allocation: reads up to 3 past the end
       myword = wd;
       uint32_t nx = 0xFFFFFFFFu, pv = 0xFFFFFFFFu;
-      if (lane == 0 && base + 128 < p_end) nx = *reinterpret_cast<const uint32_t *>(a.pod_sidx + base + 128);
-      if (lane == 0 && base >= 4) pv = *reinterpret_cast<const uint32_t *>(a.pod_sidx + base - 4);
+      if (lane == 0 && base + 128 < p_end) nx = *reinterpret_cast<const uint32_t *>(pod_sidx + base + 128);
+      if (lane == 0 && base >= 4) pv = *reinterpret_cast<const uint32_t *>(pod_sidx + base - 4);
       nextword = __shfl_sync(0xffffffffu, nx, 0); prevword = __shfl_sync(0xffffffffu, pv, 0);
 #pragma unroll
       for (int j = 0; j < 4; j++) {
@@ -1038,7 +1054,8 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
         for (int j = 0; j < 4; j++) if (pm[j]) { const int i = 4 * (__ffs(pm[j]) - 1) + j; best_i = min(best_i, i); }
         if (best_i < (1 << 30)) {
           const int j = best_i & 3, l = best_i >> 2;
-          pm[j] &= ~(1u << l);
+#pragma unroll
+          for (int jj = 0; jj < 4; jj++) if (jj == j) pm[jj] &= ~(1u << l);   // static indices: pm stays in registers
           p = cb + best_i;
           s = (__shfl_sync(0xffffffffu, myword, l) >> (8 * j)) & 0xFF;
           // whom do I wake after my ticket (the owner of p + 1 unless that is me), and do I sleep before mine?
@@ -1052,8 +1069,10 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
         load_chunk(cb);
       }
       if (p < 0) break;
+      PROF_T(22)
       // ======== preparation outside the ticket: only owner-private data and data that never changes
       maintain_heads(S, lk, D, rke, s, lane, false);
+      PROF_T(23)
       const unsigned long long head = S.bh[s];
       if constexpr (I::kHpay) {
         if (head != 0 && S.hpay_node[s] != (int)key_node(head)) {         // payload of the best head -> shared memory,
@@ -1069,6 +1088,7 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
           __syncwarp();
         }
       }
+      PROF_T(24)
       // n_observed BEFORE pu: other warps write pu[s] / the aggregates of s (general_pod, inside their tickets) only while
       // some shape of the round is unobserved; once n_observed == ns was seen, everything read below is owner-private
       const int n_obs = ld_vol(&S.n_observed);
@@ -1097,11 +1117,14 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
           int c[EGS_G], m[EGS_G];
 #pragma unroll
           for (int g = 0; g < EGS_G; g++) { c[g] = ld_vol(&S.rc[uu][g]); m[g] = ld_vol(&S.rm[uu][g]); }
-          bk_pre = trade_lanes(c, m, gl, rq_c, rq_m, a.policy);
+          bk_pre = trade_lanes(c, m, gl, rq_c, rq_m, policy);
           if ((v_pre & 1) || ld_vol(&S.ver[uu]) != v_pre) v_pre = -1;   // a bind was writing the rows meanwhile
         }
       }
       PROF_T(0)
+#ifdef EGS_RESOLVE_PROF
+      const bool late_ = sleep_first && ld_vol(&S.turn) == p;     // the ticket was already open: it waited for my preparation
+#endif
       // ======== the ticket
       bool stopped = false;
       if (sleep_first) {                                          // else: I still hold the ticket
@@ -1111,6 +1134,14 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
       }
       if (stopped) break;
       PROF_T(1)
+#ifdef EGS_RESOLVE_PROF
+      if (p > p0) {                                               // release of pod p-1 -> start of pod p, on the chain
+        const long long gap_ = tprev - *reinterpret_cast<volatile long long *>(&S.t_release);
+        if (!sleep_first) { prof[18] += gap_; prof[19] += 1; }    // kept the ticket: my own post + preparation
+        else if (late_) { prof[20] += gap_; prof[21] += 1; }      // handed over to an owner that was not ready
+        else { prof[16] += gap_; prof[17] += 1; }                 // handed over to an owner asleep on its mbarrier
+      }
+#endif
       int reason = 0;
       if (fast) {
         // ---- fast pod: single-container shape, monotone round, every shape observed, at most one pending option
@@ -1122,13 +1153,13 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
           const int4 m0 = *reinterpret_cast<const int4 *>(&S.rm[uu][0]), m1 = *reinterpret_cast<const int4 *>(&S.rm[uu][4]);
           const int c[EGS_G] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
           const int m[EGS_G] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
-          bk = trade_lanes(c, m, gl, rq_c, rq_m, a.policy);
+          bk = trade_lanes(c, m, gl, rq_c, rq_m, policy);
           PROF_C(14, 1)
         }
 #ifdef EGS_RESOLVE_PROF
         long long q1_ = clock64() + (bk & 0);
 #endif
-        const int sc = (bk >= 0 && a.policy == EGS_BINPACK) ? (bk >> 3) * 100 : 0;
+        const int sc = (bk >= 0 && policy == EGS_BINPACK) ? (bk >> 3) * 100 : 0;
         const unsigned long long tradekey = bk >= 0 ? cand_key(sc, und) : 0ull;
         unsigned long long best = pre_best; int tw = pre_t; uint32_t masks = pre_al;
         if (xb > best) { best = xb; tw = xt; masks = 0; }
@@ -1187,6 +1218,7 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
             if (from_head) { __threadfence_block(); st_vol(&S.nT, nT + 1); }
             if (xb != 0) { S.xbest[s] = 0; S.xbest_t[s] = -1; }
             st_vol(&S.turn, p + 1);
+            PROF_RELEASE()
             if (wake >= 0) mbar_arrive(&S.mbar[wake]);
           }
 #ifdef EGS_RESOLVE_PROF
@@ -1223,7 +1255,7 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
         break;
       }
       __syncwarp();
-      if (lane == 0) { st_vol(&S.turn, p + 1); if (wake >= 0) mbar_arrive(&S.mbar[wake]); }
+      if (lane == 0) { st_vol(&S.turn, p + 1); PROF_RELEASE() if (wake >= 0) mbar_arrive(&S.mbar[wake]); }
       PROF_T(4)
     }
   }
@@ -1231,7 +1263,7 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
   resolve_epilogue(S, a);
 #ifdef EGS_RESOLVE_PROF
   if (warp == 0) prof[13] += n_pre;                             // pre-installed slots
-  if (lane == 0 && warp < nw) for (int i = 0; i < 16; i++) atomicAdd((unsigned long long *)&a.ctl->prof[i], (unsigned long long)prof[i]);
+  if (lane == 0 && warp < nw) for (int i = 0; i < RPROF; i++) atomicAdd((unsigned long long *)&a.ctl->prof[i], (unsigned long long)prof[i]);
 #endif
 }
 
@@ -1282,7 +1314,7 @@ struct RoundsState {
   RoundDesc *d_rd = nullptr; RoundDesc *h_rd = nullptr;
   RoundCtl *d_ctl = nullptr; RoundCtl *h_ctl = nullptr;
   int64_t rounds = 0, pods = 0, tracked = 0; int64_t stops[4] = {0, 0, 0, 0};
-  long long prof[16] = {0};
+  long long prof[RPROF] = {0};
 };
 
 static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_unit *units,

@@ -383,7 +383,7 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
     R.rounds += R.h_ctl->rounds; R.pods += R.h_ctl->pods; R.tracked += R.h_ctl->tracked;
     for (int i = 0; i < 4; i++) R.stops[i] += R.h_ctl->stops[i];
   }
-  if (R.h_ctl) for (int i = 0; i < 16; i++) R.prof[i] += R.h_ctl->prof[i];
+  if (R.h_ctl) for (int i = 0; i < RPROF; i++) R.prof[i] += R.h_ctl->prof[i];
   if (h->timing) for (auto &e : ev) cudaEventDestroy(e);
   *n_done = std::min(resolved, P);
   // no OPT_NEW may outlive the batch -- also after an error, so that the handle stays consistent
