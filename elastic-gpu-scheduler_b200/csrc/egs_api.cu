@@ -191,18 +191,6 @@ static int intern_slow(egs_handle *h, int C, const egs_unit *u, int *slot) {
   return EGS_OK;
 }
 
-static ReqW make_req_w(int C, const egs_unit *u) {
-  ReqW r; memset(&r, 0, sizeof r);
-  r.C = C;
-  for (int i = 0; i < C; i++) { r.core[i] = u[i].core; r.mem[i] = u[i].mem; r.cnt[i] = u[i].count; }
-  return r;
-}
-static Req make_req(int C, const egs_unit *u) {
-  Req r; memset(&r, 0, sizeof r);
-  r.C = C;
-  for (int i = 0; i < C; i++) { r.core[i] = u[i].core; r.mem[i] = u[i].mem; r.cnt[i] = u[i].count; }
-  return r;
-}
 static bool is_single(int C, const egs_unit *u) { return C == 1 && u[0].count == 0 && u[0].core >= 0 && u[0].mem >= 0; }
 
 static const AutoBatch *auto_find(const egs_handle *h, uint64_t uid) {
@@ -670,21 +658,48 @@ extern "C" int egs_option_dump(egs_handle *h, int n_containers, const egs_unit *
 static int apply_lists(egs_handle *h, int cancel, int node_id, int C, const egs_unit *units,
                        const int32_t *alloc_off, const int32_t *alloc_idx) {
   ApplyArgs a; memset(&a, 0, sizeof a);
-  a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total; a.node = node_id;
-  a.req = make_req_w(C, units); a.cancel = cancel;
+  a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total;
+  a.op.node = node_id; a.op.cancel = cancel; a.op.req = make_req<ReqW>(C, units);
   a.all_st = h->d_st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
   for (int c = 0; c < C; c++) {
     int n = alloc_off ? alloc_off[c + 1] - alloc_off[c] : 0;
     if (n < 0 || n > EGS_G || (n > 0 && !alloc_idx)) return EGS_ERR_BAD_ARG;
-    a.n_idx[c] = n;
+    a.op.n_idx[c] = n;
     for (int j = 0; j < n; j++) {
       int v = alloc_idx[alloc_off[c] + j];
       if (v < 0 || v >= h->h_gpu_count[node_id]) return EGS_ERR_BAD_ARG;   // the reference would panic
-      a.idx[c][j] = (int8_t)v;
+      a.op.idx[c][j] = (int8_t)v;
     }
   }
   k_apply<<<1, 1, 0, h->stream>>>(a);
   CK(h, cudaGetLastError());
+  return EGS_OK;
+}
+
+// The podsMap / podMaps decision of one EGS_MUT_* record on `node`, in the reference's order.  apply(cancel) makes
+// the row update the reference would make, before the bookkeeping that follows it; a failing apply ends the record.
+// The single verbs validate a pod's index lists inside apply, i.e. only when the record reaches a row update, which
+// is when the reference parses the annotations: a known uid with a malformed list is EGS_OK there.  The mutation
+// stream validates every record's lists before it applies any, so the same record fails the whole stream.
+template <class F>
+static int account(egs_handle *h, int kind, int node, uint64_t uid, F &&apply) {
+  if (kind == EGS_MUT_FORGET) {                                             // ForgetPod scheduler.go:247-267
+    if (node >= 0 && in_pods_map(h, node, uid)) {                           // node.go:131
+      TRY(apply(1));
+      if (!h->pods_map.erase(NodeUid{node, uid})) h->auto_gone_node.insert(NodeUid{node, uid});
+    }
+    if (in_pod_maps(h, uid)) {                                              // scheduler.go:261-264
+      if (!h->pod_maps.erase(uid)) h->auto_gone_pod.insert(uid);
+      h->released.insert(uid);
+    }
+    return EGS_OK;
+  }
+  if (kind == EGS_MUT_ADD && in_pod_maps(h, uid)) return EGS_OK;           // scheduler.go:239-241
+  if (!in_pods_map(h, node, uid)) {                                         // node.go:149
+    TRY(apply(0));
+    h->pods_map.insert(NodeUid{node, uid});
+  }
+  if (kind == EGS_MUT_ADD) h->pod_maps.insert(uid);                         // scheduler.go:243
   return EGS_OK;
 }
 
@@ -697,13 +712,8 @@ extern "C" int egs_pod_apply(egs_handle *h, int node_id, int n_containers, const
   if (h->h_gpu_count[node_id] == 0) return EGS_ERR_NO_NODE;
   TRY(check_units(n_containers, units, EGS_MAX_CONTAINERS_APPLY));
   TRY(flush_pending(h));
-  if (in_pod_maps(h, uid)) return EGS_OK;                                   // scheduler.go:239-241
-  if (!in_pods_map(h, node_id, uid)) {                                      // node.go:149
-    TRY(apply_lists(h, 0, node_id, n_containers, units, alloc_off, alloc_idx));
-    h->pods_map.insert(NodeUid{node_id, uid});
-  }
-  h->pod_maps.insert(uid);                                                  // scheduler.go:243
-  return EGS_OK;
+  return account(h, EGS_MUT_ADD, node_id, uid,
+                 [&](int cancel) { return apply_lists(h, cancel, node_id, n_containers, units, alloc_off, alloc_idx); });
 }
 
 // NodeAllocator.Add(pod, nil) node.go:148-160 (replay at node load, node.go:52-54)
@@ -715,11 +725,8 @@ extern "C" int egs_node_replay_pod(egs_handle *h, int node_id, int n_containers,
   if (h->h_gpu_count[node_id] == 0) return EGS_ERR_NO_NODE;
   TRY(check_units(n_containers, units, EGS_MAX_CONTAINERS_APPLY));
   TRY(flush_pending(h));
-  if (!in_pods_map(h, node_id, uid)) {
-    TRY(apply_lists(h, 0, node_id, n_containers, units, alloc_off, alloc_idx));
-    h->pods_map.insert(NodeUid{node_id, uid});
-  }
-  return EGS_OK;
+  return account(h, EGS_MUT_REPLAY, node_id, uid,
+                 [&](int cancel) { return apply_lists(h, cancel, node_id, n_containers, units, alloc_off, alloc_idx); });
 }
 
 // ForgetPod scheduler.go:247-267
@@ -732,16 +739,9 @@ extern "C" int egs_pod_cancel(egs_handle *h, int node_id, int n_containers, cons
     if (node_id >= h->max_nodes) return EGS_ERR_BAD_ARG;
     if (h->h_gpu_count[node_id] == 0) return EGS_ERR_NO_NODE;
     TRY(check_units(n_containers, units, EGS_MAX_CONTAINERS_APPLY));
-    if (in_pods_map(h, node_id, uid)) {                                     // node.go:131
-      TRY(apply_lists(h, 1, node_id, n_containers, units, alloc_off, alloc_idx));
-      if (!h->pods_map.erase(NodeUid{node_id, uid})) h->auto_gone_node.insert(NodeUid{node_id, uid});
-    }
   }
-  if (in_pod_maps(h, uid)) {                                                // scheduler.go:261-264
-    if (!h->pod_maps.erase(uid)) h->auto_gone_pod.insert(uid);
-    h->released.insert(uid);
-  }
-  return EGS_OK;
+  return account(h, EGS_MUT_FORGET, node_id, uid,
+                 [&](int cancel) { return apply_lists(h, cancel, node_id, n_containers, units, alloc_off, alloc_idx); });
 }
 
 // ------------------------------------------------------------------------------- mutation stream
@@ -762,32 +762,17 @@ static int mutations_apply_locked(egs_handle *h, int n, const egs_mutation *ops)
       for (int j = 0; j < m.n_idx[c]; j++) if (m.idx[c][j] < 0 || m.idx[c][j] >= h->h_gpu_count[m.node_id]) return EGS_ERR_BAD_ARG;
     }
   }
-  // pass 2: the podsMap / podMaps decisions in record order (node.go:131,149; scheduler.go:239-243,261-264)
+  // pass 2: the podsMap / podMaps decisions in record order; the surviving row updates are collected
   std::vector<ApplyOp> dev; dev.reserve((size_t)n);
-  auto push = [&](const egs_mutation &m, int cancel) {
-    ApplyOp o; memset(&o, 0, sizeof o);
-    o.node = m.node_id; o.cancel = cancel; o.req = make_req_w(m.n_containers, m.units);
-    for (int c = 0; c < m.n_containers; c++) { o.n_idx[c] = m.n_idx[c]; for (int j = 0; j < m.n_idx[c]; j++) o.idx[c][j] = m.idx[c][j]; }
-    dev.push_back(o);
-  };
   for (int i = 0; i < n; i++) {
     const egs_mutation &m = ops[i];
-    if (m.kind == EGS_MUT_ADD) {
-      if (in_pod_maps(h, m.uid)) continue;
-      if (!in_pods_map(h, m.node_id, m.uid)) { push(m, 0); h->pods_map.insert(NodeUid{m.node_id, m.uid}); }
-      h->pod_maps.insert(m.uid);
-    } else if (m.kind == EGS_MUT_REPLAY) {
-      if (!in_pods_map(h, m.node_id, m.uid)) { push(m, 0); h->pods_map.insert(NodeUid{m.node_id, m.uid}); }
-    } else {
-      if (m.node_id >= 0 && in_pods_map(h, m.node_id, m.uid)) {
-        push(m, 1);
-        if (!h->pods_map.erase(NodeUid{m.node_id, m.uid})) h->auto_gone_node.insert(NodeUid{m.node_id, m.uid});
-      }
-      if (in_pod_maps(h, m.uid)) {
-        if (!h->pod_maps.erase(m.uid)) h->auto_gone_pod.insert(m.uid);
-        h->released.insert(m.uid);
-      }
-    }
+    TRY(account(h, m.kind, m.node_id, m.uid, [&](int cancel) {
+      ApplyOp o; memset(&o, 0, sizeof o);
+      o.node = m.node_id; o.cancel = cancel; o.req = make_req<ReqW>(m.n_containers, m.units);
+      for (int c = 0; c < m.n_containers; c++) { o.n_idx[c] = m.n_idx[c]; for (int j = 0; j < m.n_idx[c]; j++) o.idx[c][j] = m.idx[c][j]; }
+      dev.push_back(o);
+      return EGS_OK;
+    }));
   }
   if (dev.empty()) return EGS_OK;
   // group by node, record order kept inside a node
@@ -872,7 +857,7 @@ static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_un
     a.vec_fit = p < h->vec_pods ? h->d_vec_fit + (size_t)p * h->max_nodes : nullptr;
     a.vec_score = p < h->vec_pods ? h->d_vec_score + (size_t)p * h->max_nodes : nullptr;
     a.partials = h->d_partials; a.ticket = h->d_ticket;
-    a.pod = p; a.out = out; a.do_bind = 1;
+    a.pod = p; a.out = out;
     if (is_single(C, u)) k_pass<true><<<grid, PASS_THREADS, 0, h->stream>>>(a);
     else k_pass<false><<<grid, PASS_THREADS, 0, h->stream>>>(a);
     if ((p & 1023) == 0) CK(h, cudaGetLastError());

@@ -45,6 +45,17 @@ struct Req {
   int mem[EGS_C];
   int cnt[EGS_C];
 };
+#define EGS_CA EGS_MAX_CONTAINERS_APPLY
+struct ReqW { int C; int core[EGS_CA], mem[EGS_CA], cnt[EGS_CA]; };   // a pod as AddPod / ForgetPod see it (up to 8 containers)
+
+// Req or ReqW from C units (C within the type's bound, checked by the caller); unused containers are zero.
+template <class R = Req>
+inline R make_req(int C, const egs_unit *u) {
+  R r = {};
+  r.C = C;
+  for (int i = 0; i < C; i++) { r.core[i] = u[i].core; r.mem[i] = u[i].mem; r.cnt[i] = u[i].count; }
+  return r;
+}
 
 __host__ __device__ __forceinline__ uint64_t mix64(uint64_t x) {
   uint64_t z = x + 0x9E3779B97F4A7C15ull;
@@ -334,6 +345,33 @@ EGS_HD bool transact_row(int32_t *core, int32_t *mem, int mem_total, const Req &
       int g = EGS_FFS(mk) - 1;
       if (!(core[g] >= r.core[i] && mem[g] >= r.mem[i])) return false;
       core[g] -= r.core[i]; mem[g] -= r.mem[i];
+    }
+  }
+  return true;
+}
+
+// One AddPod / ForgetPod row update with the option rebuilt from annotations (allocate.go:75-93): explicit index
+// lists; a fractional container uses its first index only.
+struct ApplyOp { int node, cancel; ReqW req; int n_idx[EGS_CA]; int8_t idx[EGS_CA][EGS_G]; };
+
+// The update on the node's rows (one thread): Cancel (gpu.go:177-191, GPU.Sub gpu.go:41-49: a whole-GPU container
+// puts its GPUs back at their totals) or Transact (gpu.go:153-175, CanAllocate + Add: the first failure stops the op,
+// no rollback).  Returns false when a Transact stopped.
+EGS_HD bool apply_op(int32_t *c, int32_t *m, int mt, const ApplyOp &op) {
+  for (int i = 0; i < op.req.C; i++) {
+    const bool whole = op.req.cnt[i] > 0;
+    const int lim = whole ? op.n_idx[i] : (op.n_idx[i] > 0 ? 1 : 0);
+    for (int j = 0; j < lim; j++) {
+      const int g = op.idx[i][j];
+      if (op.cancel) {
+        if (whole) { c[g] = EGS_CORE_PER_GPU; m[g] = mt; } else { c[g] += op.req.core[i]; m[g] += op.req.mem[i]; }
+      } else if (whole) {
+        if (!(c[g] == EGS_CORE_PER_GPU && m[g] == mt)) return false;
+        c[g] = 0; m[g] = 0;
+      } else {
+        if (!(c[g] >= op.req.core[i] && m[g] >= op.req.mem[i])) return false;
+        c[g] -= op.req.core[i]; m[g] -= op.req.mem[i];
+      }
     }
   }
   return true;

@@ -7,7 +7,10 @@
 //                fit/score digests, first-max selection and the bind (node.go:87-104) fused in
 //                the last block.  EGS_MODE_RESCAN launches it once per pod.
 //   k_gather_* : /scheduler/filter and /scheduler/priorities over an explicit candidate list.
-//   k_bind / k_apply : single-node mutations (Bind, AddPod, ForgetPod).
+//   k_bind / k_apply : single-node mutations (Bind, AddPod, ForgetPod); k_apply_many: many AddPod /
+//                ForgetPod in one launch.
+// Each reference step these kernels share is written once: Assume (assume_option), Allocate
+// (allocate_option), and the AddPod / ForgetPod row update (apply_op, egs_device.cuh).
 #pragma once
 #include "egs_device.cuh"
 
@@ -49,7 +52,7 @@ struct PassArgs {
   uint8_t *all_st; size_t slot_stride; int n_slots;   // every slot's state plane (UNFIT memo reset)
   uint8_t *vec_fit; int32_t *vec_score;    // optional full vectors
   Partial *partials; unsigned int *ticket;
-  int pod; PodOut out; int do_bind;
+  int pod; PodOut out;
 };
 
 __device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v) {
@@ -91,13 +94,45 @@ __device__ __forceinline__ void memo_reset(uint8_t *all_st, size_t slot_stride, 
   }
 }
 
-// NodeAllocator.Allocate (node.go:87-104) for the winner `w` of the current pod; one thread.
-__device__ __forceinline__ int bind_winner(const PassArgs &a, uint32_t w, uint32_t &masks) {
-  masks = 0;
-  for (int c = 0; c < a.req.C; c++) masks |= (uint32_t)a.t.al[(size_t)c * a.t.plane + w] << (8 * c);
-  a.t.st[w] = OPT_ABSENT;                                   // deferred delete, node.go:90-92
-  bool ok = transact_row(a.core_w + (size_t)w * EGS_G, a.mem_w + (size_t)w * EGS_G, a.mem_total[w], a.req, masks);
-  memo_reset(a.all_st, a.slot_stride, a.n_slots, w);
+// NodeAllocator.Assume (node.go:61-73) on node i; one thread.  An entry is reused without re-validation
+// (node.go:64-66); no entry -> Trade (node.go:67-71): the option is cached, or the failure memoised as UNFIT (the
+// reference caches nothing then and re-Trades with the same outcome).  Returns the state after Assume; `score` is
+// set when it is OPT_CACHED.  The fast Trade ignores mem_total, so SINGLE does not load it.
+template <bool SINGLE>
+__device__ __forceinline__ uint8_t assume_option(const OptTable &t, size_t i, const int32_t *core, const int32_t *mem,
+                                                 const int32_t *mem_total, const Req &req, int policy, int &score) {
+  uint8_t st = t.st[i];
+  if (st == OPT_CACHED) { score = t.sc[i]; return st; }
+  if (st != OPT_ABSENT) return st;
+  int c[EGS_G], m[EGS_G]; uint32_t masks;
+  load_row(core, mem, i, c, m);
+  if (trade_any(c, m, SINGLE ? 0 : mem_total[i], req, SINGLE, policy, score, masks)) {
+    st = OPT_CACHED;
+    t.sc[i] = score;
+    for (int k = 0; k < req.C; k++) t.al[(size_t)k * t.plane + i] = (uint8_t)(masks >> (8 * k));
+  } else {
+    st = OPT_UNFIT;
+  }
+  t.st[i] = st;
+  return st;
+}
+
+// GPU masks of node w's option, one u8 per container.
+__device__ __forceinline__ uint32_t option_masks(const OptTable &t, size_t w, int C) {
+  uint32_t masks = 0;
+  for (int c = 0; c < C; c++) masks |= (uint32_t)t.al[(size_t)c * t.plane + w] << (8 * c);
+  return masks;
+}
+
+// NodeAllocator.Allocate (node.go:87-104) of node w's cached option; one thread.  The entry goes before the Transact
+// (deferred delete, node.go:90-92); the rows changed, so the node's UNFIT memos go too.
+__device__ __forceinline__ int allocate_option(const OptTable &t, size_t w, int32_t *core, int32_t *mem, int mem_total,
+                                               const Req &req, uint8_t *all_st, size_t slot_stride, int n_slots,
+                                               uint32_t &masks) {
+  masks = option_masks(t, w, req.C);
+  t.st[w] = OPT_ABSENT;
+  const bool ok = transact_row(core + w * EGS_G, mem + w * EGS_G, mem_total, req, masks);
+  memo_reset(all_st, slot_stride, n_slots, w);
   return ok ? EGS_OK : EGS_ERR_TRANSACT;
 }
 
@@ -113,25 +148,8 @@ __global__ void __launch_bounds__(PASS_THREADS) k_pass(PassArgs a) {
   unsigned long long key = 0, fd = 0, sd = 0;
   int fit = 0;
   if (i < a.n) {
-    uint8_t st = a.t.st[i];
     int score = 0;
-    if (st == OPT_ABSENT) {                                 // cache miss -> Trade (node.go:67-71)
-      int c[EGS_G], m[EGS_G];
-      load_row(a.core, a.mem, (size_t)i, c, m);
-      uint32_t masks;
-      const int mt = SINGLE ? 0 : a.mem_total[i];
-      if (trade_any(c, m, mt, a.req, SINGLE, a.policy, score, masks)) {
-        st = OPT_CACHED;
-        a.t.sc[i] = score;
-        for (int k = 0; k < a.req.C; k++) a.t.al[(size_t)k * a.t.plane + i] = (uint8_t)(masks >> (8 * k));
-      } else {
-        st = OPT_UNFIT;                                     // not cached by the reference (node.go:68-70)
-      }
-      a.t.st[i] = st;
-    } else if (st == OPT_CACHED) {
-      score = a.t.sc[i];                                    // reused without re-validation (node.go:64-66)
-    }
-    if (st == OPT_CACHED) {
+    if (assume_option<SINGLE>(a.t, (size_t)i, a.core, a.mem, a.mem_total, a.req, a.policy, score) == OPT_CACHED) {
       fit = 1; key = cand_key(score, (uint32_t)i); fd = fit_term((uint32_t)i); sd = score_term((uint32_t)i, score);
     }
     if (a.vec_fit) a.vec_fit[i] = (uint8_t)fit;
@@ -158,12 +176,11 @@ __global__ void __launch_bounds__(PASS_THREADS) k_pass(PassArgs a) {
     *a.ticket = 0;
     int node = -1, status = EGS_ERR_NOFIT;
     uint32_t masks = 0;
-    if (key != 0 && a.do_bind) {
+    if (key != 0) {
       node = (int)key_node(key);
-      status = bind_winner(a, (uint32_t)node, masks);
+      status = allocate_option(a.t, (size_t)node, a.core_w, a.mem_w, a.mem_total[node], a.req, a.all_st, a.slot_stride,
+                               a.n_slots, masks);
       if (status != EGS_OK) masks = 0;
-    } else if (key != 0) {
-      node = (int)key_node(key); status = EGS_OK;
     }
     write_pod_out(a.out, a.pod, node, status, fit, fd, sd, masks);
   }
@@ -225,20 +242,8 @@ __global__ void __launch_bounds__(256) k_gather_filter(GatherArgs a) {
   if (j >= a.n) return;
   const int i = a.ids ? a.ids[j] : j;
   if (i < 0 || i >= a.n_nodes) { a.out_fit[j] = 0; return; }
-  uint8_t st = a.t.st[i];
-  if (st == OPT_ABSENT) {
-    int c[EGS_G], m[EGS_G], score; uint32_t masks;
-    load_row(a.core, a.mem, (size_t)i, c, m);
-    if (trade_any(c, m, a.mem_total[i], a.req, SINGLE, a.policy, score, masks)) {
-      st = OPT_CACHED;
-      a.t.sc[i] = score;
-      for (int k = 0; k < a.req.C; k++) a.t.al[(size_t)k * a.t.plane + i] = (uint8_t)(masks >> (8 * k));
-    } else {
-      st = OPT_UNFIT;
-    }
-    a.t.st[i] = st;
-  }
-  a.out_fit[j] = st == OPT_CACHED;
+  int score;
+  a.out_fit[j] = assume_option<SINGLE>(a.t, (size_t)i, a.core, a.mem, a.mem_total, a.req, a.policy, score) == OPT_CACHED;
 }
 
 // Score per node (node.go:75-85): cached score; no entry -> Assume; fails -> 0, succeeds -> the
@@ -249,19 +254,9 @@ __global__ void __launch_bounds__(256) k_gather_score(GatherArgs a) {
   if (j >= a.n) return;
   const int i = a.ids ? a.ids[j] : j;
   if (i < 0 || i >= a.n_nodes) { a.out_score[j] = 0; return; }   // scheduler.go:176-179
-  uint8_t st = a.t.st[i];
-  if (st == OPT_CACHED) { a.out_score[j] = a.t.sc[i]; return; }
-  if (st == OPT_ABSENT) {
-    int c[EGS_G], m[EGS_G], score; uint32_t masks;
-    load_row(a.core, a.mem, (size_t)i, c, m);
-    if (trade_any(c, m, a.mem_total[i], a.req, SINGLE, a.policy, score, masks)) {
-      a.t.st[i] = OPT_CACHED; a.t.sc[i] = score;              // Assume cached it before the nil deref
-      for (int k = 0; k < a.req.C; k++) a.t.al[(size_t)k * a.t.plane + i] = (uint8_t)(masks >> (8 * k));
-      *a.panic_flag = 1;
-    } else {
-      a.t.st[i] = OPT_UNFIT;
-    }
-  }
+  if (a.t.st[i] == OPT_CACHED) { a.out_score[j] = a.t.sc[i]; return; }
+  int score;                                                       // Assume caches the option before the nil deref
+  if (assume_option<SINGLE>(a.t, (size_t)i, a.core, a.mem, a.mem_total, a.req, a.policy, score) == OPT_CACHED) *a.panic_flag = 1;
   a.out_score[j] = 0;
 }
 
@@ -278,60 +273,32 @@ __global__ void k_bind(BindArgs a) {
   const bool had = a.t.st[w] == OPT_CACHED;
   uint32_t masks = 0; int status = EGS_ERR_NO_OPTION, score = 0;
   if (had) {
-    for (int c = 0; c < a.req.C; c++) masks |= (uint32_t)a.t.al[(size_t)c * a.t.plane + w] << (8 * c);
     score = a.t.sc[w];
     status = EGS_OK;
-    if (a.consume) {
-      a.t.st[w] = OPT_ABSENT;
-      if (!a.skip_transact) {
-        bool ok = transact_row(a.core + w * EGS_G, a.mem + w * EGS_G, a.mem_total[w], a.req, masks);
-        memo_reset(a.all_st, a.slot_stride, a.n_slots, w);
-        status = ok ? EGS_OK : EGS_ERR_TRANSACT;
-      }
+    if (a.consume && !a.skip_transact) {
+      status = allocate_option(a.t, w, a.core, a.mem, a.mem_total[w], a.req, a.all_st, a.slot_stride, a.n_slots, masks);
+    } else {                                     // peek, or Bind of a known uid (node.go:149): the entry goes, rows stay
+      masks = option_masks(a.t, w, a.req.C);
+      if (a.consume) a.t.st[w] = OPT_ABSENT;
     }
   }
   a.result[0] = had; a.result[1] = status; a.result[2] = (int32_t)masks; a.result[3] = score;
 }
 
-// AddPod / ForgetPod with the option rebuilt from annotations (allocate.go:75-93):
-// explicit index lists, Transact (gpu.go:153-175) or Cancel (gpu.go:177-191).
-#define EGS_CA EGS_MAX_CONTAINERS_APPLY
-struct ReqW { int C; int core[EGS_CA], mem[EGS_CA], cnt[EGS_CA]; };   // a pod as AddPod / ForgetPod see it (up to 8 containers)
+// AddPod / ForgetPod of one pod (apply_op) on node op.node.
 struct ApplyArgs {
   int32_t *core, *mem; const int32_t *mem_total;
-  int node; ReqW req;
-  int n_idx[EGS_CA]; int8_t idx[EGS_CA][EGS_G];
+  ApplyOp op;
   uint8_t *all_st; size_t slot_stride; int n_slots;
-  int cancel;
 };
 __global__ void k_apply(ApplyArgs a) {
-  int32_t *c = a.core + (size_t)a.node * EGS_G, *m = a.mem + (size_t)a.node * EGS_G;
-  const int mt = a.mem_total[a.node];
-  bool stop = false;
-  for (int i = 0; i < a.req.C && !stop; i++) {
-    const bool whole = a.req.cnt[i] > 0;
-    const int lim = whole ? a.n_idx[i] : (a.n_idx[i] > 0 ? 1 : 0);
-    for (int j = 0; j < lim; j++) {
-      const int g = a.idx[i][j];
-      if (a.cancel) {                                          // GPU.Sub gpu.go:41-49
-        if (whole) { c[g] = EGS_CORE_PER_GPU; m[g] = mt; } else { c[g] += a.req.core[i]; m[g] += a.req.mem[i]; }
-      } else {                                                 // CanAllocate + Add
-        if (whole) {
-          if (!(c[g] == EGS_CORE_PER_GPU && m[g] == mt)) { stop = true; break; }
-          c[g] = 0; m[g] = 0;
-        } else {
-          if (!(c[g] >= a.req.core[i] && m[g] >= a.req.mem[i])) { stop = true; break; }
-          c[g] -= a.req.core[i]; m[g] -= a.req.mem[i];
-        }
-      }
-    }
-  }
-  memo_reset(a.all_st, a.slot_stride, a.n_slots, (size_t)a.node);
+  const size_t w = (size_t)a.op.node;
+  apply_op(a.core + w * EGS_G, a.mem + w * EGS_G, a.mem_total[w], a.op);
+  memo_reset(a.all_st, a.slot_stride, a.n_slots, w);
 }
 
 // Many AddPod / ForgetPod row updates in ONE launch: the host has grouped the records by node (record order kept
-// inside a node); one thread per touched node applies its run with the arithmetic of k_apply.
-struct ApplyOp { int node, cancel; ReqW req; int n_idx[EGS_CA]; int8_t idx[EGS_CA][EGS_G]; };
+// inside a node); one thread per touched node applies its run.
 struct ApplyManyArgs {
   int32_t *core, *mem; const int32_t *mem_total;
   const ApplyOp *ops; const int32_t *group_off; int n_groups;   // group g = ops[group_off[g] .. group_off[g+1])
@@ -340,32 +307,10 @@ struct ApplyManyArgs {
 __global__ void k_apply_many(ApplyManyArgs a) {
   const int gi = blockIdx.x * blockDim.x + threadIdx.x;
   if (gi >= a.n_groups) return;
-  const int node = a.ops[a.group_off[gi]].node;
-  int32_t *c = a.core + (size_t)node * EGS_G, *m = a.mem + (size_t)node * EGS_G;
-  const int mt = a.mem_total[node];
-  for (int o = a.group_off[gi]; o < a.group_off[gi + 1]; o++) {
-    const ApplyOp &op = a.ops[o];
-    bool stop = false;
-    for (int i = 0; i < op.req.C && !stop; i++) {
-      const bool whole = op.req.cnt[i] > 0;
-      const int lim = whole ? op.n_idx[i] : (op.n_idx[i] > 0 ? 1 : 0);
-      for (int j = 0; j < lim; j++) {
-        const int g = op.idx[i][j];
-        if (op.cancel) {                                         // GPU.Sub gpu.go:41-49
-          if (whole) { c[g] = EGS_CORE_PER_GPU; m[g] = mt; } else { c[g] += op.req.core[i]; m[g] += op.req.mem[i]; }
-        } else {                                                 // CanAllocate + Add; first failure stops, no rollback (gpu.go:153-175)
-          if (whole) {
-            if (!(c[g] == EGS_CORE_PER_GPU && m[g] == mt)) { stop = true; break; }
-            c[g] = 0; m[g] = 0;
-          } else {
-            if (!(c[g] >= op.req.core[i] && m[g] >= op.req.mem[i])) { stop = true; break; }
-            c[g] -= op.req.core[i]; m[g] -= op.req.mem[i];
-          }
-        }
-      }
-    }
-  }
-  memo_reset(a.all_st, a.slot_stride, a.n_slots, (size_t)node);
+  const size_t w = (size_t)a.ops[a.group_off[gi]].node;
+  for (int o = a.group_off[gi]; o < a.group_off[gi + 1]; o++)
+    apply_op(a.core + w * EGS_G, a.mem + w * EGS_G, a.mem_total[w], a.ops[o]);
+  memo_reset(a.all_st, a.slot_stride, a.n_slots, w);
 }
 
 // Rows of nodes [node0, node0+n) were overwritten from the host.  full != 0 (node_set: a fresh

@@ -1,16 +1,8 @@
 // device_on_host.cu -- the kernels' integer arithmetic (egs_device.cuh: Trade fast path, general Trade,
-// Transact) compiled for the HOST, so the CPU test suite can check the very source the GPU runs against
-// the oracle (tests/test_device_arith_host.py).  Not part of libegs.
-#include <cstring>
-
+// Transact, the AddPod / ForgetPod row update) compiled for the HOST, so the CPU test suite can check the very
+// source the GPU runs against the oracle (tests/test_device_arith_host.py).  Not part of libegs.
 #include "../egs_device.cuh"
 
-static Req make_req(int C, const egs_unit *u) {
-  Req r; memset(&r, 0, sizeof r);
-  r.C = C;
-  for (int i = 0; i < C; i++) { r.core[i] = u[i].core; r.mem[i] = u[i].mem; r.cnt[i] = u[i].count; }
-  return r;
-}
 static void rows(const int32_t *core, const int32_t *mem, int (&c)[EGS_G], int (&m)[EGS_G]) {
   for (int g = 0; g < EGS_G; g++) { c[g] = core[g]; m[g] = mem[g]; }
 }
@@ -63,6 +55,18 @@ int egsdh_trade_lanes(const int32_t *core, const int32_t *mem, int rq_core, int 
 int egsdh_transact(int32_t *core, int32_t *mem, int mem_total, int C, const egs_unit *units, uint32_t masks) {
   const Req r = make_req(C, units);
   return transact_row(core, mem, mem_total, r, masks) ? 1 : 0;
+}
+// apply_op (k_apply / k_apply_many) on one node's rows: C <= EGS_MAX_CONTAINERS_APPLY containers, container c's
+// GPU indices in idx[c*EGS_MAX_GPUS .. + n_idx[c])
+int egsdh_apply(int32_t *core, int32_t *mem, int mem_total, int C, const egs_unit *units, const int32_t *n_idx,
+                const int32_t *idx, int cancel) {
+  ApplyOp op = {};
+  op.cancel = cancel; op.req = make_req<ReqW>(C, units);
+  for (int c = 0; c < C; c++) {
+    op.n_idx[c] = n_idx[c];
+    for (int j = 0; j < n_idx[c]; j++) op.idx[c][j] = (int8_t)idx[c * EGS_G + j];
+  }
+  return apply_op(core, mem, mem_total, op) ? 1 : 0;
 }
 int egsdh_is_single(int C, const egs_unit *units) { const Req r = make_req(C, units); return req_is_single(r) ? 1 : 0; }
 unsigned long long egsdh_cand_key(int32_t score, uint32_t node) { return cand_key(score, node); }

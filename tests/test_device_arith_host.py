@@ -1,6 +1,6 @@
 """The kernels' integer arithmetic -- csrc/egs_device.cuh: the Trade fast path (prefix/suffix maxima,
-unsigned-min PAD trick, packed q*8+g key) and its one-GPU-per-lane form in the resolver, the general DFS Trade
-and Transact -- compiled for the host
+unsigned-min PAD trick, packed q*8+g key) and its one-GPU-per-lane form in the resolver, the general DFS Trade,
+Transact and the AddPod / ForgetPod row update -- compiled for the host
 (csrc/host_test/device_on_host.cu) and checked against the oracle WITHOUT a GPU.  Same source the kernels
 inline; the device SASS is unaffected by the host build."""
 import ctypes as C
@@ -21,6 +21,7 @@ def DH():
     L.egsdh_trade.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     L.egsdh_trade_leaves.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     L.egsdh_transact.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint32]
+    L.egsdh_apply.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     L.egsdh_trade_lanes.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     L.egsdh_is_single.argtypes = [C.c_int, C.c_void_p]
     for f in ("egsdh_cand_key", "egsdh_fit_term", "egsdh_score_term"):
@@ -142,6 +143,55 @@ def test_kernel_transact_equals_oracle(DH, rows, req, mt, stale):
     ok = DH.egsdh_transact(core.ctypes.data, mem.ctypes.data, mt, len(req), _units(req).ctypes.data, masks)
     assert bool(ok) == po.transact(g, opt)
     assert [(int(core[i]), int(mem[i])) for i in range(len(g))] == [(x.core_avail, x.mem_avail) for x in g]
+
+
+@st.composite
+def apply_records(draw):
+    """(mem_total, rows, records) on one node of 1..8 GPUs whose rows may sit above their totals.  A record is
+    (cancel, [(unit, GPU indices)]) with up to 8 fractional, whole-GPU or sentinel containers; the index lists are
+    what the annotations hold, so they may repeat a GPU or name one that no longer fits."""
+    mt = draw(st.integers(1, 40))
+    rows = draw(st.lists(st.tuples(st.integers(0, 103), st.integers(0, mt + 3)), min_size=1, max_size=8))
+    gpu = st.integers(0, len(rows) - 1)
+    container = st.one_of(
+        st.tuples(st.tuples(st.integers(0, 100), st.integers(0, 40), st.just(0)), st.lists(gpu, max_size=2)),
+        st.tuples(st.tuples(st.just(0), st.just(0), st.integers(1, 3)), st.lists(gpu, max_size=4)),
+        st.tuples(st.just((-1, -1, 0)), st.lists(gpu, max_size=1)),
+    )
+    records = draw(st.lists(st.tuples(st.booleans(), st.lists(container, min_size=1, max_size=8)), min_size=1, max_size=4))
+    return mt, rows, records
+
+
+@settings(max_examples=600, deadline=None)
+@given(case=apply_records())
+def test_apply_row_update_equals_oracle(DH, case):
+    """apply_op, the row update of k_apply and k_apply_many, against the oracle's NodeAllocator.Add / Forget (what
+    AddPod / ForgetPod call) with fresh uids, so every record reaches the rows: Transact stops at the first GPU that
+    cannot take its container and keeps the Adds before it; Cancel puts a whole-GPU container's GPUs back at their
+    totals; a fractional container uses its first index only."""
+    mt, rows, records = case
+    s = po.Scheduler(po.POLICY_BINPACK)
+    s.add_node(100 * len(rows), mt * len(rows))
+    s.set_rows(0, [c for c, _ in rows], [m for _, m in rows])
+    na = s.nodes[0]
+    core, mem = _pad(rows)
+    for uid, (cancel, containers) in enumerate(records):
+        req = [u for u, _ in containers]
+        alloc = [list(ix) for _, ix in containers]
+        n_idx = np.array([len(ix) for ix in alloc], np.int32)
+        idx = np.zeros((len(alloc), 8), np.int32)
+        for c, ix in enumerate(alloc):
+            idx[c, :len(ix)] = ix
+        got = DH.egsdh_apply(core.ctypes.data, mem.ctypes.data, mt, len(req), _units(req).ctypes.data,
+                             n_idx.ctypes.data, idx.ctypes.data, int(cancel))
+        if cancel:
+            na.pods_map[uid] = True                                   # the pod is on the node: Forget cancels it
+            na.forget(req, alloc, uid)
+            assert got == 1
+        else:
+            assert bool(got) == na.add(uid, po.GPUOption(request=req, allocated=alloc))
+        assert [(int(core[g]), int(mem[g])) for g in range(len(rows))] == s.rows(0)
+        assert (core[len(rows):] == PAD).all() and (mem[len(rows):] == PAD).all()
 
 
 def _trade_leaves(DH, rows, mt, req, policy):
