@@ -32,9 +32,13 @@ def nvcc_path() -> str:
     return p
 
 
+def _libegs_sources():
+    return sorted(glob.glob(os.path.join(CSRC, "*.cu")) + glob.glob(os.path.join(CSRC, "*.cuh")) +
+                  glob.glob(os.path.join(CSRC, "*.h")) + [os.path.join(ROOT, "include", "egs.h")])
+
+
 def build_libegs(force: bool = False, verbose: bool = False) -> str:
-    srcs = sorted(glob.glob(os.path.join(CSRC, "*.cu")) + glob.glob(os.path.join(CSRC, "*.cuh")) +
-                  [os.path.join(ROOT, "include", "egs.h")])
+    srcs = _libegs_sources()
     if force or _stale(LIBEGS, srcs):
         os.makedirs(LIBDIR, exist_ok=True)
         cmd = [nvcc_path()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + \
@@ -49,8 +53,7 @@ LIBPROF = os.path.join(LIBDIR, "libegs_prof.so")
 def build_prof(force: bool = False) -> str:
     """PROFILING ONLY (tools/gpu_round.sh, tools/prof_sections.py with EGS_LIB=libegs_prof.so): libegs with the
     resolver's clock64 section counters compiled in (-DEGS_RESOLVE_PROF).  Not part of build_all."""
-    srcs = sorted(glob.glob(os.path.join(CSRC, "*.cu")) + glob.glob(os.path.join(CSRC, "*.cuh")) +
-                  [os.path.join(ROOT, "include", "egs.h")])
+    srcs = _libegs_sources()
     if force or _stale(LIBPROF, srcs):
         os.makedirs(LIBDIR, exist_ok=True)
         flags = [f for f in NVCC_FLAGS if f != "-DEGS_RESOLVE_PROF"]
@@ -95,6 +98,19 @@ def build_devhost(force: bool = False) -> str:
     return LIBDEVHOST
 
 
+LIBPODBOOK = os.path.join(LIBDIR, "libegs_podbook.so")
+
+
+def build_podbook(force: bool = False) -> str:
+    """The uid bookkeeping (csrc/pod_book.h) behind a small C API: CPU-side tests only."""
+    src = os.path.join(CSRC, "host_test", "pod_book_on_host.cc")
+    deps = [src, os.path.join(CSRC, "pod_book.h"), os.path.join(ROOT, "include", "egs.h")]
+    if force or _stale(LIBPODBOOK, deps):
+        os.makedirs(LIBDIR, exist_ok=True)
+        subprocess.check_call(["g++", "-O2", "-std=c++17", "-Wall", "-fPIC", "-shared", "-o", LIBPODBOOK, src])
+    return LIBPODBOOK
+
+
 SHIM_DOUBLE = os.path.join(ROOT, "integration", "_build", "shim_double")
 
 
@@ -113,4 +129,5 @@ def build_all(force: bool = False) -> None:
     build_libegs(force)
     build_host(force)
     build_devhost(force)
+    build_podbook(force)
     build_shim_double(force)

@@ -14,14 +14,8 @@
 
 #include "egs_kernels.cuh"
 #include "egs_rounds.cuh"
+#include "pod_book.h"
 
-struct NodeUid {
-  int node; uint64_t uid;
-  bool operator==(const NodeUid &o) const { return node == o.node && uid == o.uid; }
-};
-struct NodeUidHash {
-  size_t operator()(const NodeUid &k) const { return (size_t)mix64(k.uid ^ ((uint64_t)(uint32_t)k.node << 40)); }
-};
 struct Shape { int C; egs_unit u[EGS_C]; };
 
 // Pinned host buffer holding (node[n], status[n]) of a batch.  Recycled through egs_handle::pin_pool: cudaMallocHost /
@@ -30,9 +24,6 @@ struct PinBuf { int32_t *p = nullptr; size_t cap = 0; };   // cap in int32 eleme
 struct PendingBatch {           // results of a batch whose uid bookkeeping is applied lazily
   int n; uint64_t uid0; std::vector<uint64_t> uids; int32_t *h_node, *h_status; PinBuf buf; cudaEvent_t done;
 };
-// A finished batch with library-assigned UIDs [uid0, uid0+n): podsMap / podMaps membership is read
-// straight from the result arrays (node.go:150, scheduler.go:224) -- no per-pod hash insert.
-struct AutoBatch { uint64_t uid0; int n; int32_t *h_node, *h_status; PinBuf buf; bool nodes_valid; };
 
 struct egs_handle {
   int policy = 0, max_nodes = 0, n_pad = 0, g_max = 0, device = 0, n_sm = 0;
@@ -51,13 +42,9 @@ struct egs_handle {
   struct ShapeCacheEnt { uint64_t h; int slot; };
   std::vector<ShapeCacheEnt> shape_cache = std::vector<ShapeCacheEnt>(1024, ShapeCacheEnt{0, -1});   // open addressing
   // reference bookkeeping that never reaches the device
-  std::unordered_set<NodeUid, NodeUidHash> pods_map;           // NodeAllocator.podsMap (node.go:16)
-  std::unordered_set<uint64_t> pod_maps, released;             // BaseScheduler.podMaps / releasedPodMap
-  std::vector<PendingBatch> pending;
-  std::vector<AutoBatch> auto_batches;
+  PodBook book;                                                 // podsMap / podMaps / releasedPodMap
+  std::vector<PendingBatch> pending;                            // batches whose results have not reached the book
   std::vector<PinBuf> pin_pool;                                 // idle pinned result buffers (at most PIN_POOL_MAX)
-  std::unordered_set<uint64_t> auto_gone_pod;                  // auto uids erased from podMaps (ForgetPod)
-  std::unordered_set<NodeUid, NodeUidHash> auto_gone_node;     // auto (node, uid) erased from a podsMap
   uint64_t next_uid = 0x8000000000000000ull;
   // scratch
   Partial *d_partials = nullptr; unsigned int *d_ticket = nullptr; int32_t *d_result = nullptr;
@@ -193,46 +180,17 @@ static int intern_slow(egs_handle *h, int C, const egs_unit *u, int *slot) {
 
 static bool is_single(int C, const egs_unit *u) { return C == 1 && u[0].count == 0 && u[0].core >= 0 && u[0].mem >= 0; }
 
-static const AutoBatch *auto_find(const egs_handle *h, uint64_t uid) {
-  for (const auto &b : h->auto_batches) if (uid >= b.uid0 && uid < b.uid0 + (uint64_t)b.n) return &b;
-  return nullptr;
-}
-static bool in_pods_map(const egs_handle *h, int node, uint64_t uid) {
-  if (h->pods_map.count(NodeUid{node, uid})) return true;
-  const AutoBatch *b = auto_find(h, uid);
-  return b && b->nodes_valid && b->h_node[uid - b->uid0] == node && !h->auto_gone_node.count(NodeUid{node, uid});
-}
-static bool in_pod_maps(const egs_handle *h, uint64_t uid) {
-  if (h->pod_maps.count(uid)) return true;
-  const AutoBatch *b = auto_find(h, uid);
-  return b && b->h_node[uid - b->uid0] >= 0 && b->h_status[uid - b->uid0] == EGS_OK && !h->auto_gone_pod.count(uid);
-}
 constexpr size_t PIN_POOL_MAX = 4;
-static int pin_get(egs_handle *h, size_t n, PinBuf *out);
 static void pin_put(egs_handle *h, PinBuf b) {
   if (!b.p) return;
   if (h->pin_pool.size() < PIN_POOL_MAX) h->pin_pool.push_back(b); else cudaFreeHost(b.p);
-}
-static void free_auto_batches(egs_handle *h) {
-  for (auto &b : h->auto_batches) pin_put(h, b.buf);
-  h->auto_batches.clear(); h->auto_gone_pod.clear(); h->auto_gone_node.clear();
 }
 
 static int flush_pending(egs_handle *h) {
   for (auto &b : h->pending) {
     CK(h, cudaEventSynchronize(b.done));
-    if (b.uids.empty()) {                                        // library-assigned contiguous uids: keep the arrays
-      h->auto_batches.push_back(AutoBatch{b.uid0, b.n, b.h_node, b.h_status, b.buf, true});
-      cudaEventDestroy(b.done);
-      continue;
-    }
-    for (int p = 0; p < b.n; p++) {
-      uint64_t uid = b.uids.empty() ? b.uid0 + (uint64_t)p : b.uids[p];
-      if (b.h_node[p] >= 0) {
-        h->pods_map.insert(NodeUid{b.h_node[p], uid});                 // node.go:150
-        if (b.h_status[p] == EGS_OK) h->pod_maps.insert(uid);          // scheduler.go:224
-      }
-    }
+    if (b.uids.empty()) h->book.add_run(b.uid0, b.n, b.h_node, b.h_status);     // library-assigned uids
+    else h->book.add_batch(b.uids.data(), b.n, b.h_node, b.h_status);
     pin_put(h, b.buf); cudaEventDestroy(b.done);
   }
   h->pending.clear();
@@ -300,7 +258,6 @@ extern "C" int egs_destroy(egs_handle *h) {
   cudaSetDevice(h->device);
   cudaStreamSynchronize(h->stream);
   flush_pending(h);
-  free_auto_batches(h);
   for (auto &b : h->pin_pool) cudaFreeHost(b.p);
   h->pin_pool.clear();
   rounds_free(&h->rounds);
@@ -390,28 +347,6 @@ static int load_rows(egs_handle *h, int node0, int n, int gpu_count, int mem_tot
   return EGS_OK;
 }
 
-// podsMap entries of nodes [node0, node0+n) vanish with their NodeAllocator (one pass)
-static void drop_node_pods(egs_handle *h, int node0, int n) {
-  if (h->pods_map.empty() && h->auto_batches.empty()) return;   // batches with library-assigned uids live in auto_batches
-  if (node0 == 0 && n >= h->max_nodes) {
-    h->pods_map.clear();
-    // auto batches: every node reloaded -> no podsMap entry survives; podMaps (scheduler level) does
-    for (auto &b : h->auto_batches) b.nodes_valid = false;
-    h->auto_gone_node.clear();
-    return;
-  }
-  // partial reload: materialise the auto batches into the hash sets first (rare path)
-  for (auto &b : h->auto_batches)
-    for (int p = 0; p < b.n; p++) if (b.h_node[p] >= 0) {
-      const uint64_t uid = b.uid0 + p;
-      if (b.nodes_valid && !h->auto_gone_node.count(NodeUid{b.h_node[p], uid})) h->pods_map.insert(NodeUid{b.h_node[p], uid});
-      if (b.h_status[p] == EGS_OK && !h->auto_gone_pod.count(uid)) h->pod_maps.insert(uid);
-    }
-  free_auto_batches(h);
-  for (auto it = h->pods_map.begin(); it != h->pods_map.end();)
-    if (it->node >= node0 && it->node < node0 + n) it = h->pods_map.erase(it); else ++it;
-}
-
 // wait for in-flight batches and drop their bookkeeping without applying it
 static int discard_pending(egs_handle *h) {
   for (auto &b : h->pending) {
@@ -427,7 +362,7 @@ extern "C" int egs_node_set(egs_handle *h, int node_id, int gpu_count, int mem_t
   Guard g(h);
   TRY(flush_pending(h));
   TRY(load_rows(h, node_id, 1, gpu_count, mem_total_per_gpu, nullptr, nullptr, true));
-  drop_node_pods(h, node_id, 1);
+  h->book.drop_nodes(node_id, 1);
   return EGS_OK;
 }
 
@@ -456,7 +391,7 @@ extern "C" int egs_state_load_bulk(egs_handle *h, int node0, int n, int gpu_coun
   // pending batch results only feed podsMap/podMaps; podMaps (scheduler level) survives a node reload
   TRY(flush_pending(h));
   TRY(load_rows(h, node0, n, gpu_count, mem_total, free_core, free_mem, true));
-  drop_node_pods(h, node0, n);
+  h->book.drop_nodes(node0, n);
   return EGS_OK;
 }
 
@@ -510,7 +445,7 @@ extern "C" int egs_state_restore(egs_handle *h) {
     CK(h, cudaMemsetAsync(h->d_st, OPT_ABSENT, (size_t)h->n_pad * h->shapes.size(), h->stream));
   std::fill(h->slot_cold.begin(), h->slot_cold.end(), 1);
   h->h_gpu_count = h->snap_gpu_count; h->h_mem_total = h->snap_mem_total;
-  h->pods_map.clear(); h->pod_maps.clear(); h->released.clear(); free_auto_batches(h);
+  h->book.clear();
   return EGS_OK;
 }
 
@@ -590,17 +525,14 @@ static int bind_or_peek(egs_handle *h, int consume, int node_id, int C, const eg
   a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total; a.node = node_id;
   a.req = make_req(C, units); a.t = table(h, slot);
   a.all_st = h->d_st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
-  const bool known = consume && in_pods_map(h, node_id, uid);
+  const bool known = consume && h->book.in_pods_map(node_id, uid);
   a.skip_transact = known ? 1 : 0; a.consume = consume; a.result = h->d_result;
   k_bind<<<1, 1, 0, h->stream>>>(a);
   CK(h, cudaGetLastError());
   CK(h, cudaMemcpyAsync(h->h_result, h->d_result, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaStreamSynchronize(h->stream));
   memcpy(res4, h->h_result, 4 * sizeof(int32_t));
-  if (consume) {
-    if (res4[0] && !known) h->pods_map.insert(NodeUid{node_id, uid});     // node.go:150, before Transact
-    if (res4[1] == EGS_OK) h->pod_maps.insert(uid);                       // scheduler.go:224
-  }
+  if (consume) h->book.record_bind(node_id, uid, res4[0] != 0, known, res4[1]);
   return EGS_OK;
 }
 
@@ -676,33 +608,6 @@ static int apply_lists(egs_handle *h, int cancel, int node_id, int C, const egs_
   return EGS_OK;
 }
 
-// The podsMap / podMaps decision of one EGS_MUT_* record on `node`, in the reference's order.  apply(cancel) makes
-// the row update the reference would make, before the bookkeeping that follows it; a failing apply ends the record.
-// The single verbs validate a pod's index lists inside apply, i.e. only when the record reaches a row update, which
-// is when the reference parses the annotations: a known uid with a malformed list is EGS_OK there.  The mutation
-// stream validates every record's lists before it applies any, so the same record fails the whole stream.
-template <class F>
-static int account(egs_handle *h, int kind, int node, uint64_t uid, F &&apply) {
-  if (kind == EGS_MUT_FORGET) {                                             // ForgetPod scheduler.go:247-267
-    if (node >= 0 && in_pods_map(h, node, uid)) {                           // node.go:131
-      TRY(apply(1));
-      if (!h->pods_map.erase(NodeUid{node, uid})) h->auto_gone_node.insert(NodeUid{node, uid});
-    }
-    if (in_pod_maps(h, uid)) {                                              // scheduler.go:261-264
-      if (!h->pod_maps.erase(uid)) h->auto_gone_pod.insert(uid);
-      h->released.insert(uid);
-    }
-    return EGS_OK;
-  }
-  if (kind == EGS_MUT_ADD && in_pod_maps(h, uid)) return EGS_OK;           // scheduler.go:239-241
-  if (!in_pods_map(h, node, uid)) {                                         // node.go:149
-    TRY(apply(0));
-    h->pods_map.insert(NodeUid{node, uid});
-  }
-  if (kind == EGS_MUT_ADD) h->pod_maps.insert(uid);                         // scheduler.go:243
-  return EGS_OK;
-}
-
 // AddPod scheduler.go:229-245
 extern "C" int egs_pod_apply(egs_handle *h, int node_id, int n_containers, const egs_unit *units,
                              const int32_t *alloc_off, const int32_t *alloc_idx, uint64_t uid) {
@@ -712,8 +617,8 @@ extern "C" int egs_pod_apply(egs_handle *h, int node_id, int n_containers, const
   if (h->h_gpu_count[node_id] == 0) return EGS_ERR_NO_NODE;
   TRY(check_units(n_containers, units, EGS_MAX_CONTAINERS_APPLY));
   TRY(flush_pending(h));
-  return account(h, EGS_MUT_ADD, node_id, uid,
-                 [&](int cancel) { return apply_lists(h, cancel, node_id, n_containers, units, alloc_off, alloc_idx); });
+  return h->book.account(EGS_MUT_ADD, node_id, uid,
+                         [&](int cancel) { return apply_lists(h, cancel, node_id, n_containers, units, alloc_off, alloc_idx); });
 }
 
 // NodeAllocator.Add(pod, nil) node.go:148-160 (replay at node load, node.go:52-54)
@@ -725,8 +630,8 @@ extern "C" int egs_node_replay_pod(egs_handle *h, int node_id, int n_containers,
   if (h->h_gpu_count[node_id] == 0) return EGS_ERR_NO_NODE;
   TRY(check_units(n_containers, units, EGS_MAX_CONTAINERS_APPLY));
   TRY(flush_pending(h));
-  return account(h, EGS_MUT_REPLAY, node_id, uid,
-                 [&](int cancel) { return apply_lists(h, cancel, node_id, n_containers, units, alloc_off, alloc_idx); });
+  return h->book.account(EGS_MUT_REPLAY, node_id, uid,
+                         [&](int cancel) { return apply_lists(h, cancel, node_id, n_containers, units, alloc_off, alloc_idx); });
 }
 
 // ForgetPod scheduler.go:247-267
@@ -740,8 +645,8 @@ extern "C" int egs_pod_cancel(egs_handle *h, int node_id, int n_containers, cons
     if (h->h_gpu_count[node_id] == 0) return EGS_ERR_NO_NODE;
     TRY(check_units(n_containers, units, EGS_MAX_CONTAINERS_APPLY));
   }
-  return account(h, EGS_MUT_FORGET, node_id, uid,
-                 [&](int cancel) { return apply_lists(h, cancel, node_id, n_containers, units, alloc_off, alloc_idx); });
+  return h->book.account(EGS_MUT_FORGET, node_id, uid,
+                         [&](int cancel) { return apply_lists(h, cancel, node_id, n_containers, units, alloc_off, alloc_idx); });
 }
 
 // ------------------------------------------------------------------------------- mutation stream
@@ -766,7 +671,7 @@ static int mutations_apply_locked(egs_handle *h, int n, const egs_mutation *ops)
   std::vector<ApplyOp> dev; dev.reserve((size_t)n);
   for (int i = 0; i < n; i++) {
     const egs_mutation &m = ops[i];
-    TRY(account(h, m.kind, m.node_id, m.uid, [&](int cancel) {
+    TRY(h->book.account(m.kind, m.node_id, m.uid, [&](int cancel) {
       ApplyOp o; memset(&o, 0, sizeof o);
       o.node = m.node_id; o.cancel = cancel; o.req = make_req<ReqW>(m.n_containers, m.units);
       for (int c = 0; c < m.n_containers; c++) { o.n_idx[c] = m.n_idx[c]; for (int j = 0; j < m.n_idx[c]; j++) o.idx[c][j] = m.idx[c][j]; }
@@ -817,12 +722,12 @@ extern "C" int egs_pod_known(egs_handle *h, uint64_t uid) {
   if (!h) return 0;
   Guard g(h);
   if (flush_pending(h) != EGS_OK) return 0;
-  return in_pod_maps(h, uid) ? 1 : 0;
+  return h->book.in_pod_maps(uid) ? 1 : 0;
 }
 extern "C" int egs_pod_released(egs_handle *h, uint64_t uid) {
   if (!h) return 0;
   Guard g(h);
-  return h->released.count(uid) ? 1 : 0;
+  return h->book.released(uid) ? 1 : 0;
 }
 
 // ------------------------------------------------------------------------------- batch loop
@@ -882,7 +787,7 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
     TRY(flush_pending(h));
     std::unordered_set<uint64_t> seen; seen.reserve((size_t)P * 2);
     for (int p = 0; p < P; p++) {
-      if (!seen.insert(uids[p]).second || in_pod_maps(h, uids[p])) return fail(h, EGS_ERR_BAD_ARG, "duplicate or known uid");
+      if (!seen.insert(uids[p]).second || h->book.in_pod_maps(uids[p])) return fail(h, EGS_ERR_BAD_ARG, "duplicate or known uid");
     }
   }
   PodOut dev = out;

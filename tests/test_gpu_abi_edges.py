@@ -133,6 +133,38 @@ def test_node_reload_after_auto_uid_batch_drops_pods_map():
     assert e.pod_released(uid)                                                  # scheduler-level podMaps had it
 
 
+def test_auto_uid_bound_again_elsewhere_then_forgotten_is_unknown():
+    """A pod with a library-assigned uid U won node 0 in a batch; then Bind puts U on node 1 as well (podMaps[U] is set
+    again without a check, scheduler.go:224).  ForgetPod on node 1 deletes U from podMaps (scheduler.go:261-264), so
+    U is no longer known, while node 0's podsMap still holds it and a ForgetPod there cancels node 0's rows."""
+    import oracle_c as oc
+    eg = _eg()
+    U = 0x8000000000000000
+    req = [(20, 4, 0)]
+    c_off = np.array([0, 1], np.int32)
+    e = eg.Egs(0, 2)
+    o = oc.OracleC(0)
+    for n in range(2):
+        assert e.node_set_allocatable(n, 200, 32) == 0
+        o.add_node(200, 32)
+    assert e.state_load(0, [60, 100], [10, 16]) == 0                          # node 0 the fuller: binpack picks it
+    o.set_rows(0, [60, 100], [10, 16])
+    got = e.schedule_batch(c_off, np.array(req, np.int32), mode=eg.capi.EGS_MODE_ROUNDS)   # uids == NULL: U
+    ref = o.schedule_batch(c_off, np.array(req, np.int64), uids=np.array([U], np.uint64))
+    assert got["node"][0] == ref["node"][0] == 0 and got["status"][0] == ref["status"][0] == 0
+    assert list(e.filter([1], req)) == list(o.filter([1], req)) == [1]
+    st, alloc = e.bind(1, req, U)
+    assert (st, alloc) == o.bind(1, req, U) and st == 0
+    assert e.pod_cancel(1, req, alloc, U) == o.forget_pod(1, req, alloc, U) == 0
+    assert not o.known_pod(U) and not e.pod_known(U)
+    assert o.released_pod(U) and e.pod_released(U)
+    assert e.rows(0) == o.rows(0) and e.rows(1) == o.rows(1)
+    g = int(np.log2(got["alloc_mask"][0][0]))
+    assert e.pod_cancel(0, req, [[g]], U) == o.forget_pod(0, req, [[g]], U) == 0
+    assert e.rows(0) == o.rows(0) == [(60, 10), (100, 16)] and e.rows(1) == o.rows(1)
+    e.close()
+
+
 def test_accounting_verbs_take_pods_with_up_to_8_containers():
     """A pod with sidecars (6 containers: 4 without GPU request = {-1,-1} sentinel units, gpu.go:9-13 / allocate.go:41-45)
     that ANOTHER scheduler placed must be subtracted from the node cache exactly like the reference does (AddPod,
