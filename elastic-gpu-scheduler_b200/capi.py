@@ -11,6 +11,7 @@ import numpy as np
 from . import _build
 
 EGS_MAX_GPUS = 8
+EGS_MAX_GPUS_WIDE = 16
 EGS_MAX_CONTAINERS = 4
 EGS_BINPACK, EGS_SPREAD = 0, 1
 (EGS_OK, EGS_ERR_NOFIT, EGS_ERR_NO_OPTION, EGS_ERR_TRANSACT, EGS_ERR_BAD_ARG, EGS_ERR_OVERFLOW_GUARD,
@@ -18,6 +19,16 @@ EGS_BINPACK, EGS_SPREAD = 0, 1
 EGS_MODE_AUTO, EGS_MODE_RESCAN, EGS_MODE_ROUNDS = 0, 1, 2
 EGS_K_EVALUATE, EGS_K_PASS, EGS_K_SELECT, EGS_K_RESOLVE = 0, 1, 2, 3
 EGS_PAD = -(1 << 31)
+
+
+def row_width(g_max: int) -> int:
+    """EGS_ROW_WIDTH: int32 cells per node row of a handle created with `g_max`."""
+    return EGS_MAX_GPUS_WIDE if g_max > EGS_MAX_GPUS else EGS_MAX_GPUS
+
+
+def mask_dtype(g_max: int):
+    """One GPU mask of a handle created with `g_max` (EGS_MASK_BYTES little-endian bytes)."""
+    return np.dtype("<u2") if g_max > EGS_MAX_GPUS else np.dtype(np.uint8)
 
 # every symbol include/egs.h declares
 SYMBOLS = [
@@ -130,7 +141,7 @@ def units_array(req: Sequence[Tuple[int, int, int]]) -> np.ndarray:
 
 
 def masks_to_lists(masks, n_containers: int):
-    return [[g for g in range(8) if (int(masks[c]) >> g) & 1] for c in range(n_containers)]
+    return [[g for g in range(EGS_MAX_GPUS_WIDE) if (int(masks[c]) >> g) & 1] for c in range(n_containers)]
 
 
 def _alloc_arrays(alloc):
@@ -151,6 +162,7 @@ class Egs:
         if st != EGS_OK:
             raise EgsError(st, "egs_create", "(is a CUDA device visible?)")
         self.max_nodes, self.g_max, self.policy = max_nodes, g_max, policy
+        self.row_w, self.mask_dtype = row_width(g_max), mask_dtype(g_max)
 
     def close(self):
         if getattr(self, "h", None):
@@ -185,7 +197,7 @@ class Egs:
 
     def state_dump(self, node0: int = 0, n: Optional[int] = None):
         n = self.max_nodes - node0 if n is None else n
-        core = np.zeros((n, 8), np.int32); mem = np.zeros((n, 8), np.int32)
+        core = np.zeros((n, self.row_w), np.int32); mem = np.zeros((n, self.row_w), np.int32)
         gc = np.zeros(n, np.int32); mt = np.zeros(n, np.int32)
         self._ck(self.L.egs_state_dump(self.h, node0, n, _p(core), _p(mem), _p(gc), _p(mt)), "egs_state_dump")
         return core, mem, gc, mt
@@ -218,13 +230,13 @@ class Egs:
         return st, out[:n]
 
     def bind(self, node: int, req, uid: int):
-        masks = np.zeros(4, np.uint8)
+        masks = np.zeros(4, self.mask_dtype)
         st = self.L.egs_bind(self.h, node, len(req), _p(units_array(req)), uid, _p(masks))
         return st, (masks_to_lists(masks, len(req)) if st == EGS_OK else None)
 
     def peek(self, node: int, req):
         valid, score = C.c_int32(0), C.c_int32(0)
-        masks = np.zeros(4, np.uint8)
+        masks = np.zeros(4, self.mask_dtype)
         self._ck(self.L.egs_option_peek(self.h, node, len(req), _p(units_array(req)), C.byref(valid),
                                         C.byref(score), _p(masks)), "egs_option_peek")
         if not valid.value:
@@ -232,9 +244,10 @@ class Egs:
         return masks_to_lists(masks, len(req)), score.value
 
     def option_dump(self, req, node0: int = 0, n: Optional[int] = None):
-        """Option cache of request `req` on nodes [node0, node0+n): (state u8, score i32, alloc_mask u8[n,4])."""
+        """Option cache of request `req` on nodes [node0, node0+n): (state u8, score i32, alloc_mask [n,4] of
+        mask_dtype: u8, or u16 on a wide handle)."""
         n = self.max_nodes - node0 if n is None else n
-        st = np.zeros(max(n, 1), np.uint8); sc = np.zeros(max(n, 1), np.int32); am = np.zeros((max(n, 1), 4), np.uint8)
+        st = np.zeros(max(n, 1), np.uint8); sc = np.zeros(max(n, 1), np.int32); am = np.zeros((max(n, 1), 4), self.mask_dtype)
         self._ck(self.L.egs_option_dump(self.h, len(req), _p(units_array(req)), node0, n, _p(st), _p(sc), _p(am)),
                  "egs_option_dump")
         return st[:n], sc[:n], am[:n]
@@ -256,7 +269,7 @@ class Egs:
         c_off = np.ascontiguousarray(c_off, np.int32); units = np.ascontiguousarray(units, np.int32)
         at = np.ascontiguousarray(mut_at, np.int32); a = mutations_array(records)
         out = dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
-                   alloc_mask=np.zeros((P, 4), np.uint8), fit_count=np.zeros(P, np.int32),
+                   alloc_mask=np.zeros((P, 4), self.mask_dtype), fit_count=np.zeros(P, np.int32),
                    fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
         u = None if uids is None else np.ascontiguousarray(uids, np.uint64)
         self._ck(self.L.egs_schedule_batch_mut(self.h, mode, P, _p(c_off), _p(units), _p(u), len(records), _p(at), _p(a),
@@ -277,7 +290,7 @@ class Egs:
         c_off = np.ascontiguousarray(c_off, np.int32)
         units = np.ascontiguousarray(units, np.int32)
         out = dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
-                   alloc_mask=np.zeros((P, 4), np.uint8), fit_count=np.zeros(P, np.int32),
+                   alloc_mask=np.zeros((P, 4), self.mask_dtype), fit_count=np.zeros(P, np.int32),
                    fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
         u = None if uids is None else np.ascontiguousarray(uids, np.uint64)
         self._ck(self.L.egs_schedule_batch(self.h, mode, P, _p(c_off), _p(units), _p(u), _p(out["node"]),
@@ -292,7 +305,7 @@ class Egs:
         units = np.ascontiguousarray(units, np.int32)
         vec_pods = min(vec_pods, P)
         out = dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
-                   alloc_mask=np.zeros((P, 4), np.uint8), fit_count=np.zeros(P, np.int32),
+                   alloc_mask=np.zeros((P, 4), self.mask_dtype), fit_count=np.zeros(P, np.int32),
                    fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64),
                    vec_fit=np.zeros((max(vec_pods, 1), self.max_nodes), np.uint8),
                    vec_score=np.zeros((max(vec_pods, 1), self.max_nodes), np.int32))

@@ -8,6 +8,7 @@
 #include <algorithm>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <unordered_set>
 #include <vector>
@@ -27,6 +28,7 @@ struct PendingBatch {           // results of a batch whose uid bookkeeping is a
 
 struct egs_handle {
   int policy = 0, max_nodes = 0, n_pad = 0, g_max = 0, device = 0, n_sm = 0;
+  int row_w = EGS_G, mask_b = 1;          // EGS_ROW_WIDTH(g_max), EGS_MASK_BYTES(g_max)
   int rank = 0, world = 1, lo = 0, hi = 0;
   cudaStream_t stream = nullptr;
   int32_t *d_core = nullptr, *d_mem = nullptr, *d_mem_total = nullptr;
@@ -56,7 +58,7 @@ struct egs_handle {
   // batch outputs
   int32_t *d_o_node = nullptr, *d_o_status = nullptr, *d_o_fit = nullptr; uint8_t *d_o_alloc = nullptr;
   unsigned long long *d_o_fd = nullptr, *d_o_sd = nullptr; int out_cap = 0;
-  ApplyOp *d_ops = nullptr; int32_t *d_group_off = nullptr; size_t ops_cap = 0;   // egs_mutations_apply
+  void *d_ops = nullptr; int32_t *d_group_off = nullptr; size_t ops_cap = 0;   // egs_mutations_apply: ApplyOp<row_w>[]
   uint8_t *d_vec_fit = nullptr; int32_t *d_vec_score = nullptr; size_t vec_cap = 0; int vec_pods = 0;   // egs_schedule_batch_vec
   // profiling
   int64_t k_launches[EGS_K_COUNT] = {0}; double k_ms[EGS_K_COUNT] = {0}; int timing = 0;
@@ -77,6 +79,20 @@ struct egs_handle {
 
 static int fail(egs_handle *h, int code, const char *msg) { h->err = msg; return code; }
 
+// The one place the row width picks a kernel instantiation: f(std::integral_constant<int, G>()) with G the handle's
+// row width, 8 or 16.
+template <class F>
+static int by_width(const egs_handle *h, F &&f) {
+  return h->row_w == 16 ? f(std::integral_constant<int, 16>()) : f(std::integral_constant<int, EGS_G>());
+}
+static bool is_wide(const egs_handle *h) { return h->row_w > EGS_G; }
+
+// Packed option masks (container c at bits [G*c, G*c + G)) -> EGS_MAX_CONTAINERS little-endian masks of mask_b bytes.
+static void put_masks(const egs_handle *h, uint64_t masks, uint8_t *out) {
+  for (int c = 0; c < EGS_C; c++)
+    for (int b = 0; b < h->mask_b; b++) out[c * h->mask_b + b] = (uint8_t)(masks >> (h->row_w * c + 8 * b));
+}
+
 static int ensure_stage(egs_handle *h, size_t bytes) {
   if (bytes <= h->h_stage_cap) return EGS_OK;
   if (h->h_stage) cudaFreeHost(h->h_stage);
@@ -92,7 +108,7 @@ static OptTable table(egs_handle *h, int slot) {
   t.plane = (size_t)h->n_pad;
   t.st = h->d_st + (size_t)slot * h->n_pad;
   t.sc = h->d_sc + (size_t)slot * h->n_pad;
-  t.al = h->d_al + (size_t)slot * EGS_C * h->n_pad;
+  t.al = h->d_al + (size_t)slot * EGS_C * h->n_pad * h->mask_b;
   return t;
 }
 
@@ -100,15 +116,15 @@ static int grow_slots(egs_handle *h, int need) {
   if (need <= h->slot_cap) return EGS_OK;
   int cap = std::max(need, std::max(16, h->slot_cap * 2));
   uint8_t *st; int32_t *sc; uint8_t *al;
-  size_t np = (size_t)h->n_pad;
+  size_t np = (size_t)h->n_pad, al_plane = np * EGS_C * h->mask_b;
   CK(h, cudaMalloc(&st, np * cap));
   CK(h, cudaMalloc(&sc, np * cap * sizeof(int32_t)));
-  CK(h, cudaMalloc(&al, np * cap * EGS_C));
+  CK(h, cudaMalloc(&al, al_plane * cap));
   CK(h, cudaMemsetAsync(st, OPT_ABSENT, np * cap, h->stream));
   if (h->slot_cap) {
     CK(h, cudaMemcpyAsync(st, h->d_st, np * h->slot_cap, cudaMemcpyDeviceToDevice, h->stream));
     CK(h, cudaMemcpyAsync(sc, h->d_sc, np * h->slot_cap * sizeof(int32_t), cudaMemcpyDeviceToDevice, h->stream));
-    CK(h, cudaMemcpyAsync(al, h->d_al, np * h->slot_cap * EGS_C, cudaMemcpyDeviceToDevice, h->stream));
+    CK(h, cudaMemcpyAsync(al, h->d_al, al_plane * h->slot_cap, cudaMemcpyDeviceToDevice, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
     cudaFree(h->d_st); cudaFree(h->d_sc); cudaFree(h->d_al);
   }
@@ -215,12 +231,13 @@ static int pin_get(egs_handle *h, size_t n, PinBuf *out) {
 
 // ------------------------------------------------------------------------------- lifecycle
 extern "C" int egs_create(int policy, int max_nodes, int g_max, int device, egs_handle **out) {
-  if (!out || max_nodes < 1 || g_max < 1 || g_max > EGS_G || (policy != EGS_BINPACK && policy != EGS_SPREAD))
+  if (!out || max_nodes < 1 || g_max < 1 || g_max > EGS_MAX_GPUS_WIDE || (policy != EGS_BINPACK && policy != EGS_SPREAD))
     return EGS_ERR_BAD_ARG;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1 || device < 0 || device >= ndev) return EGS_ERR_CUDA;
   egs_handle *h = new egs_handle();
   h->policy = policy; h->max_nodes = max_nodes; h->g_max = g_max; h->device = device;
+  h->row_w = EGS_ROW_WIDTH(g_max); h->mask_b = EGS_MASK_BYTES(g_max);
   h->n_pad = (max_nodes + 1023) / 1024 * 1024;
   h->lo = 0; h->hi = max_nodes;
   h->h_gpu_count.assign(max_nodes, 0); h->h_mem_total.assign(max_nodes, 0);
@@ -228,13 +245,13 @@ extern "C" int egs_create(int policy, int max_nodes, int g_max, int device, egs_
     CK(h, cudaSetDevice(device));
     CK(h, cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device));
     CK(h, cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    size_t rows = (size_t)h->n_pad * EGS_G * sizeof(int32_t);
+    size_t rows = (size_t)h->n_pad * h->row_w * sizeof(int32_t);
     CK(h, cudaMalloc(&h->d_core, rows));
     CK(h, cudaMalloc(&h->d_mem, rows));
     CK(h, cudaMalloc(&h->d_mem_total, (size_t)h->n_pad * sizeof(int32_t)));
     CK(h, cudaMemsetAsync(h->d_mem_total, 0, (size_t)h->n_pad * sizeof(int32_t), h->stream));
     // EGS_PAD == 0x80000000: fill through a pinned pattern-free path (memset is per byte)
-    std::vector<int32_t> pad((size_t)h->n_pad * EGS_G, EGS_PAD);
+    std::vector<int32_t> pad((size_t)h->n_pad * h->row_w, EGS_PAD);
     CK(h, cudaMemcpy(h->d_core, pad.data(), rows, cudaMemcpyHostToDevice));
     CK(h, cudaMemcpy(h->d_mem, pad.data(), rows, cudaMemcpyHostToDevice));
     int nblk = (h->n_pad + PASS_THREADS - 1) / PASS_THREADS;
@@ -322,25 +339,26 @@ static int load_rows(egs_handle *h, int node0, int n, int gpu_count, int mem_tot
   if (node0 < 0 || n < 0 || node0 + n > h->max_nodes || gpu_count < 1 || gpu_count > h->g_max) return EGS_ERR_BAD_ARG;
   if (mem_total < 0 || mem_total > EGS_MAX_MEM_PER_GPU) return EGS_ERR_OVERFLOW_GUARD;
   if (n == 0) return EGS_OK;
-  size_t cells = (size_t)n * EGS_G;
+  const int W = h->row_w;
+  size_t cells = (size_t)n * W;
   TRY(ensure_stage(h, cells * 2 * sizeof(int32_t) + (size_t)n * sizeof(int32_t)));
   CK(h, cudaStreamSynchronize(h->stream));   // staging buffer reuse
   int32_t *sc = (int32_t *)h->h_stage, *sm = sc + cells, *st = sm + cells;
   for (int i = 0; i < n; i++) {
-    for (int g = 0; g < EGS_G; g++) {
+    for (int g = 0; g < W; g++) {
       int32_t cv = EGS_PAD, mv = EGS_PAD;
       if (g < gpu_count) {
         cv = core ? core[(size_t)i * gpu_count + g] : EGS_CORE_PER_GPU;
         mv = mem ? mem[(size_t)i * gpu_count + g] : mem_total;
         if (cv < 0 || cv > EGS_MAX_CORE_LOAD || mv < 0 || mv > EGS_MAX_MEM_PER_GPU) return EGS_ERR_OVERFLOW_GUARD;
       }
-      sc[(size_t)i * EGS_G + g] = cv; sm[(size_t)i * EGS_G + g] = mv;
+      sc[(size_t)i * W + g] = cv; sm[(size_t)i * W + g] = mv;
     }
     st[i] = mem_total;
     h->h_gpu_count[node0 + i] = gpu_count; h->h_mem_total[node0 + i] = mem_total;
   }
-  CK(h, cudaMemcpyAsync(h->d_core + (size_t)node0 * EGS_G, sc, cells * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
-  CK(h, cudaMemcpyAsync(h->d_mem + (size_t)node0 * EGS_G, sm, cells * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+  CK(h, cudaMemcpyAsync(h->d_core + (size_t)node0 * W, sc, cells * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+  CK(h, cudaMemcpyAsync(h->d_mem + (size_t)node0 * W, sm, cells * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
   CK(h, cudaMemcpyAsync(h->d_mem_total + node0, st, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
   TRY(reset_nodes(h, node0, n, fresh ? 1 : 0));
   if (fresh && node0 == 0 && n >= h->max_nodes) std::fill(h->slot_cold.begin(), h->slot_cold.end(), 1);
@@ -400,11 +418,11 @@ extern "C" int egs_state_dump(egs_handle *h, int node0, int n, int32_t *free_cor
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
   if (node0 < 0 || n < 0 || node0 + n > h->max_nodes) return EGS_ERR_BAD_ARG;
-  size_t cells = (size_t)n * EGS_G;
+  size_t cells = (size_t)n * h->row_w;
   TRY(ensure_stage(h, cells * 2 * sizeof(int32_t)));
   int32_t *sc = (int32_t *)h->h_stage, *sm = sc + cells;
-  CK(h, cudaMemcpyAsync(sc, h->d_core + (size_t)node0 * EGS_G, cells * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
-  CK(h, cudaMemcpyAsync(sm, h->d_mem + (size_t)node0 * EGS_G, cells * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+  CK(h, cudaMemcpyAsync(sc, h->d_core + (size_t)node0 * h->row_w, cells * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+  CK(h, cudaMemcpyAsync(sm, h->d_mem + (size_t)node0 * h->row_w, cells * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaStreamSynchronize(h->stream));
   if (free_core) memcpy(free_core, sc, cells * sizeof(int32_t));
   if (free_mem) memcpy(free_mem, sm, cells * sizeof(int32_t));
@@ -418,7 +436,7 @@ extern "C" int egs_state_dump(egs_handle *h, int node0, int n, int32_t *free_cor
 extern "C" int egs_state_snapshot(egs_handle *h) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  const size_t rows = (size_t)h->n_pad * EGS_G * sizeof(int32_t);
+  const size_t rows = (size_t)h->n_pad * h->row_w * sizeof(int32_t);
   if (!h->d_snap_core) {
     CK(h, cudaMalloc(&h->d_snap_core, rows));
     CK(h, cudaMalloc(&h->d_snap_mem, rows));
@@ -437,7 +455,7 @@ extern "C" int egs_state_restore(egs_handle *h) {
   Guard g(h);
   if (!h->d_snap_core) return fail(h, EGS_ERR_BAD_ARG, "no snapshot");
   TRY(discard_pending(h));
-  const size_t rows = (size_t)h->n_pad * EGS_G * sizeof(int32_t);
+  const size_t rows = (size_t)h->n_pad * h->row_w * sizeof(int32_t);
   CK(h, cudaMemcpyAsync(h->d_core, h->d_snap_core, rows, cudaMemcpyDeviceToDevice, h->stream));
   CK(h, cudaMemcpyAsync(h->d_mem, h->d_snap_mem, rows, cudaMemcpyDeviceToDevice, h->stream));
   CK(h, cudaMemcpyAsync(h->d_mem_total, h->d_snap_total, (size_t)h->n_pad * sizeof(int32_t), cudaMemcpyDeviceToDevice, h->stream));
@@ -485,7 +503,11 @@ static int gather(egs_handle *h, bool score, int n, const int32_t *node_ids, int
   const int grid = (n + 255) / 256;
   if (score) {
     CK(h, cudaMemsetAsync(h->d_result + 8, 0, sizeof(int32_t), h->stream));
-    if (single) k_gather_score<true><<<grid, 256, 0, h->stream>>>(a); else k_gather_score<false><<<grid, 256, 0, h->stream>>>(a);
+    by_width(h, [&](auto W) -> int {
+      constexpr int G = decltype(W)::value;
+      if (single) k_gather_score<G, true><<<grid, 256, 0, h->stream>>>(a); else k_gather_score<G, false><<<grid, 256, 0, h->stream>>>(a);
+      return EGS_OK;
+    });
     CK(h, cudaGetLastError());
     CK(h, cudaMemcpyAsync(h->h_stage, h->d_score, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaMemcpyAsync(h->h_result, h->d_result + 8, sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
@@ -493,7 +515,11 @@ static int gather(egs_handle *h, bool score, int n, const int32_t *node_ids, int
     memcpy(out_score, h->h_stage, (size_t)n * sizeof(int32_t));
     return h->h_result[0] ? EGS_ERR_PANIC : EGS_OK;
   }
-  if (single) k_gather_filter<true><<<grid, 256, 0, h->stream>>>(a); else k_gather_filter<false><<<grid, 256, 0, h->stream>>>(a);
+  by_width(h, [&](auto W) -> int {
+    constexpr int G = decltype(W)::value;
+    if (single) k_gather_filter<G, true><<<grid, 256, 0, h->stream>>>(a); else k_gather_filter<G, false><<<grid, 256, 0, h->stream>>>(a);
+    return EGS_OK;
+  });
   CK(h, cudaGetLastError());
   CK(h, cudaMemcpyAsync(h->h_stage, h->d_fit, (size_t)n, cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaStreamSynchronize(h->stream));
@@ -514,8 +540,9 @@ extern "C" int egs_score(egs_handle *h, int n, const int32_t *node_ids, int n_co
   return gather(h, true, n, node_ids, n_containers, units, nullptr, out_score);
 }
 
+// res[0] had entry, res[1] status, res[2] score; *masks the option's packed masks
 static int bind_or_peek(egs_handle *h, int consume, int node_id, int C, const egs_unit *units, uint64_t uid,
-                        int32_t *res4) {
+                        int32_t *res, uint64_t *masks) {
   if (node_id < 0 || node_id >= h->max_nodes) return EGS_ERR_BAD_ARG;
   if (h->h_gpu_count[node_id] == 0) return EGS_ERR_NO_NODE;
   int slot;
@@ -527,12 +554,18 @@ static int bind_or_peek(egs_handle *h, int consume, int node_id, int C, const eg
   a.all_st = h->d_st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
   const bool known = consume && h->book.in_pods_map(node_id, uid);
   a.skip_transact = known ? 1 : 0; a.consume = consume; a.result = h->d_result;
-  k_bind<<<1, 1, 0, h->stream>>>(a);
+  by_width(h, [&](auto W) -> int {
+    constexpr int G = decltype(W)::value;
+    k_bind<G><<<1, 1, 0, h->stream>>>(a);
+    return EGS_OK;
+  });
   CK(h, cudaGetLastError());
-  CK(h, cudaMemcpyAsync(h->h_result, h->d_result, 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+  CK(h, cudaMemcpyAsync(h->h_result, h->d_result, 5 * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaStreamSynchronize(h->stream));
-  memcpy(res4, h->h_result, 4 * sizeof(int32_t));
-  if (consume) h->book.record_bind(node_id, uid, res4[0] != 0, known, res4[1]);
+  const int32_t *r = h->h_result;
+  res[0] = r[0]; res[1] = r[1]; res[2] = r[3];
+  *masks = (uint32_t)r[2] | (is_wide(h) ? (uint64_t)(uint32_t)r[4] << 32 : 0);
+  if (consume) h->book.record_bind(node_id, uid, res[0] != 0, known, res[1]);
   return EGS_OK;
 }
 
@@ -540,10 +573,9 @@ extern "C" int egs_bind(egs_handle *h, int node_id, int n_containers, const egs_
                         uint8_t *out_alloc_mask) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  int32_t r[4];
-  TRY(bind_or_peek(h, 1, node_id, n_containers, units, uid, r));
-  if (out_alloc_mask)
-    for (int c = 0; c < EGS_C; c++) out_alloc_mask[c] = r[1] == EGS_OK ? (uint8_t)((uint32_t)r[2] >> (8 * c)) : 0;
+  int32_t r[3]; uint64_t masks;
+  TRY(bind_or_peek(h, 1, node_id, n_containers, units, uid, r, &masks));
+  if (out_alloc_mask) put_masks(h, r[1] == EGS_OK ? masks : 0, out_alloc_mask);
   return r[1];
 }
 
@@ -551,11 +583,11 @@ extern "C" int egs_option_peek(egs_handle *h, int node_id, int n_containers, con
                                int32_t *out_valid, int32_t *out_score, uint8_t *out_alloc_mask) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  int32_t r[4];
-  TRY(bind_or_peek(h, 0, node_id, n_containers, units, 0, r));
+  int32_t r[3]; uint64_t masks;
+  TRY(bind_or_peek(h, 0, node_id, n_containers, units, 0, r, &masks));
   if (out_valid) *out_valid = r[0];
-  if (out_score) *out_score = r[3];
-  if (out_alloc_mask) for (int c = 0; c < EGS_C; c++) out_alloc_mask[c] = r[0] ? (uint8_t)((uint32_t)r[2] >> (8 * c)) : 0;
+  if (out_score) *out_score = r[2];
+  if (out_alloc_mask) put_masks(h, r[0] ? masks : 0, out_alloc_mask);
   return EGS_OK;
 }
 
@@ -568,44 +600,50 @@ extern "C" int egs_option_dump(egs_handle *h, int n_containers, const egs_unit *
   TRY(intern(h, n_containers, units, &slot));
   if (n == 0) return EGS_OK;
   const OptTable t = table(h, slot);
-  const size_t sn = (size_t)n;
-  TRY(ensure_stage(h, sn * (1 + 4 + EGS_C)));
+  const size_t sn = (size_t)n, mb = (size_t)h->mask_b;
+  TRY(ensure_stage(h, sn * (1 + 4 + EGS_C * mb)));
   CK(h, cudaStreamSynchronize(h->stream));
   char *s = (char *)h->h_stage;
   int32_t *hs = (int32_t *)s; uint8_t *hst = (uint8_t *)(hs + sn); uint8_t *hal = hst + sn;
   CK(h, cudaMemcpyAsync(hs, t.sc + node0, 4 * sn, cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaMemcpyAsync(hst, t.st + node0, sn, cudaMemcpyDeviceToHost, h->stream));
   for (int c = 0; c < EGS_C; c++)
-    CK(h, cudaMemcpyAsync(hal + (size_t)c * sn, t.al + (size_t)c * t.plane + node0, sn, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaMemcpyAsync(hal + (size_t)c * sn * mb, t.al + ((size_t)c * t.plane + node0) * mb, sn * mb, cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaStreamSynchronize(h->stream));
   for (size_t i = 0; i < sn; i++) {
     const bool cached = hst[i] == OPT_CACHED;
     if (out_state) out_state[i] = hst[i] == OPT_CACHED ? 1 : hst[i] == OPT_UNFIT ? 2 : 0;
     if (out_score) out_score[i] = cached ? hs[i] : 0;
-    if (out_alloc_mask) for (int c = 0; c < EGS_C; c++) out_alloc_mask[i * EGS_C + c] = (cached && c < n_containers) ? hal[(size_t)c * sn + i] : 0;
+    if (out_alloc_mask)
+      for (int c = 0; c < EGS_C; c++)
+        for (size_t b = 0; b < mb; b++)
+          out_alloc_mask[(i * EGS_C + c) * mb + b] = (cached && c < n_containers) ? hal[((size_t)c * sn + i) * mb + b] : 0;
   }
   return EGS_OK;
 }
 
 static int apply_lists(egs_handle *h, int cancel, int node_id, int C, const egs_unit *units,
                        const int32_t *alloc_off, const int32_t *alloc_idx) {
-  ApplyArgs a; memset(&a, 0, sizeof a);
-  a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total;
-  a.op.node = node_id; a.op.cancel = cancel; a.op.req = make_req<ReqW>(C, units);
-  a.all_st = h->d_st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
-  for (int c = 0; c < C; c++) {
-    int n = alloc_off ? alloc_off[c + 1] - alloc_off[c] : 0;
-    if (n < 0 || n > EGS_G || (n > 0 && !alloc_idx)) return EGS_ERR_BAD_ARG;
-    a.op.n_idx[c] = n;
-    for (int j = 0; j < n; j++) {
-      int v = alloc_idx[alloc_off[c] + j];
-      if (v < 0 || v >= h->h_gpu_count[node_id]) return EGS_ERR_BAD_ARG;   // the reference would panic
-      a.op.idx[c][j] = (int8_t)v;
+  return by_width(h, [&](auto W) -> int {
+    constexpr int G = decltype(W)::value;
+    ApplyArgs<G> a; memset(&a, 0, sizeof a);
+    a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total;
+    a.op.node = node_id; a.op.cancel = cancel; a.op.req = make_req<ReqW>(C, units);
+    a.all_st = h->d_st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
+    for (int c = 0; c < C; c++) {
+      int n = alloc_off ? alloc_off[c + 1] - alloc_off[c] : 0;
+      if (n < 0 || n > G || (n > 0 && !alloc_idx)) return EGS_ERR_BAD_ARG;
+      a.op.n_idx[c] = n;
+      for (int j = 0; j < n; j++) {
+        int v = alloc_idx[alloc_off[c] + j];
+        if (v < 0 || v >= h->h_gpu_count[node_id]) return EGS_ERR_BAD_ARG;   // the reference would panic
+        a.op.idx[c][j] = (int8_t)v;
+      }
     }
-  }
-  k_apply<<<1, 1, 0, h->stream>>>(a);
-  CK(h, cudaGetLastError());
-  return EGS_OK;
+    k_apply<G><<<1, 1, 0, h->stream>>>(a);
+    CK(h, cudaGetLastError());
+    return EGS_OK;
+  });
 }
 
 // AddPod scheduler.go:229-245
@@ -651,6 +689,7 @@ extern "C" int egs_pod_cancel(egs_handle *h, int node_id, int n_containers, cons
 
 // ------------------------------------------------------------------------------- mutation stream
 // caller holds the lock; pending batch bookkeeping already flushed
+template <int G> static int mutations_rows(egs_handle *h, int n, const egs_mutation *ops);
 static int mutations_apply_locked(egs_handle *h, int n, const egs_mutation *ops) {
   if (n < 0 || (n > 0 && !ops)) return EGS_ERR_BAD_ARG;
   if (n == 0) return EGS_OK;
@@ -663,16 +702,23 @@ static int mutations_apply_locked(egs_handle *h, int n, const egs_mutation *ops)
     if (h->h_gpu_count[m.node_id] == 0) return EGS_ERR_NO_NODE;
     TRY(check_units(m.n_containers, m.units, EGS_MAX_CONTAINERS_APPLY));
     for (int c = 0; c < m.n_containers; c++) {
-      if (m.n_idx[c] < 0 || m.n_idx[c] > EGS_G) return EGS_ERR_BAD_ARG;
+      if (m.n_idx[c] < 0 || m.n_idx[c] > EGS_MAX_GPUS) return fail(h, EGS_ERR_BAD_ARG, "a mutation record holds at most EGS_MAX_GPUS indices per container");
       for (int j = 0; j < m.n_idx[c]; j++) if (m.idx[c][j] < 0 || m.idx[c][j] >= h->h_gpu_count[m.node_id]) return EGS_ERR_BAD_ARG;
     }
   }
+  return by_width(h, [&](auto W) -> int { return mutations_rows<decltype(W)::value>(h, n, ops); });
+}
+
+// passes 2 and 3 of mutations_apply_locked on a handle of row width G
+template <int G>
+static int mutations_rows(egs_handle *h, int n, const egs_mutation *ops) {
+  typedef ApplyOp<G> Op;
   // pass 2: the podsMap / podMaps decisions in record order; the surviving row updates are collected
-  std::vector<ApplyOp> dev; dev.reserve((size_t)n);
+  std::vector<Op> dev; dev.reserve((size_t)n);
   for (int i = 0; i < n; i++) {
     const egs_mutation &m = ops[i];
     TRY(h->book.account(m.kind, m.node_id, m.uid, [&](int cancel) {
-      ApplyOp o; memset(&o, 0, sizeof o);
+      Op o; memset(&o, 0, sizeof o);
       o.node = m.node_id; o.cancel = cancel; o.req = make_req<ReqW>(m.n_containers, m.units);
       for (int c = 0; c < m.n_containers; c++) { o.n_idx[c] = m.n_idx[c]; for (int j = 0; j < m.n_idx[c]; j++) o.idx[c][j] = m.idx[c][j]; }
       dev.push_back(o);
@@ -685,9 +731,9 @@ static int mutations_apply_locked(egs_handle *h, int n, const egs_mutation *ops)
   for (size_t i = 0; i < order.size(); i++) order[i] = (int)i;
   std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return dev[x].node < dev[y].node; });
   const size_t nd = dev.size();
-  TRY(ensure_stage(h, nd * sizeof(ApplyOp) + (nd + 1) * sizeof(int32_t)));
+  TRY(ensure_stage(h, nd * sizeof(Op) + (nd + 1) * sizeof(int32_t)));
   CK(h, cudaStreamSynchronize(h->stream));
-  ApplyOp *so = (ApplyOp *)h->h_stage; int32_t *sg = (int32_t *)(so + nd);
+  Op *so = (Op *)h->h_stage; int32_t *sg = (int32_t *)(so + nd);
   int ng = 0;
   for (size_t i = 0; i < nd; i++) {
     so[i] = dev[order[i]];
@@ -697,16 +743,16 @@ static int mutations_apply_locked(egs_handle *h, int n, const egs_mutation *ops)
   if (nd > h->ops_cap) {
     if (h->d_ops) { cudaFree(h->d_ops); cudaFree(h->d_group_off); h->d_ops = nullptr; h->d_group_off = nullptr; h->ops_cap = 0; }
     const size_t cap = std::max(nd, (size_t)1024);
-    CK(h, cudaMalloc(&h->d_ops, cap * sizeof(ApplyOp)));
+    CK(h, cudaMalloc(&h->d_ops, cap * sizeof(Op)));
     CK(h, cudaMalloc(&h->d_group_off, (cap + 1) * sizeof(int32_t)));
     h->ops_cap = cap;
   }
-  CK(h, cudaMemcpyAsync(h->d_ops, so, nd * sizeof(ApplyOp), cudaMemcpyHostToDevice, h->stream));
+  CK(h, cudaMemcpyAsync(h->d_ops, so, nd * sizeof(Op), cudaMemcpyHostToDevice, h->stream));
   CK(h, cudaMemcpyAsync(h->d_group_off, sg, (size_t)(ng + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
-  ApplyManyArgs ka;
-  ka.core = h->d_core; ka.mem = h->d_mem; ka.mem_total = h->d_mem_total; ka.ops = h->d_ops; ka.group_off = h->d_group_off; ka.n_groups = ng;
+  ApplyManyArgs<G> ka;
+  ka.core = h->d_core; ka.mem = h->d_mem; ka.mem_total = h->d_mem_total; ka.ops = (const Op *)h->d_ops; ka.group_off = h->d_group_off; ka.n_groups = ng;
   ka.all_st = h->d_st; ka.slot_stride = (size_t)h->n_pad; ka.n_slots = (int)h->shapes.size();
-  k_apply_many<<<(ng + 127) / 128, 128, 0, h->stream>>>(ka);
+  k_apply_many<G><<<(ng + 127) / 128, 128, 0, h->stream>>>(ka);
   CK(h, cudaGetLastError());
   return EGS_OK;
 }
@@ -740,7 +786,7 @@ static int ensure_out(egs_handle *h, int P) {
   CK(h, cudaMalloc(&h->d_o_node, sizeof(int32_t) * (size_t)cap));
   CK(h, cudaMalloc(&h->d_o_status, sizeof(int32_t) * (size_t)cap));
   CK(h, cudaMalloc(&h->d_o_fit, sizeof(int32_t) * (size_t)cap));
-  CK(h, cudaMalloc(&h->d_o_alloc, (size_t)cap * EGS_C));
+  CK(h, cudaMalloc(&h->d_o_alloc, (size_t)cap * EGS_C * h->mask_b));
   CK(h, cudaMalloc(&h->d_o_fd, sizeof(unsigned long long) * (size_t)cap));
   CK(h, cudaMalloc(&h->d_o_sd, sizeof(unsigned long long) * (size_t)cap));
   h->out_cap = cap;
@@ -763,8 +809,12 @@ static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_un
     a.vec_score = p < h->vec_pods ? h->d_vec_score + (size_t)p * h->max_nodes : nullptr;
     a.partials = h->d_partials; a.ticket = h->d_ticket;
     a.pod = p; a.out = out;
-    if (is_single(C, u)) k_pass<true><<<grid, PASS_THREADS, 0, h->stream>>>(a);
-    else k_pass<false><<<grid, PASS_THREADS, 0, h->stream>>>(a);
+    by_width(h, [&](auto W) -> int {
+      constexpr int G = decltype(W)::value;
+      if (is_single(C, u)) k_pass<G, true><<<grid, PASS_THREADS, 0, h->stream>>>(a);
+      else k_pass<G, false><<<grid, PASS_THREADS, 0, h->stream>>>(a);
+      return EGS_OK;
+    });
     if ((p & 1023) == 0) CK(h, cudaGetLastError());
   }
   CK(h, cudaGetLastError());
@@ -772,9 +822,16 @@ static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_un
   return EGS_OK;
 }
 
+// A wide handle has no rounds engine: EGS_MODE_ROUNDS is refused before the batch touches anything, and
+// EGS_MODE_AUTO runs the per-pod engine there.
+static int refuse_wide_rounds(egs_handle *h, int mode) {
+  return is_wide(h) && mode == EGS_MODE_ROUNDS ? fail(h, EGS_ERR_BAD_ARG, "EGS_MODE_ROUNDS needs g_max <= EGS_MAX_GPUS") : EGS_OK;
+}
+
 static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, const egs_unit *units,
                         const uint64_t *uids, PodOut out, bool device_out) {
   if (P < 0 || (P > 0 && (!c_off || !units))) return EGS_ERR_BAD_ARG;
+  TRY(refuse_wide_rounds(h, mode));
   if (P == 0) return EGS_OK;
   if (h->world > 1 && mode == EGS_MODE_RESCAN) return fail(h, EGS_ERR_BAD_ARG, "EGS_MODE_RESCAN is single-shard");
   std::vector<int> slots((size_t)P);
@@ -800,7 +857,7 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
     if (!dev.node) dev.node = h->d_o_node;          // uid bookkeeping needs node + status
     if (!dev.status) dev.status = h->d_o_status;
   }
-  if (mode == EGS_MODE_AUTO) mode = EGS_MODE_ROUNDS;
+  if (mode == EGS_MODE_AUTO) mode = is_wide(h) ? EGS_MODE_RESCAN : EGS_MODE_ROUNDS;
   int batch_rc = EGS_OK, n_done = P;
   if (mode == EGS_MODE_RESCAN) TRY(batch_rescan(h, P, c_off, units, slots, dev));
   else if (mode == EGS_MODE_ROUNDS) batch_rc = batch_rounds(h, P, c_off, units, slots, dev, &n_done);
@@ -823,7 +880,8 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
 
   if (!device_out) {
     size_t sp = (size_t)P;
-    TRY(ensure_stage(h, sp * (4 + 4 + 4 + EGS_C + 8 + 8)));
+    const size_t ab = (size_t)EGS_C * h->mask_b;   // alloc bytes per pod
+    TRY(ensure_stage(h, sp * (4 + 4 + 4 + ab + 8 + 8)));
     char *s = (char *)h->h_stage;
     int32_t *hn = (int32_t *)s, *hs = hn + sp, *hf = hs + sp;
     unsigned long long *hfd = (unsigned long long *)(hf + sp), *hsd = hfd + sp;
@@ -833,14 +891,14 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
     if (out.fit_count) CK(h, cudaMemcpyAsync(hf, dev.fit_count, 4 * sp, cudaMemcpyDeviceToHost, h->stream));
     if (out.fit_digest) CK(h, cudaMemcpyAsync(hfd, dev.fit_digest, 8 * sp, cudaMemcpyDeviceToHost, h->stream));
     if (out.score_digest) CK(h, cudaMemcpyAsync(hsd, dev.score_digest, 8 * sp, cudaMemcpyDeviceToHost, h->stream));
-    if (out.alloc) CK(h, cudaMemcpyAsync(ha, dev.alloc, EGS_C * sp, cudaMemcpyDeviceToHost, h->stream));
+    if (out.alloc) CK(h, cudaMemcpyAsync(ha, dev.alloc, ab * sp, cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaStreamSynchronize(h->stream));
     if (out.node) memcpy(out.node, hn, 4 * sp);
     if (out.status) memcpy(out.status, hs, 4 * sp);
     if (out.fit_count) memcpy(out.fit_count, hf, 4 * sp);
     if (out.fit_digest) memcpy(out.fit_digest, hfd, 8 * sp);
     if (out.score_digest) memcpy(out.score_digest, hsd, 8 * sp);
-    if (out.alloc) memcpy(out.alloc, ha, EGS_C * sp);
+    if (out.alloc) memcpy(out.alloc, ha, ab * sp);
   } else {
     CK(h, cudaStreamSynchronize(h->stream));
   }
@@ -866,6 +924,7 @@ extern "C" int egs_schedule_batch_mut(egs_handle *h, int mode, int n_pods, const
   for (int j = 0; j < n_mut; j++)
     if (mut_at[j] < 0 || mut_at[j] > n_pods || (j > 0 && mut_at[j] < mut_at[j - 1])) return EGS_ERR_BAD_ARG;
   Guard g(h);
+  TRY(refuse_wide_rounds(h, mode));                              // before the first record is applied
   // segments of pods between mutation points; the lock is held throughout, exactly one "call at a time"
   int p = 0, j = 0;
   while (p < n_pods || j < n_mut) {
@@ -880,7 +939,7 @@ extern "C" int egs_schedule_batch_mut(egs_handle *h, int mode, int n_pods, const
     const int q = j < n_mut ? mut_at[j] : n_pods;                // next mutation point (> p)
     PodOut o;
     o.node = out_node ? out_node + p : nullptr; o.status = out_status ? out_status + p : nullptr;
-    o.alloc = out_alloc_mask ? out_alloc_mask + (size_t)p * EGS_C : nullptr; o.fit_count = out_fit_count ? out_fit_count + p : nullptr;
+    o.alloc = out_alloc_mask ? out_alloc_mask + (size_t)p * EGS_C * h->mask_b : nullptr; o.fit_count = out_fit_count ? out_fit_count + p : nullptr;
     o.fit_digest = out_fit_digest ? (unsigned long long *)out_fit_digest + p : nullptr;
     o.score_digest = out_score_digest ? (unsigned long long *)out_score_digest + p : nullptr;
     // the segment's pods as a batch of its own: offsets rebased
@@ -926,6 +985,8 @@ extern "C" int egs_schedule_batch_device(egs_handle *h, int mode, int n_pods, co
                                          uint64_t *d_out_fit_digest, uint64_t *d_out_score_digest) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
+  if ((uintptr_t)d_out_alloc_mask % ((uintptr_t)EGS_C * h->mask_b))     // one packed word per pod (write_pod_out)
+    return fail(h, EGS_ERR_BAD_ARG, "d_out_alloc_mask must be aligned to EGS_MAX_CONTAINERS * EGS_MASK_BYTES(g_max)");
   PodOut o; o.node = d_out_node; o.status = d_out_status; o.alloc = d_out_alloc_mask; o.fit_count = d_out_fit_count;
   o.fit_digest = (unsigned long long *)d_out_fit_digest; o.score_digest = (unsigned long long *)d_out_score_digest;
   return batch_common(h, mode, n_pods, h_c_off, h_units, nullptr, o, true);
@@ -943,6 +1004,7 @@ extern "C" int egs_shard_range(int max_nodes, int rank, int world, int *lo, int 
 extern "C" int egs_shard_set(egs_handle *h, int rank, int world) {
   if (!h || world < 1 || world > RD || rank < 0 || rank >= world) return EGS_ERR_BAD_ARG;
   Guard g(h);
+  if (is_wide(h)) return fail(h, EGS_ERR_BAD_ARG, "the sharded engine is the rounds engine: it needs g_max <= EGS_MAX_GPUS");
   h->rank = rank; h->world = world;
   egs_shard_range(h->max_nodes, rank, world, &h->lo, &h->hi);
   return EGS_OK;
@@ -965,7 +1027,7 @@ extern "C" int egs_profile_evaluate(egs_handle *h, int n_containers, const egs_u
   if (!h->d_ev_fit) {
     CK(h, cudaMalloc(&h->d_ev_fit, np));
     CK(h, cudaMalloc(&h->d_ev_score, np * sizeof(int32_t)));
-    CK(h, cudaMalloc(&h->d_ev_gpu, np * EGS_C));
+    CK(h, cudaMalloc(&h->d_ev_gpu, np * EGS_C * h->mask_b));
   }
   const size_t flush_bytes = (size_t)256 << 20;
   if (flush_l2 && !h->d_flush) CK(h, cudaMalloc(&h->d_flush, flush_bytes));
@@ -977,15 +1039,21 @@ extern "C" int egs_profile_evaluate(egs_handle *h, int n_containers, const egs_u
   int items = 2;                                  // nodes per thread (tuning knob for experiments)
   if (const char *ev = getenv("EGS_EVAL_ITEMS")) items = atoi(ev);
   if (items != 1 && items != 2 && items != 4) items = 2;
+  if (is_wide(h)) items = 1;                      // a 16-wide row already keeps 8 loads of 16 B in flight per thread
   const int grid = (h->max_nodes + 256 * items - 1) / (256 * items);
   auto launch = [&]() {
-    if (single) {
-      if (items == 1) k_evaluate<true, 1><<<grid, 256, 0, h->stream>>>(a);
-      else if (items == 2) k_evaluate<true, 2><<<grid, 256, 0, h->stream>>>(a);
-      else k_evaluate<true, 4><<<grid, 256, 0, h->stream>>>(a);
-    } else {
-      k_evaluate<false, 1><<<(h->max_nodes + 255) / 256, 256, 0, h->stream>>>(a);
-    }
+    by_width(h, [&](auto W) -> int {
+      constexpr int G = decltype(W)::value;
+      if (!single) k_evaluate<G, false, 1><<<(h->max_nodes + 255) / 256, 256, 0, h->stream>>>(a);
+      else if constexpr (G == EGS_G) {
+        if (items == 1) k_evaluate<G, true, 1><<<grid, 256, 0, h->stream>>>(a);
+        else if (items == 2) k_evaluate<G, true, 2><<<grid, 256, 0, h->stream>>>(a);
+        else k_evaluate<G, true, 4><<<grid, 256, 0, h->stream>>>(a);
+      } else {
+        k_evaluate<G, true, 1><<<grid, 256, 0, h->stream>>>(a);
+      }
+      return EGS_OK;
+    });
   };
   cudaEvent_t e0, e1;
   CK(h, cudaEventCreate(&e0)); CK(h, cudaEventCreate(&e1));

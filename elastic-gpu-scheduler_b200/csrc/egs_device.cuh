@@ -1,7 +1,8 @@
 // egs_device.cuh -- device-side GPU/GPUs arithmetic of the reference's L0 layer
 // (pkg/scheduler/{gpu,rater}.go) on the int32 SoA rows.  Pure integer work.
 //
-// A node's row is free_core[8], free_mem[8]; GPUs a node does not have hold
+// A node's row is free_core[G], free_mem[G] with G = EGS_ROW_WIDTH(g_max) (8, or 16 on a wide handle); GPUs a node
+// does not have hold
 // EGS_PAD in BOTH arrays.  EGS_PAD = INT32_MIN fails every CanAllocate test
 // (requests are >= -1, gpu.go:51-56) and is skipped by the Rate min/max scan,
 // so no per-node gpu_count has to be read on the hot path.
@@ -80,14 +81,30 @@ __host__ __device__ __forceinline__ uint64_t cand_key(int32_t score, uint32_t no
 __host__ __device__ __forceinline__ uint32_t key_node(uint64_t key) { return 0xFFFFFFFFu - (uint32_t)key; }
 __host__ __device__ __forceinline__ int32_t key_score(uint64_t key) { return (int32_t)(key >> 32); }
 
-// 2 x 16-byte read-only loads per array: one node's row (32 B core + 32 B mem).
+// Per row width G: the GPU mask of one container (Mask) and the masks of a pod's EGS_C containers packed into one
+// word (Packed: container k at bits [G*k, G*k + G)), and LG = log2(G) for the folded Trade keys.
+template <int G> struct RowWidth;
+template <> struct RowWidth<8> { typedef uint8_t Mask; typedef uint32_t Packed; static constexpr int LG = 3; };
+template <> struct RowWidth<16> { typedef uint16_t Mask; typedef uint64_t Packed; static constexpr int LG = 4; };
+template <int G> using MaskT = typename RowWidth<G>::Mask;
+template <int G> using PackedT = typename RowWidth<G>::Packed;
+
+// G/4 16-byte read-only loads per array: one node's row (4*G B core + 4*G B mem), all issued before any use.
+template <int G>
 __device__ __forceinline__ void load_row(const int32_t *__restrict__ core, const int32_t *__restrict__ mem,
-                                         size_t node, int (&c)[EGS_G], int (&m)[EGS_G]) {
-  const int4 *pc = reinterpret_cast<const int4 *>(core + node * EGS_G);
-  const int4 *pm = reinterpret_cast<const int4 *>(mem + node * EGS_G);
-  int4 c0 = __ldg(pc), c1 = __ldg(pc + 1), m0 = __ldg(pm), m1 = __ldg(pm + 1);
-  c[0] = c0.x; c[1] = c0.y; c[2] = c0.z; c[3] = c0.w; c[4] = c1.x; c[5] = c1.y; c[6] = c1.z; c[7] = c1.w;
-  m[0] = m0.x; m[1] = m0.y; m[2] = m0.z; m[3] = m0.w; m[4] = m1.x; m[5] = m1.y; m[6] = m1.z; m[7] = m1.w;
+                                         size_t node, int (&c)[G], int (&m)[G]) {
+  const int4 *pc = reinterpret_cast<const int4 *>(core + node * G);
+  const int4 *pm = reinterpret_cast<const int4 *>(mem + node * G);
+  int4 cv[G / 4], mv[G / 4];
+#pragma unroll
+  for (int q = 0; q < G / 4; q++) cv[q] = __ldg(pc + q);
+#pragma unroll
+  for (int q = 0; q < G / 4; q++) mv[q] = __ldg(pm + q);
+#pragma unroll
+  for (int q = 0; q < G / 4; q++) {
+    c[4 * q] = cv[q].x; c[4 * q + 1] = cv[q].y; c[4 * q + 2] = cv[q].z; c[4 * q + 3] = cv[q].w;
+    m[4 * q] = mv[q].x; m[4 * q + 1] = mv[q].y; m[4 * q + 2] = mv[q].z; m[4 * q + 3] = mv[q].w;
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -100,40 +117,44 @@ __device__ __forceinline__ void load_row(const int32_t *__restrict__ core, const
 //   * PAD (0x80000000) is the largest UNSIGNED and the smallest SIGNED value: an unsigned min
 //     and a signed max both ignore absent GPUs without any select (valid rows are >= 0).
 //   * score = Range/(1+1)*100 with Range = x/2, x >= 0  ==  (x >> 2) * 100        (rater.go:49-50)
-//   * candidates are folded as key = q*8 + g: one max keeps the last maximal GPU.
+//   * candidates are folded as key = q*G + g: one max keeps the last maximal GPU.  q = x >> 2 with
+//     x <= 2*(EGS_MAX_MEM_PER_GPU + EGS_MAX_CORE_LOAD) < 2^26.1, so q < 2^24.1 and the largest key,
+//     q*16 + 15, stays below 2^28: no int32 overflow at G = 16 under the load / unit guards.
 // Returns true when some GPU fits; score / gpu index by reference.
 // ---------------------------------------------------------------------------------------------
-EGS_HD bool trade_single(const int (&c)[EGS_G], const int (&m)[EGS_G], int rc, int rm,
+template <int G>
+EGS_HD bool trade_single(const int (&c)[G], const int (&m)[G], int rc, int rm,
                          int policy, int &score, int &gidx) {
+  constexpr int LG = RowWidth<G>::LG;
   int bestkey = -1;
   if (policy == EGS_BINPACK) {
     unsigned ucmin = 0xFFFFFFFFu, ummin = 0xFFFFFFFFu;
-    int cpre[EGS_G], csuf[EGS_G], mpre[EGS_G], msuf[EGS_G];
-    cpre[0] = INT32_MIN; mpre[0] = INT32_MIN; csuf[EGS_G - 1] = INT32_MIN; msuf[EGS_G - 1] = INT32_MIN;
+    int cpre[G], csuf[G], mpre[G], msuf[G];
+    cpre[0] = INT32_MIN; mpre[0] = INT32_MIN; csuf[G - 1] = INT32_MIN; msuf[G - 1] = INT32_MIN;
 #pragma unroll
-    for (int g = 0; g < EGS_G; g++) { ucmin = EGS_MIN(ucmin, (unsigned)c[g]); ummin = EGS_MIN(ummin, (unsigned)m[g]); }
+    for (int g = 0; g < G; g++) { ucmin = EGS_MIN(ucmin, (unsigned)c[g]); ummin = EGS_MIN(ummin, (unsigned)m[g]); }
 #pragma unroll
-    for (int g = 1; g < EGS_G; g++) { cpre[g] = EGS_MAX(cpre[g - 1], c[g - 1]); mpre[g] = EGS_MAX(mpre[g - 1], m[g - 1]); }
+    for (int g = 1; g < G; g++) { cpre[g] = EGS_MAX(cpre[g - 1], c[g - 1]); mpre[g] = EGS_MAX(mpre[g - 1], m[g - 1]); }
 #pragma unroll
-    for (int g = EGS_G - 2; g >= 0; g--) { csuf[g] = EGS_MAX(csuf[g + 1], c[g + 1]); msuf[g] = EGS_MAX(msuf[g + 1], m[g + 1]); }
+    for (int g = G - 2; g >= 0; g--) { csuf[g] = EGS_MAX(csuf[g + 1], c[g + 1]); msuf[g] = EGS_MAX(msuf[g + 1], m[g + 1]); }
     const int cmin = (int)ucmin, mmin = (int)ummin;
 #pragma unroll
-    for (int g = 0; g < EGS_G; g++) {
+    for (int g = 0; g < G; g++) {
       const bool ok = (c[g] >= rc) && (m[g] >= rm);         // CanAllocate gpu.go:55; PAD rows fail
       const int nc = c[g] - rc, nm = m[g] - rm;             // GPU.Add gpu.go:36-37
       const int cmx = EGS_MAX3(cpre[g], csuf[g], nc), cmn = EGS_MIN(cmin, nc);
       const int mmx = EGS_MAX3(mpre[g], msuf[g], nm), mmn = EGS_MIN(mmin, nm);
       const int x = (mmx + cmx) - (mmn + cmn);
-      const int key = ok ? ((x >> 2) * 8 + g) : -1;
+      const int key = ok ? ((x >> 2) * G + g) : -1;
       bestkey = EGS_MAX(bestkey, key);
     }
-    score = (bestkey >> 3) * 100;
+    score = (bestkey >> LG) * 100;
   } else {                                                   // Spread.Rate == 0 (rater.go:56-59): last feasible GPU
 #pragma unroll
-    for (int g = 0; g < EGS_G; g++) bestkey = ((c[g] >= rc) && (m[g] >= rm)) ? g : bestkey;
+    for (int g = 0; g < G; g++) bestkey = ((c[g] >= rc) && (m[g] >= rm)) ? g : bestkey;
     score = 0;
   }
-  gidx = bestkey & 7;
+  gidx = bestkey & (G - 1);
   return bestkey >= 0;
 }
 
@@ -159,13 +180,15 @@ EGS_HD int trade_lane_key(const int (&c)[EGS_G], const int (&m)[EGS_G], int gl, 
 // General Trade: up to EGS_C containers, whole-GPU units, sentinel units.  Depth-first over
 // the containers exactly as gpu.go:72-123.  Cold path: rows live in local memory.
 // ---------------------------------------------------------------------------------------------
+template <int G>
 struct TradeCtx {
-  int c[EGS_G], m[EGS_G];
+  typedef PackedT<G> P;
+  int c[G], m[G];
   int mem_total, policy;
   const Req *r;
-  uint32_t masks;       // 4 x u8: GPUs chosen per container on the current DFS path
+  P masks;              // 4 x Mask: GPUs chosen per container on the current DFS path
   int best;
-  uint32_t best_masks;
+  P best_masks;
   bool found;
 };
 
@@ -174,20 +197,21 @@ struct TradeCtx {
 #else
 #define EGS_HD_NOINLINE __host__ __device__ inline
 #endif
-EGS_HD_NOINLINE void trade_leaf(TradeCtx &t) {  // gpu.go:73-93
+template <int G>
+EGS_HD_NOINLINE void trade_leaf(TradeCtx<G> &t) {  // gpu.go:73-93
   int s = 0;
   if (t.policy == EGS_BINPACK) {
     // rateIndexes: containers holding exactly one GPU (gpu.go:76-83); k = distinct GPUs (rater.go:19-30)
     uint32_t used = 0;
 #pragma unroll 1
     for (int i = 0; i < t.r->C; i++) {
-      uint32_t mk = (t.masks >> (8 * i)) & 0xFFu;
+      uint32_t mk = (uint32_t)(t.masks >> (G * i)) & ((1u << G) - 1u);
       if (EGS_POPC(mk) == 1) used |= mk;
     }
     int k = EGS_POPC(used);
     int cmin = INT32_MAX, cmax = INT32_MIN, mmin = INT32_MAX, mmax = INT32_MIN;
 #pragma unroll 1
-    for (int g = 0; g < EGS_G; g++) {
+    for (int g = 0; g < G; g++) {
       if (t.c[g] == EGS_PAD) continue;
       cmin = EGS_MIN(cmin, t.c[g]); cmax = EGS_MAX(cmax, t.c[g]);
       mmin = EGS_MIN(mmin, t.m[g]); mmax = EGS_MAX(mmax, t.m[g]);
@@ -201,46 +225,50 @@ EGS_HD_NOINLINE void trade_leaf(TradeCtx &t) {  // gpu.go:73-93
   t.best_masks = t.masks;
 }
 
-template <int CI>
-EGS_HD_NOINLINE void trade_dfs(TradeCtx &t) {
-  if (CI == t.r->C) { trade_leaf(t); return; }
-  const int rc = t.r->core[CI], rm = t.r->mem[CI], cnt = t.r->cnt[CI];
-  const uint32_t keep = t.masks & ~(0xFFu << (8 * CI));
-  if (cnt > 0) {  // gpu.go:95-109 with GetFreeGPUs gpu.go:193-202 on the mutated rows
-    uint32_t fm = 0; int nf = 0;
+template <int G, int CI>
+EGS_HD_NOINLINE void trade_dfs(TradeCtx<G> &t) {
+  typedef PackedT<G> P;
+  if constexpr (CI == EGS_C) {
+    trade_leaf(t);
+  } else {
+    if (CI == t.r->C) { trade_leaf(t); return; }
+    const int rc = t.r->core[CI], rm = t.r->mem[CI], cnt = t.r->cnt[CI];
+    const P keep = t.masks & ~((P)MaskT<G>(~0u) << (G * CI));
+    if (cnt > 0) {  // gpu.go:95-109 with GetFreeGPUs gpu.go:193-202 on the mutated rows
+      uint32_t fm = 0; int nf = 0;
 #pragma unroll 1
-    for (int g = 0; g < EGS_G; g++)
-      if (nf < cnt && t.c[g] == EGS_CORE_PER_GPU && t.m[g] == t.mem_total) { fm |= 1u << g; nf++; }
-    if (nf < cnt) return;
+      for (int g = 0; g < G; g++)
+        if (nf < cnt && t.c[g] == EGS_CORE_PER_GPU && t.m[g] == t.mem_total) { fm |= 1u << g; nf++; }
+      if (nf < cnt) return;
 #pragma unroll 1
-    for (int g = 0; g < EGS_G; g++) if ((fm >> g) & 1u) { t.c[g] = 0; t.m[g] = 0; }          // Add gpu.go:32-34
-    t.masks = keep | (fm << (8 * CI));
-    trade_dfs<CI + 1>(t);
+      for (int g = 0; g < G; g++) if ((fm >> g) & 1u) { t.c[g] = 0; t.m[g] = 0; }          // Add gpu.go:32-34
+      t.masks = keep | ((P)fm << (G * CI));
+      trade_dfs<G, CI + 1>(t);
 #pragma unroll 1
-    for (int g = 0; g < EGS_G; g++) if ((fm >> g) & 1u) { t.c[g] = EGS_CORE_PER_GPU; t.m[g] = t.mem_total; }  // Sub gpu.go:42-44
+      for (int g = 0; g < G; g++) if ((fm >> g) & 1u) { t.c[g] = EGS_CORE_PER_GPU; t.m[g] = t.mem_total; }  // Sub gpu.go:42-44
+      t.masks = keep;
+      return;
+    }
+#pragma unroll 1
+    for (int g = 0; g < G; g++) {  // gpu.go:110-122
+      if (!(t.c[g] >= rc && t.m[g] >= rm)) continue;
+      t.c[g] -= rc; t.m[g] -= rm;
+      t.masks = keep | (((P)1u << g) << (G * CI));
+      trade_dfs<G, CI + 1>(t);
+      t.c[g] += rc; t.m[g] += rm;
+    }
     t.masks = keep;
-    return;
   }
-#pragma unroll 1
-  for (int g = 0; g < EGS_G; g++) {  // gpu.go:110-122
-    if (!(t.c[g] >= rc && t.m[g] >= rm)) continue;
-    t.c[g] -= rc; t.m[g] -= rm;
-    t.masks = keep | ((1u << g) << (8 * CI));
-    trade_dfs<CI + 1>(t);
-    t.c[g] += rc; t.m[g] += rm;
-  }
-  t.masks = keep;
 }
-template <>
-EGS_HD_NOINLINE void trade_dfs<EGS_C>(TradeCtx &t) { trade_leaf(t); }
 
-EGS_HD bool trade_general(const int (&c)[EGS_G], const int (&m)[EGS_G], int mem_total,
-                          const Req &r, int policy, int &score, uint32_t &masks) {
-  TradeCtx t;
+template <int G>
+EGS_HD bool trade_general(const int (&c)[G], const int (&m)[G], int mem_total,
+                          const Req &r, int policy, int &score, PackedT<G> &masks) {
+  TradeCtx<G> t;
 #pragma unroll
-  for (int g = 0; g < EGS_G; g++) { t.c[g] = c[g]; t.m[g] = m[g]; }
+  for (int g = 0; g < G; g++) { t.c[g] = c[g]; t.m[g] = m[g]; }
   t.mem_total = mem_total; t.policy = policy; t.r = &r; t.masks = 0; t.best = 0; t.best_masks = 0; t.found = false;
-  trade_dfs<0>(t);
+  trade_dfs<G, 0>(t);
   score = t.best; masks = t.best_masks;
   return t.found;
 }
@@ -317,13 +345,14 @@ __host__ __device__ __forceinline__ bool req_is_single(const Req &r) {
   return r.C == 1 && r.cnt[0] == 0 && r.core[0] >= 0 && r.mem[0] >= 0;
 }
 
-// Trade dispatch.  `masks` packs one u8 GPU mask per container.
-EGS_HD bool trade_any(const int (&c)[EGS_G], const int (&m)[EGS_G], int mem_total,
-                      const Req &r, bool single, int policy, int &score, uint32_t &masks) {
+// Trade dispatch.  `masks` packs one G-bit GPU mask per container.
+template <int G>
+EGS_HD bool trade_any(const int (&c)[G], const int (&m)[G], int mem_total,
+                      const Req &r, bool single, int policy, int &score, PackedT<G> &masks) {
   if (single) {
     int g;
     bool ok = trade_single(c, m, r.core[0], r.mem[0], policy, score, g);
-    masks = 1u << g;
+    masks = (PackedT<G>)1u << g;
     return ok;
   }
   return trade_general(c, m, mem_total, r, policy, score, masks);
@@ -331,12 +360,13 @@ EGS_HD bool trade_any(const int (&c)[EGS_G], const int (&m)[EGS_G], int mem_tota
 
 // GPUs.Transact gpu.go:153-175 on the node's rows in global memory (one thread).
 // Returns true on success; on failure the Adds already made stay (no rollback).
+template <int G>
 EGS_HD bool transact_row(int32_t *core, int32_t *mem, int mem_total, const Req &r,
-                         uint32_t masks) {
+                         PackedT<G> masks) {
   for (int i = 0; i < r.C; i++) {
-    uint32_t mk = (masks >> (8 * i)) & 0xFFu;
+    uint32_t mk = (uint32_t)(masks >> (G * i)) & ((1u << G) - 1u);
     if (r.cnt[i] > 0) {
-      for (int g = 0; g < EGS_G; g++) {
+      for (int g = 0; g < G; g++) {
         if (!((mk >> g) & 1u)) continue;
         if (!(core[g] == EGS_CORE_PER_GPU && mem[g] == mem_total)) return false;
         core[g] = 0; mem[g] = 0;
@@ -351,13 +381,15 @@ EGS_HD bool transact_row(int32_t *core, int32_t *mem, int mem_total, const Req &
 }
 
 // One AddPod / ForgetPod row update with the option rebuilt from annotations (allocate.go:75-93): explicit index
-// lists; a fractional container uses its first index only.
-struct ApplyOp { int node, cancel; ReqW req; int n_idx[EGS_CA]; int8_t idx[EGS_CA][EGS_G]; };
+// lists; a fractional container uses its first index only.  A whole-GPU container lists up to G indices.
+template <int G>
+struct ApplyOp { int node, cancel; ReqW req; int n_idx[EGS_CA]; int8_t idx[EGS_CA][G]; };
 
 // The update on the node's rows (one thread): Cancel (gpu.go:177-191, GPU.Sub gpu.go:41-49: a whole-GPU container
 // puts its GPUs back at their totals) or Transact (gpu.go:153-175, CanAllocate + Add: the first failure stops the op,
 // no rollback).  Returns false when a Transact stopped.
-EGS_HD bool apply_op(int32_t *c, int32_t *m, int mt, const ApplyOp &op) {
+template <int G>
+EGS_HD bool apply_op(int32_t *c, int32_t *m, int mt, const ApplyOp<G> &op) {
   for (int i = 0; i < op.req.C; i++) {
     const bool whole = op.req.cnt[i] > 0;
     const int lim = whole ? op.n_idx[i] : (op.n_idx[i] > 0 ? 1 : 0);

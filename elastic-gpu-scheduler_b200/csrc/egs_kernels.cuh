@@ -11,6 +11,8 @@
 //                ForgetPod in one launch.
 // Each reference step these kernels share is written once: Assume (assume_option), Allocate
 // (allocate_option), and the AddPod / ForgetPod row update (apply_op, egs_device.cuh).
+// Every kernel here is a template on the row width G (8, or 16 on a handle with g_max > 8); the rounds engine
+// (egs_rounds.cuh) uses the 8-wide instantiations only.
 #pragma once
 #include "egs_device.cuh"
 
@@ -19,7 +21,7 @@
 struct OptTable {            // option cache of ONE request shape (slot)
   uint8_t *st;               // [N_pad]  OPT_*
   int32_t *sc;               // [N_pad]  option.Score
-  uint8_t *al;               // [EGS_C][N_pad] GPU mask per container (option.Allocated)
+  uint8_t *al;               // [EGS_C][N_pad] MaskT<G> GPU mask per container (option.Allocated)
   size_t plane;              // N_pad
 };
 
@@ -27,20 +29,21 @@ struct Partial { unsigned long long key, fd, sd; int fit; int pad; };
 
 struct PodOut {              // per-pod outputs of the batch loop (device pointers, may be null)
   int32_t *node, *status, *fit_count;
-  uint8_t *alloc;            // [P][EGS_C]
+  uint8_t *alloc;            // [P][EGS_C] MaskT<G>
   unsigned long long *fit_digest, *score_digest;
 };
 
-// The six per-pod outputs of pod p; `masks` packs the EGS_C alloc bytes of the pod (one u8 GPU mask per container).
+// The six per-pod outputs of pod p; `masks` packs the EGS_C alloc masks of the pod (one MaskT<G> per container).
+template <int G>
 __device__ __forceinline__ void write_pod_out(const PodOut &o, int p, int node, int status, int fit, unsigned long long fd,
-                                              unsigned long long sd, uint32_t masks) {
-  static_assert(EGS_C == 4, "alloc row == one 32-bit word");
+                                              unsigned long long sd, PackedT<G> masks) {
+  static_assert(EGS_C * sizeof(MaskT<G>) == sizeof(PackedT<G>), "alloc row == one packed word");
   if (o.node) o.node[p] = node;
   if (o.status) o.status[p] = status;
   if (o.fit_count) o.fit_count[p] = fit;
   if (o.fit_digest) o.fit_digest[p] = fd;
   if (o.score_digest) o.score_digest[p] = sd;
-  if (o.alloc) reinterpret_cast<uint32_t *>(o.alloc)[p] = masks;
+  if (o.alloc) reinterpret_cast<PackedT<G> *>(o.alloc)[p] = masks;
 }
 
 struct PassArgs {
@@ -98,18 +101,18 @@ __device__ __forceinline__ void memo_reset(uint8_t *all_st, size_t slot_stride, 
 // (node.go:64-66); no entry -> Trade (node.go:67-71): the option is cached, or the failure memoised as UNFIT (the
 // reference caches nothing then and re-Trades with the same outcome).  Returns the state after Assume; `score` is
 // set when it is OPT_CACHED.  The fast Trade ignores mem_total, so SINGLE does not load it.
-template <bool SINGLE>
+template <int G, bool SINGLE>
 __device__ __forceinline__ uint8_t assume_option(const OptTable &t, size_t i, const int32_t *core, const int32_t *mem,
                                                  const int32_t *mem_total, const Req &req, int policy, int &score) {
   uint8_t st = t.st[i];
   if (st == OPT_CACHED) { score = t.sc[i]; return st; }
   if (st != OPT_ABSENT) return st;
-  int c[EGS_G], m[EGS_G]; uint32_t masks;
+  int c[G], m[G]; PackedT<G> masks;
   load_row(core, mem, i, c, m);
   if (trade_any(c, m, SINGLE ? 0 : mem_total[i], req, SINGLE, policy, score, masks)) {
     st = OPT_CACHED;
     t.sc[i] = score;
-    for (int k = 0; k < req.C; k++) t.al[(size_t)k * t.plane + i] = (uint8_t)(masks >> (8 * k));
+    for (int k = 0; k < req.C; k++) reinterpret_cast<MaskT<G> *>(t.al)[(size_t)k * t.plane + i] = (MaskT<G>)(masks >> (G * k));
   } else {
     st = OPT_UNFIT;
   }
@@ -117,21 +120,23 @@ __device__ __forceinline__ uint8_t assume_option(const OptTable &t, size_t i, co
   return st;
 }
 
-// GPU masks of node w's option, one u8 per container.
-__device__ __forceinline__ uint32_t option_masks(const OptTable &t, size_t w, int C) {
-  uint32_t masks = 0;
-  for (int c = 0; c < C; c++) masks |= (uint32_t)t.al[(size_t)c * t.plane + w] << (8 * c);
+// GPU masks of node w's option, one MaskT<G> per container.
+template <int G>
+__device__ __forceinline__ PackedT<G> option_masks(const OptTable &t, size_t w, int C) {
+  PackedT<G> masks = 0;
+  for (int c = 0; c < C; c++) masks |= (PackedT<G>)reinterpret_cast<const MaskT<G> *>(t.al)[(size_t)c * t.plane + w] << (G * c);
   return masks;
 }
 
 // NodeAllocator.Allocate (node.go:87-104) of node w's cached option; one thread.  The entry goes before the Transact
 // (deferred delete, node.go:90-92); the rows changed, so the node's UNFIT memos go too.
+template <int G>
 __device__ __forceinline__ int allocate_option(const OptTable &t, size_t w, int32_t *core, int32_t *mem, int mem_total,
                                                const Req &req, uint8_t *all_st, size_t slot_stride, int n_slots,
-                                               uint32_t &masks) {
-  masks = option_masks(t, w, req.C);
+                                               PackedT<G> &masks) {
+  masks = option_masks<G>(t, w, req.C);
   t.st[w] = OPT_ABSENT;
-  const bool ok = transact_row(core + w * EGS_G, mem + w * EGS_G, mem_total, req, masks);
+  const bool ok = transact_row<G>(core + w * G, mem + w * G, mem_total, req, masks);
   memo_reset(all_st, slot_stride, n_slots, w);
   return ok ? EGS_OK : EGS_ERR_TRANSACT;
 }
@@ -140,8 +145,10 @@ __device__ __forceinline__ int allocate_option(const OptTable &t, size_t w, int3
 // k_pass: one pod, all nodes.  One thread per node; block partials; the last block to finish
 // (atomic ticket) folds the partials, picks the first max and binds it.
 // --------------------------------------------------------------------------------------------
-template <bool SINGLE>
-__global__ void __launch_bounds__(PASS_THREADS) k_pass(PassArgs a) {
+// At G = 16 a minimum of one block per SM lifts ptxas's default 64-register cap, under which the 16-wide row spills
+// (70 / 80 registers without spills, sm_90a); 0 leaves the 8-wide instantiations exactly as they were.
+template <int G, bool SINGLE>
+__global__ void __launch_bounds__(PASS_THREADS, G > EGS_G ? 1 : 0) k_pass(PassArgs a) {
   __shared__ Partial sm[PASS_THREADS / 32];
   __shared__ bool is_last;
   const int i = blockIdx.x * PASS_THREADS + threadIdx.x;
@@ -149,7 +156,7 @@ __global__ void __launch_bounds__(PASS_THREADS) k_pass(PassArgs a) {
   int fit = 0;
   if (i < a.n) {
     int score = 0;
-    if (assume_option<SINGLE>(a.t, (size_t)i, a.core, a.mem, a.mem_total, a.req, a.policy, score) == OPT_CACHED) {
+    if (assume_option<G, SINGLE>(a.t, (size_t)i, a.core, a.mem, a.mem_total, a.req, a.policy, score) == OPT_CACHED) {
       fit = 1; key = cand_key(score, (uint32_t)i); fd = fit_term((uint32_t)i); sd = score_term((uint32_t)i, score);
     }
     if (a.vec_fit) a.vec_fit[i] = (uint8_t)fit;
@@ -175,14 +182,14 @@ __global__ void __launch_bounds__(PASS_THREADS) k_pass(PassArgs a) {
   if (threadIdx.x == 0) {
     *a.ticket = 0;
     int node = -1, status = EGS_ERR_NOFIT;
-    uint32_t masks = 0;
+    PackedT<G> masks = 0;
     if (key != 0) {
       node = (int)key_node(key);
-      status = allocate_option(a.t, (size_t)node, a.core_w, a.mem_w, a.mem_total[node], a.req, a.all_st, a.slot_stride,
+      status = allocate_option<G>(a.t, (size_t)node, a.core_w, a.mem_w, a.mem_total[node], a.req, a.all_st, a.slot_stride,
                                a.n_slots, masks);
       if (status != EGS_OK) masks = 0;
     }
-    write_pod_out(a.out, a.pod, node, status, fit, fd, sd, masks);
+    write_pod_out<G>(a.out, a.pod, node, status, fit, fd, sd, masks);
   }
 }
 
@@ -195,14 +202,14 @@ struct EvalArgs {
   const int32_t *core, *mem, *mem_total;
   int lo, n, policy;                                            // nodes [lo, lo + n)
   Req req;
-  uint8_t *fit; int32_t *score; uint8_t *gpu; size_t plane;     // gpu: [C][plane]; all indexed by node id
+  uint8_t *fit; int32_t *score; uint8_t *gpu; size_t plane;     // gpu: [C][plane] MaskT<G>; all indexed by node id
   uint8_t v_fit, v_unfit;                                       // byte written for fit / unfit (1/0, or OPT_NEW/OPT_UNFIT
 };                                                              // when the target is an option table)
 
-template <bool SINGLE, int ITEMS>
+template <int G, bool SINGLE, int ITEMS>
 __global__ void __launch_bounds__(256) k_evaluate(EvalArgs a) {
   const int base = blockIdx.x * (256 * ITEMS) + threadIdx.x;
-  int c[ITEMS][EGS_G], m[ITEMS][EGS_G];
+  int c[ITEMS][G], m[ITEMS][G];
 #pragma unroll
   for (int it = 0; it < ITEMS; it++) {
     const int j = base + it * 256;
@@ -213,13 +220,14 @@ __global__ void __launch_bounds__(256) k_evaluate(EvalArgs a) {
     const int j = base + it * 256;
     if (j >= a.n) continue;
     const int i = a.lo + j;
-    int score; uint32_t masks;
+    int score; PackedT<G> masks;
     const int mt = SINGLE ? 0 : a.mem_total[i];
     const bool ok = trade_any(c[it], m[it], mt, a.req, SINGLE, a.policy, score, masks);
     a.fit[i] = ok ? a.v_fit : a.v_unfit;
     a.score[i] = ok ? score : 0;
-    if (SINGLE) a.gpu[i] = ok ? (uint8_t)masks : 0;
-    else for (int k = 0; k < a.req.C; k++) a.gpu[(size_t)k * a.plane + i] = ok ? (uint8_t)(masks >> (8 * k)) : 0;
+    MaskT<G> *gpu = reinterpret_cast<MaskT<G> *>(a.gpu);
+    if (SINGLE) gpu[i] = ok ? (MaskT<G>)masks : 0;
+    else for (int k = 0; k < a.req.C; k++) gpu[(size_t)k * a.plane + i] = ok ? (MaskT<G>)(masks >> (G * k)) : 0;
   }
 }
 
@@ -236,19 +244,19 @@ struct GatherArgs {
 };
 
 // Assume per node (node.go:61-73)
-template <bool SINGLE>
+template <int G, bool SINGLE>
 __global__ void __launch_bounds__(256) k_gather_filter(GatherArgs a) {
   const int j = blockIdx.x * 256 + threadIdx.x;
   if (j >= a.n) return;
   const int i = a.ids ? a.ids[j] : j;
   if (i < 0 || i >= a.n_nodes) { a.out_fit[j] = 0; return; }
   int score;
-  a.out_fit[j] = assume_option<SINGLE>(a.t, (size_t)i, a.core, a.mem, a.mem_total, a.req, a.policy, score) == OPT_CACHED;
+  a.out_fit[j] = assume_option<G, SINGLE>(a.t, (size_t)i, a.core, a.mem, a.mem_total, a.req, a.policy, score) == OPT_CACHED;
 }
 
 // Score per node (node.go:75-85): cached score; no entry -> Assume; fails -> 0, succeeds -> the
 // reference dereferences nil (panic) -- flagged.
-template <bool SINGLE>
+template <int G, bool SINGLE>
 __global__ void __launch_bounds__(256) k_gather_score(GatherArgs a) {
   const int j = blockIdx.x * 256 + threadIdx.x;
   if (j >= a.n) return;
@@ -256,7 +264,7 @@ __global__ void __launch_bounds__(256) k_gather_score(GatherArgs a) {
   if (i < 0 || i >= a.n_nodes) { a.out_score[j] = 0; return; }   // scheduler.go:176-179
   if (a.t.st[i] == OPT_CACHED) { a.out_score[j] = a.t.sc[i]; return; }
   int score;                                                       // Assume caches the option before the nil deref
-  if (assume_option<SINGLE>(a.t, (size_t)i, a.core, a.mem, a.mem_total, a.req, a.policy, score) == OPT_CACHED) *a.panic_flag = 1;
+  if (assume_option<G, SINGLE>(a.t, (size_t)i, a.core, a.mem, a.mem_total, a.req, a.policy, score) == OPT_CACHED) *a.panic_flag = 1;
   a.out_score[j] = 0;
 }
 
@@ -266,50 +274,56 @@ struct BindArgs {
   uint8_t *all_st; size_t slot_stride; int n_slots;
   int skip_transact;          // uid already in the node's podsMap (node.go:149)
   int consume;                // 1: Bind (delete the entry); 0: peek
-  int32_t *result;            // [0] had entry, [1] status, [2] masks, [3] score
+  int32_t *result;            // [0] had entry, [1] status, [2] masks (low 32 bits), [3] score, [4] masks >> 32 (G = 16)
 };
+template <int G>
 __global__ void k_bind(BindArgs a) {
   const size_t w = (size_t)a.node;
   const bool had = a.t.st[w] == OPT_CACHED;
-  uint32_t masks = 0; int status = EGS_ERR_NO_OPTION, score = 0;
+  PackedT<G> masks = 0; int status = EGS_ERR_NO_OPTION, score = 0;
   if (had) {
     score = a.t.sc[w];
     status = EGS_OK;
     if (a.consume && !a.skip_transact) {
-      status = allocate_option(a.t, w, a.core, a.mem, a.mem_total[w], a.req, a.all_st, a.slot_stride, a.n_slots, masks);
+      status = allocate_option<G>(a.t, w, a.core, a.mem, a.mem_total[w], a.req, a.all_st, a.slot_stride, a.n_slots, masks);
     } else {                                     // peek, or Bind of a known uid (node.go:149): the entry goes, rows stay
-      masks = option_masks(a.t, w, a.req.C);
+      masks = option_masks<G>(a.t, w, a.req.C);
       if (a.consume) a.t.st[w] = OPT_ABSENT;
     }
   }
   a.result[0] = had; a.result[1] = status; a.result[2] = (int32_t)masks; a.result[3] = score;
+  if constexpr (sizeof(masks) > 4) a.result[4] = (int32_t)(masks >> 32);
 }
 
 // AddPod / ForgetPod of one pod (apply_op) on node op.node.
+template <int G>
 struct ApplyArgs {
   int32_t *core, *mem; const int32_t *mem_total;
-  ApplyOp op;
+  ApplyOp<G> op;
   uint8_t *all_st; size_t slot_stride; int n_slots;
 };
-__global__ void k_apply(ApplyArgs a) {
+template <int G>
+__global__ void k_apply(ApplyArgs<G> a) {
   const size_t w = (size_t)a.op.node;
-  apply_op(a.core + w * EGS_G, a.mem + w * EGS_G, a.mem_total[w], a.op);
+  apply_op(a.core + w * G, a.mem + w * G, a.mem_total[w], a.op);
   memo_reset(a.all_st, a.slot_stride, a.n_slots, w);
 }
 
 // Many AddPod / ForgetPod row updates in ONE launch: the host has grouped the records by node (record order kept
 // inside a node); one thread per touched node applies its run.
+template <int G>
 struct ApplyManyArgs {
   int32_t *core, *mem; const int32_t *mem_total;
-  const ApplyOp *ops; const int32_t *group_off; int n_groups;   // group g = ops[group_off[g] .. group_off[g+1])
+  const ApplyOp<G> *ops; const int32_t *group_off; int n_groups;   // group g = ops[group_off[g] .. group_off[g+1])
   uint8_t *all_st; size_t slot_stride; int n_slots;
 };
-__global__ void k_apply_many(ApplyManyArgs a) {
+template <int G>
+__global__ void k_apply_many(ApplyManyArgs<G> a) {
   const int gi = blockIdx.x * blockDim.x + threadIdx.x;
   if (gi >= a.n_groups) return;
   const size_t w = (size_t)a.ops[a.group_off[gi]].node;
   for (int o = a.group_off[gi]; o < a.group_off[gi + 1]; o++)
-    apply_op(a.core + w * EGS_G, a.mem + w * EGS_G, a.mem_total[w], a.ops[o]);
+    apply_op(a.core + w * G, a.mem + w * G, a.mem_total[w], a.ops[o]);
   memo_reset(a.all_st, a.slot_stride, a.n_slots, w);
 }
 

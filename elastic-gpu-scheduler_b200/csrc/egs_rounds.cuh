@@ -784,7 +784,7 @@ __device__ __noinline__ int general_pod(SM &S, const MwArgs &a, const unsigned l
         consume_option(S, s, t, win, fitc, ofd, osd);
         S.dirty[t] = 1;
         const int v = S.ver[t]; st_vol(&S.ver[t], v + 1);
-        ok = transact_row(S.rc[t], S.rm[t], S.mt[t], S.reqs[s], masks) ? 1 : 0;
+        ok = transact_row<EGS_G>(S.rc[t], S.rm[t], S.mt[t], S.reqs[s], masks) ? 1 : 0;
         st_vol(&S.ver[t], v + 2);
       }
       ok = __shfl_sync(0xffffffffu, ok, 0);
@@ -812,7 +812,7 @@ __device__ __noinline__ int general_pod(SM &S, const MwArgs &a, const unsigned l
   }
   if (lane == 0) {
     if (win == 0) S.pu[s] = -1;                                 // every pending option of s was Traded above
-    write_pod_out(a.out, p, o_node, o_status, fitc, ofd, osd, o_masks);
+    write_pod_out<EGS_G>(a.out, p, o_node, o_status, fitc, ofd, osd, o_masks);
   }
   __syncwarp();
   return 0;
@@ -1238,7 +1238,7 @@ __global__ void __launch_bounds__(32 * MW_MAX_WARPS, 1) k_resolve_mw(MwArgs a) {
             }
             if (win != 0) consume_option(S, s, tw, win, fit, fd, sd);
             else { S.afit[s] = fit; S.afd[s] = fd; S.asd[s] = sd; S.pu[s] = -1; }
-            write_pod_out(a.out, p, o_node, o_status, fit, fd, sd, o_masks);
+            write_pod_out<EGS_G>(a.out, p, o_node, o_status, fit, fd, sd, o_masks);
           }
           __syncwarp();
           PROF_T(3)

@@ -216,8 +216,8 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
       ea.policy = h->policy; ea.req = make_req(sh.C, sh.u);
       ea.fit = tb.st + (size_t)slot * tb.n_pad; ea.score = tb.sc + (size_t)slot * tb.n_pad;
       ea.gpu = tb.al + (size_t)slot * EGS_C * tb.n_pad; ea.plane = tb.n_pad; ea.v_fit = OPT_NEW; ea.v_unfit = OPT_UNFIT;
-      if (is_single(sh.C, sh.u)) k_evaluate<true, 2><<<(ea.n + 511) / 512, 256, 0, h->stream>>>(ea);
-      else k_evaluate<false, 1><<<(ea.n + 255) / 256, 256, 0, h->stream>>>(ea);
+      if (is_single(sh.C, sh.u)) k_evaluate<EGS_G, true, 2><<<(ea.n + 511) / 512, 256, 0, h->stream>>>(ea);
+      else k_evaluate<EGS_G, false, 1><<<(ea.n + 255) / 256, 256, 0, h->stream>>>(ea);
       cold++;
     }
     if (e0) {

@@ -18,14 +18,15 @@ static const char *ret(HostCtx *c, const std::string &s) { c->buf = s; return c-
 
 extern "C" {
 
-void *egsh_create(int policy, int max_nodes, int device) {
+// g_max: the widest node (EGS_MAX_GPUS, or up to EGS_MAX_GPUS_WIDE)
+void *egsh_create(int policy, int max_nodes, int device, int g_max) {
   HostCtx *c = new HostCtx();
   c->sch = new CudaUnitScheduler(policy, max_nodes, device, [c](const std::string &name, NodeInfo *out) -> std::string {
     auto it = c->cluster.find(name);
     if (it == c->cluster.end()) return "nodes \"" + name + "\" not found";
     *out = it->second;
     return "";
-  });
+  }, g_max);
   if (!c->sch->ok()) { delete c->sch; delete c; return nullptr; }
   return c;
 }

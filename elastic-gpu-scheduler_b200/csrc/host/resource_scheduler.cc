@@ -14,9 +14,19 @@ static int64_t requestOf(const Container &c, const char *key) {   // GetGPUCoreF
   return it == c.requests.end() ? 0 : it->second;
 }
 
-CudaUnitScheduler::CudaUnitScheduler(int policy, int max_nodes, int device, NodeProvider provider)
-    : max_nodes_(max_nodes), provider_(std::move(provider)) {
-  if (egs_create(policy, max_nodes, EGS_MAX_GPUS, device, &h_) != EGS_OK) h_ = nullptr;
+CudaUnitScheduler::CudaUnitScheduler(int policy, int max_nodes, int device, NodeProvider provider, int g_max)
+    : max_nodes_(max_nodes), g_max_(g_max), provider_(std::move(provider)) {
+  if (egs_create(policy, max_nodes, g_max, device, &h_) != EGS_OK) h_ = nullptr;
+}
+
+// The GPU ids of container c's mask (EGS_MASK_BYTES(g_max) little-endian bytes at masks[c * EGS_MASK_BYTES]), joined.
+std::string CudaUnitScheduler::gpuList(const uint8_t *masks, size_t c, const char *sep) const {
+  const int nb = EGS_MASK_BYTES(g_max_);
+  uint32_t m = 0;
+  for (int b = 0; b < nb; b++) m |= (uint32_t)masks[c * nb + b] << (8 * b);
+  std::string v;
+  for (int g = 0; g < 8 * nb; g++) if (m >> g & 1) v += (v.empty() ? "" : sep) + std::to_string(g);
+  return v;
 }
 CudaUnitScheduler::~CudaUnitScheduler() {
   if (h_) egs_destroy(h_);
@@ -135,7 +145,7 @@ std::vector<int64_t> CudaUnitScheduler::Score(const std::vector<std::string> &no
 }
 
 std::string CudaUnitScheduler::gpusJson(int node_id) {
-  int32_t core[EGS_MAX_GPUS], mem[EGS_MAX_GPUS], gc = 0, mt = 0;
+  int32_t core[EGS_MAX_GPUS_WIDE], mem[EGS_MAX_GPUS_WIDE], gc = 0, mt = 0;   // EGS_ROW_WIDTH(g_max) cells used
   if (egs_state_dump(h_, node_id, 1, core, mem, &gc, &mt) != EGS_OK) return "[]";
   std::ostringstream os;
   os << "[";
@@ -152,9 +162,9 @@ std::string CudaUnitScheduler::Bind(const std::string &node, Pod *pod) {
   if (id < 0) return err;                                                                     // scheduler.go:190-193
   std::vector<egs_unit> req;
   if (!RequestOf(*pod, &req)) return "libegs: pods with more than 4 containers are not supported by the device path";
-  uint8_t masks[EGS_MAX_CONTAINERS] = {0, 0, 0, 0};
+  uint8_t masks[2 * EGS_MAX_CONTAINERS] = {};                  // room for EGS_MASK_BYTES <= 2
   // option text for the Transact error has to be read before the entry is consumed
-  int32_t valid = 0, score = 0; uint8_t pm[EGS_MAX_CONTAINERS] = {0, 0, 0, 0};
+  int32_t valid = 0, score = 0; uint8_t pm[2 * EGS_MAX_CONTAINERS] = {};
   egs_option_peek(h_, id, (int)req.size(), req.data(), &valid, &score, pm);
   const std::string gpus_before = gpusJson(id);
   int st = egs_bind(h_, id, (int)req.size(), req.data(), uidOf(pod->uid), masks);
@@ -164,10 +174,7 @@ std::string CudaUnitScheduler::Bind(const std::string &node, Pod *pod) {
     std::ostringstream os;
     os << "can't trade option &{Request:" << RequestString(req) << " Allocated:[";
     for (size_t c = 0; c < req.size(); c++) {
-      os << (c ? " " : "") << "[";
-      bool first = true;
-      for (int g = 0; g < EGS_MAX_GPUS; g++) if (pm[c] >> g & 1) { os << (first ? "" : " ") << g; first = false; }
-      os << "]";
+      os << (c ? " " : "") << "[" << gpuList(pm, c, " ") << "]";
     }
     os << "] Score:" << score << "} on " << gpusJson(id) << " because the GPU's residual memory or core can't satisfy the container";
     return os.str();
@@ -175,9 +182,7 @@ std::string CudaUnitScheduler::Bind(const std::string &node, Pod *pod) {
   if (st != EGS_OK) return std::string("libegs: ") + egs_status_string(st);
   // GetUpdatedPodAnnotationSpec pod.go:57-78
   for (size_t c = 0; c < pod->containers.size(); c++) {
-    std::string v;
-    for (int g = 0; g < EGS_MAX_GPUS; g++) if (masks[c] >> g & 1) v += (v.empty() ? "" : ",") + std::to_string(g);
-    pod->annotations[std::string(kAnnotationContainerPrefix) + pod->containers[c].name] = v;
+    pod->annotations[std::string(kAnnotationContainerPrefix) + pod->containers[c].name] = gpuList(masks, c, ",");
   }
   pod->annotations[kEGPUAssumed] = "true";
   pod->labels[kEGPUAssumed] = "true";

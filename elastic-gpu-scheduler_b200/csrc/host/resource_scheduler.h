@@ -56,8 +56,9 @@ class ResourceScheduler {                // scheduler.go:30-39 (errors are "" fo
 
 class CudaUnitScheduler : public ResourceScheduler {
  public:
-  // policy: EGS_BINPACK / EGS_SPREAD (cmd/main.go:45-54); max_nodes bounds the dense node-id space
-  CudaUnitScheduler(int policy, int max_nodes, int device, NodeProvider provider);
+  // policy: EGS_BINPACK / EGS_SPREAD (cmd/main.go:45-54); max_nodes bounds the dense node-id space; g_max is the widest
+  // node (egs_create): EGS_MAX_GPUS, or up to EGS_MAX_GPUS_WIDE for servers with more GPUs
+  CudaUnitScheduler(int policy, int max_nodes, int device, NodeProvider provider, int g_max = EGS_MAX_GPUS);
   ~CudaUnitScheduler() override;
   bool ok() const { return h_ != nullptr; }
 
@@ -82,10 +83,12 @@ class CudaUnitScheduler : public ResourceScheduler {
   int getNodeInfo(const std::string &name, std::string *err);   // scheduler.go:62-84 -> dense id or -1
   static uint64_t uidOf(const std::string &uid);
   std::string gpusJson(int node_id);                            // GPUs.String (gpu.go:60-63)
+  std::string gpuList(const uint8_t *masks, size_t c, const char *sep) const;   // GPU ids of container c's mask
   static void optionFromPod(const Pod &pod, std::vector<int32_t> *off, std::vector<int32_t> *idx);  // allocate.go:75-93
 
   egs_handle *h_ = nullptr;
   int max_nodes_;
+  int g_max_;
   NodeProvider provider_;
   std::unordered_map<std::string, int> node_ids_;
   std::vector<std::string> node_names_;

@@ -6,6 +6,7 @@ import ctypes as C
 from typing import Dict, List, Optional, Sequence, Tuple
 
 from . import _build
+from .capi import EGS_MAX_GPUS
 
 _lib = None
 
@@ -15,7 +16,7 @@ def _load():
     if _lib is None:
         L = C.CDLL(_build.build_host())
         vp, cp, i64 = C.c_void_p, C.c_char_p, C.c_int64
-        L.egsh_create.restype = vp; L.egsh_create.argtypes = [C.c_int, C.c_int, C.c_int]
+        L.egsh_create.restype = vp; L.egsh_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
         L.egsh_destroy.argtypes = [vp]
         L.egsh_register_node.argtypes = [vp, cp, i64, i64]
         L.egsh_register_assumed_pod.argtypes = [vp, cp, vp]
@@ -66,9 +67,10 @@ class Pod:
 
 
 class CudaUnitScheduler:
-    def __init__(self, policy: int, max_nodes: int = 1024, device: int = 0):
+    def __init__(self, policy: int, max_nodes: int = 1024, device: int = 0, g_max: int = EGS_MAX_GPUS):
+        """g_max: the widest node; above EGS_MAX_GPUS (up to 16) the handle is wide."""
         self.L = _load()
-        self.h = self.L.egsh_create(policy, max_nodes, device)
+        self.h = self.L.egsh_create(policy, max_nodes, device, g_max)
         if not self.h:
             raise RuntimeError("egsh_create failed (no CUDA device?)")
 

@@ -20,10 +20,11 @@
  * and calls cudaSetDevice on entry, so cgo thread-hopping is fine.
  *
  * The device state is an int32 SoA node/GPU cache:
- *   free_core[N][EGS_MAX_GPUS], free_mem[N][EGS_MAX_GPUS], mem_total[N]
+ *   free_core[N][W], free_mem[N][W], mem_total[N]      W = EGS_ROW_WIDTH(g_max)
  * (CoreTotal == 100 for every GPU, pkg/utils/types.go:6) plus, per interned
  * request shape s, the per-node option cache of node.go:19
- *   opt_state[s][N] (u8), opt_score[s][N] (i32), opt_alloc[s][c][N] (u8 GPU mask of container c, c < 4).
+ *   opt_state[s][N] (u8), opt_score[s][N] (i32), opt_alloc[s][c][N] (GPU mask of container c, c < 4,
+ *   EGS_MASK_BYTES(g_max) bytes).
  *
  * The INTEGRATION.md at the repo root shows the cgo binding.
  */
@@ -36,12 +37,22 @@
 extern "C" {
 #endif
 
-#define EGS_MAX_GPUS        8      /* GPUs per node the SoA row holds                      */
+#define EGS_MAX_GPUS        8      /* GPUs per node the SoA row of a handle with g_max <= 8 holds; width of egs_mutation */
+#define EGS_MAX_GPUS_WIDE   16     /* widest node any handle takes (a "wide" handle: 9 <= g_max <= 16)                */
 #define EGS_MAX_CONTAINERS  4      /* containers per pod the filter / score / bind path enumerates */
 #define EGS_MAX_CONTAINERS_APPLY 8 /* containers per pod AddPod / ForgetPod / replay account (sidecars count) */
 #define EGS_CORE_PER_GPU    100    /* utils.GPUCoreEachCard, pkg/utils/types.go:6          */
 #define EGS_MAX_MEM_PER_GPU (1 << 25) /* int32 guard: Range/(k+1)*100 must fit int32 (Go int is 64-bit) */
 #define EGS_MAX_CORE_LOAD   (1 << 20) /* bound for free_core values given to egs_state_load */
+
+/* Layout of a handle created with `g_max` GPUs per node -- the one rule every row and mask buffer below follows:
+ *   EGS_ROW_WIDTH(g_max)  int32 cells per node row (egs_state_dump): 8, or 16 on a wide handle;
+ *   EGS_MASK_BYTES(g_max) bytes per GPU mask, little endian, bit g = GPU g: 1, or 2 on a wide handle.
+ * Every GPU mask output (egs_bind, egs_option_peek, egs_option_dump and out_alloc_mask of the egs_schedule_batch*
+ * calls) holds EGS_MAX_CONTAINERS masks per pod / node: element (p, c) starts at byte
+ * (p*EGS_MAX_CONTAINERS + c) * EGS_MASK_BYTES(g_max).  For g_max <= 8 this is one u8 per container, as always. */
+#define EGS_ROW_WIDTH(g_max)  ((g_max) > EGS_MAX_GPUS ? EGS_MAX_GPUS_WIDE : EGS_MAX_GPUS)
+#define EGS_MASK_BYTES(g_max) ((g_max) > EGS_MAX_GPUS ? 2 : 1)
 
 /* -priority flag, cmd/main.go:45-54 */
 enum egs_policy { EGS_BINPACK = 0, EGS_SPREAD = 1 };
@@ -67,7 +78,14 @@ typedef struct egs_handle egs_handle;
 
 /* ---- lifecycle ------------------------------------------------------------- */
 
-/* One handle drives ONE device.  `g_max` <= EGS_MAX_GPUS is the widest node. */
+/* One handle drives ONE device.  `g_max` <= EGS_MAX_GPUS_WIDE is the widest node it takes (17+: EGS_ERR_BAD_ARG).
+ * A wide handle (g_max > EGS_MAX_GPUS) has 16-wide rows and 16-bit masks (EGS_ROW_WIDTH / EGS_MASK_BYTES) and
+ * these limits, each refused with EGS_ERR_BAD_ARG and an egs_last_error text:
+ *   - its batch engine is the per-pod engine: EGS_MODE_AUTO runs EGS_MODE_RESCAN, EGS_MODE_ROUNDS is refused
+ *     and applies nothing (also no record of egs_schedule_batch_mut);
+ *   - egs_shard_set is refused: the sharded engine is the rounds engine;
+ *   - a mutation record still lists at most EGS_MAX_GPUS indices per container: a whole-GPU container of more
+ *     than 8 GPUs goes through egs_pod_apply / egs_node_replay_pod / egs_pod_cancel, whose lists take up to 16. */
 int egs_create(int policy, int max_nodes, int g_max, int device, egs_handle **out);
 int egs_destroy(egs_handle *h);
 const char *egs_last_error(egs_handle *h);
@@ -87,7 +105,7 @@ int egs_state_load(egs_handle *h, int node_id, const int32_t *free_core, const i
  * free_core/free_mem are [n][gpu_count] row-major. */
 int egs_state_load_bulk(egs_handle *h, int node0, int n, int gpu_count, int mem_total,
                         const int32_t *free_core, const int32_t *free_mem);
-/* Status(), scheduler.go:283-290: rows of nodes [node0, node0+n) as [n][EGS_MAX_GPUS]
+/* Status(), scheduler.go:283-290: rows of nodes [node0, node0+n) as [n][EGS_ROW_WIDTH(g_max)]
  * (absent GPUs read as INT32_MIN), gpu_count[n], mem_total[n]; any out pointer may be NULL. */
 int egs_state_dump(egs_handle *h, int node0, int n, int32_t *free_core, int32_t *free_mem,
                    int32_t *gpu_count, int32_t *mem_total);
@@ -109,8 +127,8 @@ int egs_filter(egs_handle *h, int n, const int32_t *node_ids, int n_containers,
 int egs_score(egs_handle *h, int n, const int32_t *node_ids, int n_containers,
               const egs_unit *units, int32_t *out_score);
 /* Bind -> NodeAllocator.Allocate (node.go:87-104): consumes the cached option, Transact
- * without rollback (gpu.go:153-175).  out_alloc_mask[c] has bit g set when GPU g goes to
- * container c (Trade only ever yields ascending index lists, so the mask is lossless). */
+ * without rollback (gpu.go:153-175).  out_alloc_mask mask c has bit g set when GPU g goes to
+ * container c (Trade only ever yields ascending index lists, so the mask is lossless); EGS_MASK_BYTES per mask. */
 int egs_bind(egs_handle *h, int node_id, int n_containers, const egs_unit *units,
              uint64_t uid, uint8_t *out_alloc_mask);
 /* Inspect the cached option of (node, request) without side effects (tests, Assume's GPUIDs). */
@@ -120,7 +138,7 @@ int egs_option_peek(egs_handle *h, int node_id, int n_containers, const egs_unit
 /* Bulk form of egs_option_peek: the option cache (node.go:19 `allocated`) of one request on nodes
  * [node0, node0+n) -- the per-shape part of Status() / a checkpoint.  out_state[i]: 0 no entry, 1 entry
  * present (possibly stale), 2 no entry and the request is known not to fit the current rows;
- * out_score[i] / out_alloc_mask[i*EGS_MAX_CONTAINERS + c] are meaningful for state 1.  Any out may be NULL. */
+ * out_score[i] / the mask (i, c) of out_alloc_mask are meaningful for state 1.  Any out may be NULL. */
 int egs_option_dump(egs_handle *h, int n_containers, const egs_unit *units, int node0, int n,
                     uint8_t *out_state, int32_t *out_score, uint8_t *out_alloc_mask);
 
@@ -170,8 +188,9 @@ int egs_pod_released(egs_handle *h, uint64_t uid);   /* 1 / 0, scheduler.go:276-
 
 /* ---- batch decision loop (device resident) ---------------------------------- */
 
-/* Limits of the device path: nodes with at most EGS_MAX_GPUS GPUs, pods with at most
- * EGS_MAX_CONTAINERS containers, per-GPU memory units <= EGS_MAX_MEM_PER_GPU (use MiB, not bytes).
+/* Limits of the device path: nodes with at most EGS_MAX_GPUS_WIDE GPUs (more than EGS_MAX_GPUS only on a wide
+ * handle, see egs_create), pods with at most EGS_MAX_CONTAINERS containers, per-GPU memory units
+ * <= EGS_MAX_MEM_PER_GPU (use MiB, not bytes).
  * Anything beyond is refused with EGS_ERR_BAD_ARG / EGS_ERR_OVERFLOW_GUARD -- never computed differently.
  *
  * Driver rule (SURVEY.md 8d), identical to kube-scheduler's filter -> prioritize ->
@@ -182,7 +201,7 @@ int egs_pod_released(egs_handle *h, uint64_t uid);   /* 1 / 0, scheduler.go:276-
  * Outputs (host pointers, any may be NULL):
  *   out_node[p]        winner node id, -1 when no node fits
  *   out_status[p]      EGS_OK / EGS_ERR_NOFIT / EGS_ERR_TRANSACT
- *   out_alloc_mask[p*EGS_MAX_CONTAINERS + c]
+ *   out_alloc_mask     mask (p, c) at byte (p*EGS_MAX_CONTAINERS + c) * EGS_MASK_BYTES(g_max)
  *   out_fit_count[p]   number of fit nodes
  *   out_fit_digest[p]  sum over fit nodes of egs_mix64(2*node+1)                       (mod 2^64)
  *   out_score_digest[p] sum over fit nodes of egs_mix64(2*node+2) * (2*(u64)(u32)score + 1)             (mod 2^64)
@@ -192,7 +211,8 @@ int egs_pod_released(egs_handle *h, uint64_t uid);   /* 1 / 0, scheduler.go:276-
  * podsMap); otherwise they must be pairwise distinct and not yet known (EGS_ERR_BAD_ARG).  A bind that
  * reaches NodeAllocator.Add records the uid in that node's podsMap even when Transact fails (node.go:150);
  * only a successful bind enters podMaps (scheduler.go:224) -- visible through egs_pod_known.
- * EGS_MODE_AUTO == EGS_MODE_ROUNDS.  Both modes produce identical outputs; RESCAN is the literal
+ * EGS_MODE_AUTO == EGS_MODE_ROUNDS on a handle with g_max <= EGS_MAX_GPUS, EGS_MODE_RESCAN on a wide handle
+ * (which refuses EGS_MODE_ROUNDS).  Both modes produce identical outputs; RESCAN is the literal
  * one-pass-per-pod form (single shard only), ROUNDS the fast exact form (DESIGN.md 3).
  */
 enum egs_batch_mode {
@@ -215,7 +235,9 @@ int egs_schedule_batch_vec(egs_handle *h, int n_pods, const int32_t *c_off, cons
                            int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest);
 
 /* Same loop with every buffer already in device memory (bench `value` leg):
- * d_* are device pointers on the handle's device, laid out as above. */
+ * d_* are device pointers on the handle's device, laid out as above.  Each pod's masks are stored as one word of
+ * EGS_MAX_CONTAINERS * EGS_MASK_BYTES(g_max) bytes, so d_out_alloc_mask must be aligned to that size (4 bytes, or 8 on
+ * a wide handle; cudaMalloc memory always is): EGS_ERR_BAD_ARG otherwise. */
 int egs_schedule_batch_device(egs_handle *h, int mode, int n_pods, const int32_t *h_c_off,
                               const egs_unit *h_units,
                               int32_t *d_out_node, int32_t *d_out_status, uint8_t *d_out_alloc_mask,

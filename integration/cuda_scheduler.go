@@ -21,6 +21,9 @@ package scheduler
 #cgo LDFLAGS: -legs
 #include <stdlib.h>
 #include "egs.h"
+// the layout macros of egs.h (cgo cannot expand function-like macros)
+static int row_width(int g_max) { return EGS_ROW_WIDTH(g_max); }
+static int mask_bytes(int g_max) { return EGS_MASK_BYTES(g_max); }
 */
 import "C"
 
@@ -53,12 +56,14 @@ type CudaUnitScheduler struct {
 	nodeName []string
 	nodeErr  map[string]error // nodes whose NodeAllocator could not be built (node.go:28-30)
 	maxNodes int
+	gMax     int // widest node the handle takes (egs_create's g_max): rows and masks are laid out for it
 }
 
 // NewCudaUnitScheduler mirrors NewGPUUnitScheduler (scheduler.go:86-106): nodes that already carry assumed pods are
-// loaded up front, every other node on first use.
+// loaded up front, every other node on first use.  gMax is the widest node of the cluster, C.EGS_MAX_GPUS for 8-GPU
+// servers, up to C.EGS_MAX_GPUS_WIDE (a wide handle: 16-wide rows, two mask bytes per container, per-pod engine).
 func NewCudaUnitScheduler(config ElasticSchedulerConfig, coreName v1.ResourceName, memName v1.ResourceName,
-	maxNodes int, device int) (ResourceScheduler, error) {
+	maxNodes int, device int, gMax int) (ResourceScheduler, error) {
 	policy := C.int(C.EGS_BINPACK)
 	if _, ok := config.Rater.(*Spread); ok {
 		policy = C.int(C.EGS_SPREAD)
@@ -68,8 +73,9 @@ func NewCudaUnitScheduler(config ElasticSchedulerConfig, coreName v1.ResourceNam
 		nodeIDs:       map[string]int32{},
 		nodeErr:       map[string]error{},
 		maxNodes:      maxNodes,
+		gMax:          gMax,
 	}
-	if st := C.egs_create(policy, C.int(maxNodes), C.int(C.EGS_MAX_GPUS), C.int(device), &d.h); st != C.EGS_OK {
+	if st := C.egs_create(policy, C.int(maxNodes), C.int(gMax), C.int(device), &d.h); st != C.EGS_OK {
 		return nil, fmt.Errorf("egs_create failed: status %d (no CUDA device?)", int(st))
 	}
 	pods, err := d.Clientset.CoreV1().Pods(metav1.NamespaceAll).List(context.Background(), metav1.ListOptions{
@@ -260,9 +266,15 @@ func (d *CudaUnitScheduler) Score(nodes []string, pod *v1.Pod) []int {
 	return scores
 }
 
-func maskToIDs(mask C.uint8_t) []int {
+// maskToIDs decodes container c's GPU mask: EGS_MASK_BYTES(gMax) little-endian bytes at masks[c*EGS_MASK_BYTES].
+func (d *CudaUnitScheduler) maskToIDs(masks []C.uint8_t, c int) []int {
+	nb := int(C.mask_bytes(C.int(d.gMax)))
+	mask := 0
+	for b := 0; b < nb; b++ {
+		mask |= int(masks[c*nb+b]) << uint(8*b)
+	}
 	ids := []int{}
-	for g := 0; g < int(C.EGS_MAX_GPUS); g++ {
+	for g := 0; g < 8*nb; g++ {
 		if (mask>>uint(g))&1 != 0 {
 			ids = append(ids, g)
 		}
@@ -283,7 +295,7 @@ func (d *CudaUnitScheduler) Bind(node string, pod *v1.Pod) (err error) {
 	if err != nil {
 		return err
 	}
-	var masks [C.EGS_MAX_CONTAINERS]C.uint8_t
+	var masks [2 * C.EGS_MAX_CONTAINERS]C.uint8_t // room for EGS_MASK_BYTES <= 2
 	switch st := C.egs_bind(d.h, C.int(id), C.int(len(units)), &units[0], uidKey(pod.UID), &masks[0]); st {
 	case C.EGS_OK:
 	case C.EGS_ERR_NO_OPTION:
@@ -295,7 +307,7 @@ func (d *CudaUnitScheduler) Bind(node string, pod *v1.Pod) (err error) {
 	}
 	ids := make([][]int, len(units))
 	for i := range units {
-		ids[i] = maskToIDs(masks[i])
+		ids[i] = d.maskToIDs(masks[:], i)
 	}
 	newPod := GetUpdatedPodAnnotationSpec(pod, ids) // pod.go:57-78
 	if _, err := d.Clientset.CoreV1().Pods(newPod.Namespace).Update(context.Background(), newPod, metav1.UpdateOptions{}); err != nil {
@@ -395,7 +407,7 @@ func (d *CudaUnitScheduler) Status() string {
 		result, _ := json.Marshal(gpus)
 		return string(result)
 	}
-	g := int(C.EGS_MAX_GPUS)
+	g := int(C.row_width(C.int(d.gMax)))
 	core := make([]C.int32_t, n*g)
 	mem := make([]C.int32_t, n*g)
 	cnt := make([]C.int32_t, n)
@@ -438,7 +450,7 @@ func BuildResourceSchedulersCuda(modes []string, config ElasticSchedulerConfig) 
 	for _, m := range modes {
 		switch m {
 		case "gpushare-cuda":
-			d, err := NewCudaUnitScheduler(config, v1alpha1.ResourceGPUCore, v1alpha1.ResourceGPUMemory, 1<<20, 0)
+			d, err := NewCudaUnitScheduler(config, v1alpha1.ResourceGPUCore, v1alpha1.ResourceGPUMemory, 1<<20, 0, int(C.EGS_MAX_GPUS))
 			if err != nil {
 				return nil, err
 			}

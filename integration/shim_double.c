@@ -12,6 +12,9 @@
  *   FORGET <uid> <node|-> <C> {<core> <mem> <n> <idx>*n}...  controller.go:306 -> egs_pod_cancel (+ podMaps / released)
  *   KNOWN <uid> / RELEASED <uid>                             controller.go:314,322 (answered from the shim's own maps)
  *   STATUS                                                   routes.go:201    -> egs_state_dump
+ *
+ * argv: [policy [g_max]] -- g_max is the widest node (egs_create), EGS_MAX_GPUS by default; masks are printed as the
+ * integer EGS_MASK_BYTES(g_max) little-endian bytes hold, rows are dumped EGS_ROW_WIDTH(g_max) wide.
  */
 #include <stdint.h>
 #include <stdio.h>
@@ -21,6 +24,7 @@
 
 #define MAXN 4096
 static egs_handle *H;
+static int G_MAX = EGS_MAX_GPUS;
 static char names[MAXN][64];
 static int n_nodes = 0;
 static uint64_t known[65536], released[65536];
@@ -34,6 +38,11 @@ static uint64_t uid_key(const char *uid) {           /* FNV-1a 64, as hash/fnv i
   uint64_t h = 0xcbf29ce484222325ull;
   for (const unsigned char *p = (const unsigned char *)uid; *p; p++) { h ^= *p; h *= 0x100000001b3ull; }
   return h;
+}
+static int mask_of(const uint8_t *masks, int c) {     /* maskToIDs: container c's mask, EGS_MASK_BYTES wide */
+  int nb = EGS_MASK_BYTES(G_MAX), v = 0;
+  for (int b = 0; b < nb; b++) v |= masks[c * nb + b] << (8 * b);
+  return v;
 }
 static int has(uint64_t *set, int n, uint64_t k) { for (int i = 0; i < n; i++) if (set[i] == k) return 1; return 0; }
 static void del(uint64_t *set, int *n, uint64_t k) { for (int i = 0; i < *n; i++) if (set[i] == k) { set[i] = set[--*n]; return; } }
@@ -61,7 +70,8 @@ static int read_units_alloc(char **tok, egs_unit *u, int32_t *off, int32_t *idx)
 
 int main(int argc, char **argv) {
   int policy = argc > 1 ? atoi(argv[1]) : 0;
-  if (egs_create(policy, MAXN, EGS_MAX_GPUS, 0, &H) != EGS_OK) { fprintf(stderr, "egs_create failed\n"); return 2; }
+  if (argc > 2) G_MAX = atoi(argv[2]);
+  if (egs_create(policy, MAXN, G_MAX, 0, &H) != EGS_OK) { fprintf(stderr, "egs_create failed\n"); return 2; }
   static char line[1 << 16];
   setvbuf(stdout, NULL, _IOLBF, 1 << 16);            /* every answer line reaches the driver at once */
   while (fgets(line, sizeof line, stdin)) {
@@ -69,7 +79,7 @@ int main(int argc, char **argv) {
     char *cmd = strtok_r(line, " \n", &tok);
     if (!cmd) continue;
     egs_unit u[EGS_MAX_CONTAINERS_APPLY];
-    int32_t off[EGS_MAX_CONTAINERS_APPLY + 1], idx[64];
+    int32_t off[EGS_MAX_CONTAINERS_APPLY + 1], idx[EGS_MAX_CONTAINERS_APPLY * EGS_MAX_GPUS_WIDE];
     if (!strcmp(cmd, "NODE")) {
       char *name = strtok_r(NULL, " \n", &tok);
       long long core = atoll(strtok_r(NULL, " \n", &tok)), mem = atoll(strtok_r(NULL, " \n", &tok));
@@ -99,12 +109,12 @@ int main(int argc, char **argv) {
     } else if (!strcmp(cmd, "BIND")) {
       char *uid = strtok_r(NULL, " \n", &tok), *node = strtok_r(NULL, " \n", &tok);
       int C = read_units(&tok, u);
-      uint8_t masks[EGS_MAX_CONTAINERS] = {0};
+      uint8_t masks[2 * EGS_MAX_CONTAINERS] = {0};
       int id = node_id(node);
       int st = id < 0 ? EGS_ERR_NO_NODE : egs_bind(H, id, C, u, uid_key(uid), masks);
       if (st == EGS_OK && !has(known, n_known, uid_key(uid))) known[n_known++] = uid_key(uid);   /* d.podMaps[pod.UID] = newPod */
       printf("BIND %d", st);
-      for (int c = 0; c < C; c++) printf(" %d", st == EGS_OK ? masks[c] : 0);
+      for (int c = 0; c < C; c++) printf(" %d", st == EGS_OK ? mask_of(masks, c) : 0);
       printf("\n");
     } else if (!strcmp(cmd, "ADD")) {
       char *uid = strtok_r(NULL, " \n", &tok), *node = strtok_r(NULL, " \n", &tok);
@@ -128,25 +138,27 @@ int main(int argc, char **argv) {
       printf("RELEASED %d\n", has(released, n_released, uid_key(strtok_r(NULL, " \n", &tok))));
     } else if (!strcmp(cmd, "ROWS")) {                                /* test support: synthetic prefill (egs_state_load) */
       int id = node_id(strtok_r(NULL, " \n", &tok)), G = atoi(strtok_r(NULL, " \n", &tok));
-      int32_t c[EGS_MAX_GPUS], m[EGS_MAX_GPUS];
+      if (G < 1 || G > EGS_MAX_GPUS_WIDE) { printf("ROWS %d\n", EGS_ERR_BAD_ARG); continue; }
+      int32_t c[EGS_MAX_GPUS_WIDE], m[EGS_MAX_GPUS_WIDE];
       for (int g = 0; g < G; g++) c[g] = atoi(strtok_r(NULL, " \n", &tok));
       for (int g = 0; g < G; g++) m[g] = atoi(strtok_r(NULL, " \n", &tok));
       printf("ROWS %d\n", egs_state_load(H, id, c, m));
     } else if (!strcmp(cmd, "PEEK")) {                                /* test support: the option Assume cached (GPUIDs) */
       int id = node_id(strtok_r(NULL, " \n", &tok));
       int C = read_units(&tok, u);
-      int32_t valid = 0, score = 0; uint8_t masks[EGS_MAX_CONTAINERS] = {0};
+      int32_t valid = 0, score = 0; uint8_t masks[2 * EGS_MAX_CONTAINERS] = {0};
       egs_option_peek(H, id, C, u, &valid, &score, masks);
       printf("PEEK %d %d", valid, score);
-      for (int c = 0; c < C; c++) printf(" %d", masks[c]);
+      for (int c = 0; c < C; c++) printf(" %d", mask_of(masks, c));
       printf("\n");
     } else if (!strcmp(cmd, "STATUS")) {
-      static int32_t core[MAXN * EGS_MAX_GPUS], mem[MAXN * EGS_MAX_GPUS], cnt[MAXN], tot[MAXN];
+      static int32_t core[MAXN * EGS_MAX_GPUS_WIDE], mem[MAXN * EGS_MAX_GPUS_WIDE], cnt[MAXN], tot[MAXN];
+      const int W = EGS_ROW_WIDTH(G_MAX);
       if (n_nodes) egs_state_dump(H, 0, n_nodes, core, mem, cnt, tot);
       printf("STATUS");
       for (int i = 0; i < n_nodes; i++) {
         printf(" %s", names[i]);
-        for (int g = 0; g < cnt[i]; g++) printf(":%d,%d", core[i * EGS_MAX_GPUS + g], mem[i * EGS_MAX_GPUS + g]);
+        for (int g = 0; g < cnt[i]; g++) printf(":%d,%d", core[i * W + g], mem[i * W + g]);
       }
       printf("\n");
     }
