@@ -165,6 +165,30 @@ class OracleC:
             return None
         return _alloc_lists(off, idx, len(req)), sc.value
 
+    def peek_many(self, node_ids, req):
+        """The cached option of `req` on each of `node_ids`: (present bool [n], score int64 [n], GPU masks u16 [n, 4],
+        one per container, up to 16 GPUs)."""
+        units, nc = _units(req), len(req)
+        off, idx, sc = np.zeros(nc + 1, np.int32), np.zeros(16 * nc + 1, np.int32), C.c_int64(0)
+        offp, idxp = _ptr(off), _ptr(idx)
+        present = np.zeros(len(node_ids), bool)
+        score = np.zeros(len(node_ids), np.int64)
+        masks = np.zeros((len(node_ids), 4), np.uint16)
+        for i, n in enumerate(node_ids):
+            if self.L.egso_peek(self.h, int(n), nc, units, C.byref(sc), offp, idxp):
+                present[i], score[i] = True, sc.value
+                for c in range(nc):
+                    masks[i, c] = sum(1 << int(g) for g in idx[off[c]:off[c + 1]])
+        return present, score, masks
+
+    def trade_fits(self, node_ids, req) -> np.ndarray:
+        """Whether Trade of `req` succeeds on the current rows of each of `node_ids` (no cache effects)."""
+        units, nc = _units(req), len(req)
+        off, idx, sc = np.zeros(nc + 1, np.int32), np.zeros(16 * nc + 1, np.int32), C.c_int64(0)
+        offp, idxp = _ptr(off), _ptr(idx)
+        return np.array([self.L.egso_trade(self.h, int(n), nc, units, offp, idxp, C.byref(sc)) == 0
+                         for n in node_ids], bool)
+
     def add_pod(self, node: int, req, alloc, uid: int) -> int:
         off, idx = _alloc_arrays(alloc)
         return self.L.egso_add_pod(self.h, node, len(req), _units(req), _ptr(off), _ptr(idx), uid)

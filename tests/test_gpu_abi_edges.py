@@ -3,16 +3,14 @@ snapshot/restore, status of unknown nodes, uid rules of the batch call."""
 import numpy as np
 import pytest
 
+import oracle_c as oc
+from oracle_harness import Cluster, compare_outputs, egs
+
 pytestmark = pytest.mark.gpu
 
 
-def _eg():
-    import egs_b200
-    return egs_b200
-
-
 def test_guards_and_bad_arguments():
-    eg = _eg(); cap = eg.capi
+    eg = egs(); cap = eg.capi
     e = eg.Egs(0, 8)
     assert e.node_set_allocatable(0, 99, 10) == cap.EGS_ERR_NO_GPU            # node.go:28-30
     assert e.node_set_allocatable(0, 900, 10) == cap.EGS_ERR_BAD_ARG          # more GPUs than the row holds
@@ -33,7 +31,7 @@ def test_guards_and_bad_arguments():
 
 
 def test_whole_gpu_larger_than_node_and_sentinel_only():
-    eg = _eg()
+    eg = egs()
     e = eg.Egs(0, 2)
     assert e.node_set_allocatable(0, 200, 32) == 0
     assert list(e.filter([0], [(0, 0, 3)])) == [0]                            # 3 whole GPUs on a 2-GPU node
@@ -46,7 +44,7 @@ def test_whole_gpu_larger_than_node_and_sentinel_only():
 
 
 def test_node_replay_then_addpod_is_idempotent():
-    eg = _eg()
+    eg = egs()
     e = eg.Egs(0, 2)
     e.node_set_allocatable(0, 400, 64)
     off = np.array([0, 1], np.int32); idx = np.array([2, 0], np.int32)
@@ -63,10 +61,9 @@ def test_node_replay_then_addpod_is_idempotent():
 
 
 def test_snapshot_restore_and_uid_rules():
-    eg = _eg(); cap = eg.capi
+    eg = egs(); cap = eg.capi
     w = eg.workloads.config(1, n_nodes=64, n_pods=300)
-    e = eg.Egs(w.policy, w.n_nodes)
-    e.state_load_bulk(0, w.gpus, w.mem_total, w.core, w.mem)
+    e = Cluster.of_workload(w).handle()
     e.snapshot()
     a = e.schedule_batch(w.c_off, w.units, mode=cap.EGS_MODE_ROUNDS)
     rows_a = e.state_dump()[:2]
@@ -75,9 +72,7 @@ def test_snapshot_restore_and_uid_rules():
     assert not e.pod_known(0x8000000000000000)
     core, mem, _, _ = e.state_dump()
     assert np.array_equal(core[:, :8], w.core) and np.array_equal(mem[:, :8], w.mem)
-    b = e.schedule_batch(w.c_off, w.units, mode=cap.EGS_MODE_RESCAN)
-    for f in a:
-        assert np.array_equal(a[f], b[f]), f
+    compare_outputs(a, e.schedule_batch(w.c_off, w.units, mode=cap.EGS_MODE_RESCAN), "rescan after restore")
     assert all(np.array_equal(x, y) for x, y in zip(rows_a, e.state_dump()[:2]))
     uids = np.arange(1000, 1300, dtype=np.uint64)
     e.restore()
@@ -92,21 +87,16 @@ def test_snapshot_restore_and_uid_rules():
 
 def test_mode_switching_keeps_state_consistent():
     """rounds -> verbs -> rescan -> rounds on one handle equals the oracle doing the same sequence."""
-    import oracle_c as oc
-    eg = _eg(); cap = eg.capi
+    eg = egs(); cap = eg.capi
     w = eg.workloads.config(4, n_nodes=48, n_pods=900)
-    e = eg.Egs(w.policy, w.n_nodes)
-    e.state_load_bulk(0, w.gpus, w.mem_total, w.core, w.mem)
-    o = oc.OracleC(w.policy)
-    for n in range(w.n_nodes):
-        o.add_node(800, 8 * w.mem_total); o.set_rows(n, w.core[n], w.mem[n])
+    cl = Cluster.of_workload(w)
+    e, o = cl.handle(), cl.oracle()
     u64 = w.units64()
     for lo, hi, mode in [(0, 300, cap.EGS_MODE_ROUNDS), (300, 600, cap.EGS_MODE_RESCAN), (600, 900, cap.EGS_MODE_ROUNDS)]:
         off = w.c_off[lo:hi + 1] - w.c_off[lo]
         ref = o.schedule_batch(off, u64[w.c_off[lo]:w.c_off[hi]], uids=np.arange(lo, hi, dtype=np.uint64))
         got = e.schedule_batch(off, w.units[w.c_off[lo]:w.c_off[hi]], uids=np.arange(lo, hi, dtype=np.uint64), mode=mode)
-        for f in ref:
-            assert np.array_equal(ref[f], got[f]), (lo, f)
+        compare_outputs(ref, got, f"pods from {lo}")
         req = [tuple(int(x) for x in w.units[w.c_off[hi - 1]])]
         assert list(e.filter(None, req)) == list(o.filter(None, req))          # verbs see the tables the batch left
         assert list(e.score(None, req)[1]) == [int(x) for x in o.score(None, req)[1]]
@@ -116,7 +106,7 @@ def test_node_reload_after_auto_uid_batch_drops_pods_map():
     """A batch with library-assigned uids keeps podsMap membership in the batch's result arrays; reloading the node
     (a fresh NodeAllocator, node.go:42-50) must drop it all the same: a later ForgetPod of such a uid is a no-op on
     the rows (node.go:131) and a bind with that uid transacts again (node.go:149)."""
-    eg = _eg()
+    eg = egs()
     e = eg.Egs(0, 1)
     e.node_set_allocatable(0, 200, 32)
     c_off = np.array([0, 1], np.int32)
@@ -137,18 +127,12 @@ def test_auto_uid_bound_again_elsewhere_then_forgotten_is_unknown():
     """A pod with a library-assigned uid U won node 0 in a batch; then Bind puts U on node 1 as well (podMaps[U] is set
     again without a check, scheduler.go:224).  ForgetPod on node 1 deletes U from podMaps (scheduler.go:261-264), so
     U is no longer known, while node 0's podsMap still holds it and a ForgetPod there cancels node 0's rows."""
-    import oracle_c as oc
-    eg = _eg()
+    eg = egs()
     U = 0x8000000000000000
     req = [(20, 4, 0)]
     c_off = np.array([0, 1], np.int32)
-    e = eg.Egs(0, 2)
-    o = oc.OracleC(0)
-    for n in range(2):
-        assert e.node_set_allocatable(n, 200, 32) == 0
-        o.add_node(200, 32)
-    assert e.state_load(0, [60, 100], [10, 16]) == 0                          # node 0 the fuller: binpack picks it
-    o.set_rows(0, [60, 100], [10, 16])
+    cl = Cluster(0, [(2, 16, ([60, 100], [10, 16])), (2, 16, None)])         # node 0 the fuller: binpack picks it
+    e, o = cl.handle(), cl.oracle()
     got = e.schedule_batch(c_off, np.array(req, np.int32), mode=eg.capi.EGS_MODE_ROUNDS)   # uids == NULL: U
     ref = o.schedule_batch(c_off, np.array(req, np.int64), uids=np.array([U], np.uint64))
     assert got["node"][0] == ref["node"][0] == 0 and got["status"][0] == ref["status"][0] == 0
@@ -170,8 +154,7 @@ def test_accounting_verbs_take_pods_with_up_to_8_containers():
     that ANOTHER scheduler placed must be subtracted from the node cache exactly like the reference does (AddPod,
     replay at node load, ForgetPod, the bulk mutation stream) even though this library's filter / score / bind stop at
     4 containers -- otherwise a restarted scheduler would over-commit the node."""
-    import oracle_c as oc
-    eg = _eg(); cap = eg.capi
+    eg = egs(); cap = eg.capi
     req = [(-1, -1, 0), (30, 4, 0), (-1, -1, 0), (0, 0, 2), (-1, -1, 0), (20, 2, 0)]
     alloc = [[0], [1], [1], [2, 3], [3], [1]]
     o = oc.OracleC(0)

@@ -4,41 +4,20 @@ checked against the oracle doing the same thing call by call."""
 import numpy as np
 import pytest
 
-import oracle_c as oc
+from oracle_harness import FIELDS, Cluster, compare_outputs, compare_rows, egs
 
 pytestmark = pytest.mark.gpu
 
-FIELDS = ["node", "status", "alloc_mask", "fit_count", "fit_digest", "score_digest"]
-
-
-def _eg():
-    import egs_b200
-    return egs_b200
-
 
 def _pair(w):
-    eg = _eg()
-    e = eg.Egs(w.policy, w.n_nodes)
-    e.state_load_bulk(0, w.gpus, w.mem_total, w.core, w.mem)
-    o = oc.OracleC(w.policy)
-    for n in range(w.n_nodes):
-        o.add_node(100 * w.gpus, w.mem_total * w.gpus)
-        o.set_rows(n, w.core[n], w.mem[n])
-    return e, o
-
-
-def _rows_equal(e, o, w, nodes):
-    core, mem, _, _ = e.state_dump()
-    for n in nodes:
-        r = o.rows(n)
-        assert [int(x) for x in core[n, :w.gpus]] == [x[0] for x in r], n
-        assert [int(x) for x in mem[n, :w.gpus]] == [x[1] for x in r], n
+    cl = Cluster.of_workload(w)
+    return cl.handle(), cl.oracle()
 
 
 def test_bulk_replay_of_assumed_pods_single_launch():
     """scheduler.go:86-106 / node.go:52-54: a restarted scheduler replays every assumed pod onto its node.  10^5
     records (some not fitting any more, some duplicated uids, a few ForgetPods in between) in ONE launch."""
-    eg = _eg(); cap = eg.capi
+    eg = egs(); cap = eg.capi
     w = eg.workloads.config(4, n_nodes=10_000, n_pods=1)
     e, o = _pair(w)
     rng = np.random.default_rng(7)
@@ -66,7 +45,7 @@ def test_bulk_replay_of_assumed_pods_single_launch():
         live.append((uid, node, req, alloc))
     before = e.profile_get(0)
     assert e.mutations_apply(recs) == 0
-    _rows_equal(e, o, w, range(w.n_nodes))
+    compare_rows(e, o, range(w.n_nodes))
     for uid, _, _, _ in live[:200]:
         assert e.pod_known(uid) == o.known_pod(uid)
     assert before == e.profile_get(0)
@@ -76,7 +55,7 @@ def test_batch_with_ten_percent_mutations_interleaved():
     """50 000 pods with ~5 000 AddPod / ForgetPod records woven in at fixed pod positions: the oracle runs segment by
     segment with the single-pod verbs in between (the order the reference's lock gives), the GPU takes the whole
     stream in one call."""
-    eg = _eg(); cap = eg.capi
+    eg = egs(); cap = eg.capi
     w = eg.workloads.config(4, n_nodes=2_000, n_pods=50_000)
     e, o = _pair(w)
     rng = np.random.default_rng(11)
@@ -96,7 +75,7 @@ def test_batch_with_ten_percent_mutations_interleaved():
         for i in range(seg.n_pods):
             if r["status"][i] == 0:
                 req = [tuple(int(x) for x in seg.units[k]) for k in range(int(seg.c_off[i]), int(seg.c_off[i + 1]))]
-                alloc = [[g for g in range(8) if r["alloc_mask"][i][c] >> g & 1] for c in range(len(req))]
+                alloc = cap.masks_to_lists(r["alloc_mask"][i], len(req))
                 bound.append((int(uids[prev + i]), int(r["node"][i]), req, alloc))
         prev = cut
         if cut == P:
@@ -113,8 +92,6 @@ def test_batch_with_ten_percent_mutations_interleaved():
             recs.append((cap.EGS_MUT_ADD, node, req, alloc, 5_000_000 + ext)); mut_at.append(cut)
             o.add_pod(node, req, alloc, 5_000_000 + ext)
     got = e.schedule_batch_mut(w.c_off, w.units, mut_at, recs, uids=uids)
-    for f in FIELDS:
-        want = np.concatenate(ref[f])
-        assert np.array_equal(want, got[f]), f"{f} differs at pod {np.argwhere(want != got[f])[:3]}"
-    _rows_equal(e, o, w, range(w.n_nodes))
+    compare_outputs({f: np.concatenate(ref[f]) for f in FIELDS}, got, "batch with mutations")
+    compare_rows(e, o, range(w.n_nodes))
     assert len(recs) > 4_000

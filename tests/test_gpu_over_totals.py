@@ -16,19 +16,15 @@ RESCAN gives the same outputs, and egs_filter / egs_score of every whole-GPU sha
 The guard case drives rows and requests to the limits of DESIGN §1 through the cold evaluate, select, the fast /
 general / leaf-parallel resolver paths, RESCAN and schedule_batch_vec.
 """
-import threading
-
 import numpy as np
 import pytest
 
-import oracle_c as oc
-from test_gpu_round_sets import Batch, _check_paths, _compare_caches, _compare_outputs, _compare_rows, _delta, \
-    _distinct_shapes, _pods
+from oracle_harness import Cluster, compare_caches, compare_outputs, compare_rows, compare_shards, egs, run_sharded
+from round_batches import Batch, check_paths, distinct_shapes, pod_picks, stats_delta
+from rounds_cases import FRAC11, OVER, SIDECAR, WHOLE1, over_totals_shapes
 
 pytestmark = pytest.mark.gpu
 
-SIDECAR, WHOLE1, FRAC11 = ((-1, -1, 0),), ((0, 0, 1),), ((1, 1, 0),)
-OVER = (0, 0, 1, 1, 1, 2, 3)                 # how far a GPU is above its totals, per row
 MEMS = (16384, 40960, 81920)                 # MiB per GPU
 MAX_CORE, MAX_MEM = 1 << 20, 1 << 25         # EGS_MAX_CORE_LOAD, EGS_MAX_MEM_PER_GPU
 # Pod uids, one range per source.  Every batch passes its uids: without them the oracle numbers each batch's pods
@@ -37,43 +33,9 @@ MAX_CORE, MAX_MEM = 1 << 20, 1 << 25         # EGS_MAX_CORE_LOAD, EGS_MAX_MEM_PE
 UID_RECORDS, UID_SIDECAR, UID_BATCH = 1 << 40, 1 << 41, 1 << 42
 
 
-def _egs():
-    import egs_b200
-    return egs_b200
-
-
-def _cap():
-    return _egs().capi
-
-
-# ------------------------------------------------------------------------------------------------ the two sides
-class Cluster:
-    """nodes: [(gpu_count, mem_total, rows or None)].  The same cluster on a library handle and on the oracle."""
-
-    def __init__(self, policy, nodes):
-        self.policy, self.nodes = policy, nodes
-
-    def handle(self, world=1, rank=0):
-        e = _egs().Egs(self.policy, len(self.nodes))
-        if world > 1:
-            e.shard_set(rank, world)
-        for n, (g, mt, rows) in enumerate(self.nodes):
-            assert e.node_set_allocatable(n, 100 * g, mt * g) == 0
-            if rows is not None:
-                assert e.state_load(n, rows[0], rows[1]) == 0
-        return e
-
-    def oracle(self):
-        o = oc.OracleC(self.policy)
-        for n, (g, mt, rows) in enumerate(self.nodes):
-            assert o.add_node(100 * g, mt * g) == n
-            if rows is not None:
-                o.set_rows(n, rows[0], rows[1])
-        return o
-
-    def over_nodes(self, o):
-        """Nodes with a GPU above its totals on the oracle's rows now."""
-        return {n for n, (g, mt, _) in enumerate(self.nodes) if any(c > 100 or m > mt for c, m in o.rows(n))}
+def _over_nodes(cl, o):
+    """Nodes with a GPU above its totals on the oracle's rows now."""
+    return {n for n, (g, mt, _) in enumerate(cl.nodes) if any(c > 100 or m > mt for c, m in o.rows(n))}
 
 
 def _forget_records(rng, cl, uid0):
@@ -85,7 +47,7 @@ def _forget_records(rng, cl, uid0):
             a, b = int(rng.choice(OVER)), int(rng.choice(OVER))
             if (a or b) and rng.integers(0, 4):
                 req, alloc = [(0, 0, 1), (a, b, 0)], [[gi], [gi]]
-                recs += [(_cap().EGS_MUT_ADD, n, req, alloc, uid), (_cap().EGS_MUT_FORGET, n, req, alloc, uid)]
+                recs += [(egs().capi.EGS_MUT_ADD, n, req, alloc, uid), (egs().capi.EGS_MUT_FORGET, n, req, alloc, uid)]
                 uid += 1
     return recs
 
@@ -95,7 +57,7 @@ def _apply_records(e, o, recs, verbs):
     not at all (the caller passes them to egs_schedule_batch_mut)."""
     verbs = verbs and e is not None
     for kind, n, req, alloc, uid in recs:
-        if kind == _cap().EGS_MUT_ADD:
+        if kind == egs().capi.EGS_MUT_ADD:
             assert o.add_pod(n, req, alloc, uid) == 0
             if verbs:
                 assert e.pod_apply(n, req, alloc, uid) == 0
@@ -144,11 +106,11 @@ def _run_route(cl, route, b, pre=None, threads=4):
     pre(e, o) brings a handle (e is None: the oracle alone) to the batch's starting state and returns mutation
     records for egs_schedule_batch_mut (route "stream") or None.  Returns (ref outputs, ROUNDS stats delta, nodes
     above their totals at batch start)."""
-    cap = _cap()
-    shapes = _distinct_shapes(b)
+    cap = egs().capi
+    shapes = distinct_shapes(b)
     o = cl.oracle()
     pre(None, o)
-    over = cl.over_nodes(o)
+    over = _over_nodes(cl, o)
     uids = np.arange(UID_BATCH, UID_BATCH + b.n_pods, dtype=np.uint64)
     ref = o.schedule_batch(b.c_off, b.units.astype(np.int64), uids=uids, threads=threads)
     for mode in (cap.EGS_MODE_ROUNDS, cap.EGS_MODE_RESCAN):
@@ -160,11 +122,11 @@ def _run_route(cl, route, b, pre=None, threads=4):
             got = e.schedule_batch_mut(b.c_off, b.units, np.zeros(len(recs_e), np.int32), recs_e, uids=uids, mode=mode)
         else:
             got = e.schedule_batch(b.c_off, b.units, uids=uids, mode=mode)
-        _compare_outputs(ref, got, f"{route} mode {mode}")
+        compare_outputs(ref, got, f"{route} mode {mode}")
         if mode == cap.EGS_MODE_ROUNDS:
-            d = _delta(e.rounds_stats(), s0)
-            _compare_rows(e, o, len(cl.nodes))
-            _compare_caches(e, o, shapes, range(len(cl.nodes)), unfit_check=True)
+            d = stats_delta(e.rounds_stats(), s0)
+            compare_rows(e, o, range(len(cl.nodes)))
+            compare_caches(e, o, shapes, range(len(cl.nodes)), unfit_check=True)
             # the verbs read the option table the batch left behind (egs_filter / egs_score trust its memos);
             # `o` is the oracle after the batch, so it answers the same filter / score questions
             _check_whole_verbs(e, o, shapes, len(cl.nodes))
@@ -185,13 +147,13 @@ def _min_pre(route):
     req, alloc = [(0, 0, 1), (1, 1, 0)], [[0], [0]]
 
     def pre(e, o):
-        cap = _cap()
+        cap = egs().capi
         if route == "sidecar":                                    # a batch of one sidecar pod
             sb = _min_batch(0, [SIDECAR])
             uids = np.array([UID_SIDECAR], np.uint64)
             r = o.schedule_batch(sb.c_off, sb.units.astype(np.int64), uids=uids)
             if e is not None:
-                _compare_outputs(r, e.schedule_batch(sb.c_off, sb.units, uids=uids, mode=cap.EGS_MODE_ROUNDS), "sidecar batch")
+                compare_outputs(r, e.schedule_batch(sb.c_off, sb.units, uids=uids, mode=cap.EGS_MODE_ROUNDS), "sidecar batch")
         elif route == "load":
             o.set_rows(0, [101], [17])
             if e is not None:
@@ -219,25 +181,6 @@ def test_minimal_whole_gpu_fits_again(route, policy):
 
 
 # ------------------------------------------------------------------------------------------------ random clusters
-def _over_shapes(rng, n):
-    """n distinct shapes, every request >= 0: WHOLE1 and FRAC11 first, then whole-GPU containers of count 1 or 2
-    (alone or with one small fractional container) and 1-3 fractional containers of 0-3 core and 0-3 MiB."""
-    def frac():
-        while True:
-            u = (int(rng.choice(OVER)), int(rng.choice(OVER)), 0)
-            if u[0] or u[1]:
-                return u
-    out = [WHOLE1, FRAC11]
-    while len(out) < n:
-        if rng.integers(0, 2):
-            sh = ((0, 0, int(rng.integers(1, 3))),) + ((frac(),) if rng.integers(0, 3) == 0 else ())
-        else:
-            sh = tuple(frac() for _ in range(int(rng.integers(1, 4))))
-        if sh not in out:
-            out.append(sh)
-    return out
-
-
 def _over_cluster(rng, n_nodes, route):
     """Route "load": every GPU at or just above its totals, a few partly used.  Other routes: a free cluster."""
     nodes = []
@@ -257,8 +200,8 @@ def _over_case(seed, route, n_shapes, n_nodes=160, n_pods=2000):
     rng = np.random.default_rng(seed)
     policy = seed % 2
     cl = Cluster(policy, _over_cluster(rng, n_nodes, route))
-    shapes = _over_shapes(rng, n_shapes)
-    b = Batch(policy, cl.nodes, shapes, _pods(rng, shapes, n_pods, "trickle" if n_shapes > 96 else "front"))
+    shapes = over_totals_shapes(rng, n_shapes)
+    b = Batch(policy, cl.nodes, shapes, pod_picks(rng, shapes, n_pods, "trickle" if n_shapes > 96 else "front"))
     recs = _forget_records(rng, cl, UID_RECORDS) if route in ("verbs", "stream") else []
     side_seed = seed + 1
 
@@ -284,7 +227,7 @@ def test_random_clusters_above_totals(route, inst):
     n_shapes = GEOMETRIES[inst]
     cl, b, pre = _over_case(100 * n_shapes + len(route), route, n_shapes)
     ref, d, over = _run_route(cl, route, b, pre)
-    _check_paths(d, n_shapes, b.n_pods)
+    check_paths(d, n_shapes, b.n_pods)
     n = _regime(ref, b, over)
     print(f"{route} {inst}: {d} over={len(over)} whole-GPU wins above totals={n}")
     assert n > 0, "no whole-GPU pod won on a node above its totals"
@@ -328,7 +271,7 @@ def test_int32_guard_limits(policy):
     shapes (a monotone round set: cold evaluate, select, fast pods); batch 2 every shape (general pods and the
     leaf-parallel Trade on the same state).  Outputs, rows and caches (option_dump scores) against the oracle; RESCAN
     and schedule_batch_vec element for element.  Under binpack the largest score seen must pass 1.5e9."""
-    cap = _cap()
+    cap = egs().capi
     rng = np.random.default_rng(2 ** 25 + policy)
     cl = Cluster(policy, _guard_cluster(rng, 300))
     shapes = _guard_shapes(rng)
@@ -344,18 +287,18 @@ def test_int32_guard_limits(policy):
         uid += b.n_pods
         n_vec = 64
         ref = o.schedule_batch(b.c_off, b.units.astype(np.int64), uids=uids, threads=4, vec_pods=n_vec)
-        _compare_outputs(ref, e.schedule_batch(b.c_off, b.units, uids=uids, mode=cap.EGS_MODE_ROUNDS), f"rounds batch {k}")
-        _compare_outputs(ref, r.schedule_batch(b.c_off, b.units, uids=uids, mode=cap.EGS_MODE_RESCAN), f"rescan batch {k}")
+        compare_outputs(ref, e.schedule_batch(b.c_off, b.units, uids=uids, mode=cap.EGS_MODE_ROUNDS), f"rounds batch {k}")
+        compare_outputs(ref, r.schedule_batch(b.c_off, b.units, uids=uids, mode=cap.EGS_MODE_RESCAN), f"rescan batch {k}")
         got = v.schedule_batch_vec(b.c_off, b.units, n_vec, uids=uids)
-        _compare_outputs(ref, got, f"vec batch {k}")
+        compare_outputs(ref, got, f"vec batch {k}")
         assert np.array_equal(ref["vec_fit"], got["vec_fit"]), f"vec_fit batch {k}"
         fit = ref["vec_fit"] == 1
         assert np.array_equal(ref["vec_score"][fit], got["vec_score"][fit]), f"vec_score batch {k}"
         top = max(top, int(got["vec_score"][fit].max(initial=0)))
-        _compare_rows(e, o, len(cl.nodes))
-        _compare_rows(r, o, len(cl.nodes))
-        _compare_caches(e, o, _distinct_shapes(b), range(len(cl.nodes)), unfit_check=True)
-        for sh in _distinct_shapes(b):
+        compare_rows(e, o, range(len(cl.nodes)))
+        compare_rows(r, o, range(len(cl.nodes)))
+        compare_caches(e, o, distinct_shapes(b), range(len(cl.nodes)), unfit_check=True)
+        for sh in distinct_shapes(b):
             st, sc, _ = e.option_dump(list(sh))
             top = max(top, int(sc[st == 1].max(initial=0)))
         if k == 0:
@@ -373,33 +316,7 @@ def test_int32_guard_limits(policy):
 def test_sharded_above_totals_equal_unsharded(world):
     """The over-totals batch ("load" route, 64 shapes) on an in-process shard group (egs_comm_init_local, one thread
     per rank): every rank's outputs equal the unsharded run, every shard's rows the unsharded rows."""
-    cap = _cap()
     cl, b, _ = _over_case(7000 + world, "load", 64, n_nodes=400, n_pods=3000)
-    e0 = cl.handle()
-    ref = e0.schedule_batch(b.c_off, b.units, mode=cap.EGS_MODE_ROUNDS)
-    ref_core, ref_mem, _, _ = e0.state_dump()
-    e0.close()
-    o = cl.oracle()
-    _compare_outputs(o.schedule_batch(b.c_off, b.units.astype(np.int64), threads=4), ref, "unsharded")
-    hs = [cl.handle(world, r) for r in range(world)]
-    cap.comm_init_local(hs)
-    outs, errs = [None] * world, []
-
-    def run(r):
-        try:
-            outs[r] = hs[r].schedule_batch(b.c_off, b.units, mode=cap.EGS_MODE_ROUNDS)
-        except Exception as ex:   # pragma: no cover
-            errs.append(repr(ex))
-    th = [threading.Thread(target=run, args=(r,)) for r in range(world)]
-    for t in th:
-        t.start()
-    for t in th:
-        t.join(timeout=600)
-    assert not errs, errs
-    for r in range(world):
-        _compare_outputs(ref, outs[r], f"world {world}, rank {r}")
-        lo, hi = cap.shard_range(len(cl.nodes), r, world)
-        core, mem, _, _ = hs[r].state_dump(lo, hi - lo)
-        assert np.array_equal(core, ref_core[lo:hi]) and np.array_equal(mem, ref_mem[lo:hi]), f"rows of shard {r}"
-    for h in hs:
-        h.close()
+    ref, rows, ranks = run_sharded(cl.handle, world, b.c_off, b.units)
+    compare_outputs(cl.oracle().schedule_batch(b.c_off, b.units.astype(np.int64), threads=4), ref, "unsharded")
+    compare_shards(ref, rows, ranks, f"world {world}")

@@ -4,21 +4,17 @@ import pytest
 
 import oracle_c as oc
 from ka_vectors import KA0_FINAL, KA0_MEM, KA0_TRACE, TRADE_KA
+from oracle_harness import Cluster, compare_caches, compare_outputs, compare_rows, egs
 from scenario import CBackend, GpuBackend, make_scenario, run_scenario
 
 pytestmark = pytest.mark.gpu
 
-FIELDS = ["node", "status", "alloc_mask", "fit_count", "fit_digest", "score_digest"]
-
-
-def _egs():
-    import egs_b200
-    return egs_b200
+KA0_CLUSTER = Cluster(0, [(2, 16, None)] * 4)          # config 0: four nodes of two 16 MiB GPUs, binpack
 
 
 @pytest.mark.parametrize("name,policy,mt,rows,req,exp", TRADE_KA, ids=[k[0] for k in TRADE_KA])
 def test_trade_ka_gpu(name, policy, mt, rows, req, exp):
-    e = _egs().Egs(policy, 4)
+    e = egs().Egs(policy, 4)
     assert e.node_set(0, len(rows), mt) == 0
     assert e.state_load(0, [r[0] for r in rows], [r[1] for r in rows]) == 0
     fit = e.filter([0], req)
@@ -29,16 +25,12 @@ def test_trade_ka_gpu(name, policy, mt, rows, req, exp):
 
 @pytest.mark.parametrize("mode", [1, 2])
 def test_ka0_batch(mode):
-    eg = _egs()
-    w = eg.workloads.config(0)
-    e = eg.Egs(0, 4)
-    for n in range(4):
-        assert e.node_set_allocatable(n, 200, 32) == 0
+    w = egs().workloads.config(0)
+    e = KA0_CLUSTER.handle()
     out = e.schedule_batch(w.c_off, w.units, mode=mode)
     for p, (fit, scores, node, status, alloc) in enumerate(KA0_TRACE):
         assert out["node"][p] == node and out["status"][p] == status and out["fit_count"][p] == sum(fit)
-        got = [g for g in range(8) if out["alloc_mask"][p][0] >> g & 1]
-        assert got == (alloc[0] if alloc else [])
+        assert egs().capi.masks_to_lists(out["alloc_mask"][p], 1) == [alloc[0] if alloc else []]
     assert [e.rows(i) for i in range(4)] == KA0_FINAL
     assert e.pod_known(0x8000000000000000 + 6) and not e.pod_known(0x8000000000000000 + 7)
 
@@ -52,59 +44,40 @@ def test_scenarios_gpu_vs_oracle(seed, policy):
     assert a == b
 
 
-def _oracle_for(w):
-    o = oc.OracleC(w.policy)
-    for n in range(w.n_nodes):
-        o.add_node(100 * w.gpus, w.mem_total * w.gpus)
-        o.set_rows(n, w.core[n], w.mem[n])
-    return o
-
-
-def _gpu_for(w, world=1):
-    eg = _egs()
-    e = eg.Egs(w.policy, w.n_nodes)
-    e.state_load_bulk(0, w.gpus, w.mem_total, w.core, w.mem)
-    return e
-
-
 def _compare_batch(w, mode, threads=1):
-    o = _oracle_for(w)
+    cl = Cluster.of_workload(w)
+    o = cl.oracle()
     ref = o.schedule_batch(w.c_off, w.units64(), threads=threads)
-    e = _gpu_for(w)
+    e = cl.handle()
     got = e.schedule_batch(w.c_off, w.units, mode=mode)
-    for f in FIELDS:
-        assert np.array_equal(ref[f], got[f]), f"{f} differs at pod {np.argwhere(ref[f] != got[f])[:3]}"
-    core, mem, _, _ = e.state_dump()
-    for n in range(w.n_nodes):
-        rows = o.rows(n)
-        assert [int(x) for x in core[n, :w.gpus]] == [r[0] for r in rows]
-        assert [int(x) for x in mem[n, :w.gpus]] == [r[1] for r in rows]
+    compare_outputs(ref, got, f"config {w.cfg} mode {mode}")
+    compare_rows(e, o, range(w.n_nodes))
     return ref, got, e, o
 
 
 @pytest.mark.parametrize("mode", [1, 2])
 def test_cfg1_full(mode):
     """BASELINE config 1 at full size: 1000 nodes x 8 GPUs, 10000 pods, binpack."""
-    _compare_batch(_egs().workloads.config(1), mode)
+    _compare_batch(egs().workloads.config(1), mode)
 
 
 @pytest.mark.parametrize("mode", [1, 2])
 def test_cfg2_prefix(mode):
     """config 2 (spread, core+memory): 10000 nodes, first 20000 pods against the oracle."""
-    _compare_batch(_egs().workloads.config(2, n_pods=20000), mode, threads=4)
+    _compare_batch(egs().workloads.config(2, n_pods=20000), mode, threads=4)
 
 
 @pytest.mark.parametrize("policy", [1, 0])
 @pytest.mark.parametrize("mode", [1, 2])
 def test_cfg3_multi_container_prefix(mode, policy):
     """config 3 (2-3 containers per pod): 50000 nodes, first 1500 pods, spread as named + binpack."""
-    _compare_batch(_egs().workloads.config(3, n_pods=1500, policy=policy), mode)
+    _compare_batch(egs().workloads.config(3, n_pods=1500, policy=policy), mode)
 
 
 @pytest.mark.parametrize("mode", [1, 2])
 def test_cfg4_prefix(mode):
     """config 4: 100000 nodes, first 3000 pods against the oracle (4-worker filter like scheduler.go:135)."""
-    _compare_batch(_egs().workloads.config(4, n_pods=3000), mode, threads=4)
+    _compare_batch(egs().workloads.config(4, n_pods=3000), mode, threads=4)
 
 
 def _late_window(cfg, policy, K, W, threads=4, sample=4000):
@@ -112,9 +85,9 @@ def _late_window(cfg, policy, K, W, threads=4, sample=4000):
     loaded into a FRESH oracle (egso_cache_load); both then schedule pods [K, K+W) and must agree on all six
     outputs, the final rows and the final caches.  This puts the oracle into the late, full-cluster regime
     (stale options, bind failures, unfit nodes) that a prefix from an empty cluster never reaches."""
-    eg = _egs()
+    eg = egs()
     full = eg.workloads.config(cfg, n_pods=K + W, policy=policy)
-    e = _gpu_for(full)
+    e = Cluster.of_workload(full).handle()
     pre = full.prefix(K)
     e.schedule_batch(pre.c_off, pre.units, mode=2)
     core, mem, _, _ = e.state_dump()
@@ -131,23 +104,11 @@ def _late_window(cfg, policy, K, W, threads=4, sample=4000):
     assert n_cached > 0
     win = eg.workloads.window(full, K, W)
     ref = o.schedule_batch(win.c_off, win.units64(), threads=threads)
-    got = e.schedule_batch(win.c_off, win.units, mode=2)
-    for f in FIELDS:
-        assert np.array_equal(ref[f], got[f]), f"cfg{cfg} K={K}: {f} differs at pod {np.argwhere(ref[f] != got[f])[:3]}"
-    core, mem, _, _ = e.state_dump()
+    compare_outputs(ref, e.schedule_batch(win.c_off, win.units, mode=2), f"cfg{cfg} K={K}")
     rng = np.random.default_rng(K)
     nodes = set(int(x) for x in rng.integers(0, full.n_nodes, sample)) | set(int(x) for x in ref["node"] if x >= 0)
-    dumps = {sh: e.option_dump(list(sh)) for sh in shapes}
-    for n in nodes:
-        rows = o.rows(n)
-        assert [int(x) for x in core[n, :full.gpus]] == [r[0] for r in rows]
-        assert [int(x) for x in mem[n, :full.gpus]] == [r[1] for r in rows]
-        for sh in shapes:
-            st, sc, am = dumps[sh]
-            pk = o.peek(n, list(sh))
-            assert (pk is not None) == (st[n] == 1), f"cache presence differs node {n} shape {sh}"
-            if pk is not None:
-                assert pk[1] == int(sc[n]) and pk[0] == [[g for g in range(8) if am[n, c] >> g & 1] for c in range(len(sh))]
+    compare_rows(e, o, nodes)
+    compare_caches(e, o, shapes, nodes, unfit_check=True)
     return ref
 
 
@@ -171,21 +132,12 @@ def test_cfg2_late_windows(K):
 def test_full_fit_and_score_vectors(cfg, n_pods, vec_pods):
     """SURVEY 8d: on configs 0-2 the FULL per-pod fit mask and score vector (what /scheduler/filter and
     /scheduler/priorities return for every candidate node) are compared element-wise with the oracle."""
-    eg = _egs()
-    w = eg.workloads.config(cfg, n_pods=n_pods)
-    if cfg == 0:
-        e = eg.Egs(0, 4)
-        o = oc.OracleC(0)
-        for n in range(4):
-            assert e.node_set_allocatable(n, 200, 32) == 0
-            o.add_node(200, 32)
-    else:
-        e = _gpu_for(w)
-        o = _oracle_for(w)
+    w = egs().workloads.config(cfg, n_pods=n_pods)
+    cl = KA0_CLUSTER if cfg == 0 else Cluster.of_workload(w)
+    e, o = cl.handle(), cl.oracle()
     ref = o.schedule_batch(w.c_off, w.units64(), vec_pods=vec_pods)
     got = e.schedule_batch_vec(w.c_off, w.units, vec_pods)
-    for f in FIELDS:
-        assert np.array_equal(ref[f], got[f]), f
+    compare_outputs(ref, got, f"config {cfg}")
     assert np.array_equal(ref["vec_fit"], got["vec_fit"])
     assert np.array_equal(ref["vec_score"], got["vec_score"])
     assert got["vec_fit"].sum() > 0
@@ -193,7 +145,7 @@ def test_full_fit_and_score_vectors(cfg, n_pods, vec_pods):
 
 def test_pressure_small_cluster():
     """Few nodes, many pods: nodes fill up, unfit nodes and stale-option bind failures appear."""
-    eg = _egs()
+    eg = egs()
     for cfg, pol in [(1, 0), (2, 1), (4, 0), (3, 1), (3, 0)]:
         w = eg.workloads.config(cfg, n_nodes=40, n_pods=4000, policy=pol)
         for mode in (1, 2):
@@ -225,14 +177,12 @@ def _conservation(w, out, e):
 def test_full_size_properties(cfg):
     """Full BASELINE sizes (cfg2: 10k nodes/100k pods; cfg4: 100k nodes/1M pods): the two
     independent device loops (per-pod rescan, rounds) agree on every output, and resources are conserved."""
-    eg = _egs()
-    w = eg.workloads.config(cfg)
-    e1 = _gpu_for(w)
-    a = e1.schedule_batch(w.c_off, w.units, mode=1)
-    e2 = _gpu_for(w)
+    w = egs().workloads.config(cfg)
+    cl = Cluster.of_workload(w)
+    a = cl.handle().schedule_batch(w.c_off, w.units, mode=1)
+    e2 = cl.handle()
     b = e2.schedule_batch(w.c_off, w.units, mode=2)
-    for f in FIELDS:
-        assert np.array_equal(a[f], b[f]), f
+    compare_outputs(a, b, f"config {cfg} rounds against rescan")
     _conservation(w, b, e2)
     assert (b["status"] != 1).all()   # the named clusters have room for every pod (no NOFIT);
     # status 3 (stale cached option, gpu.go:158-168) is reference behaviour and does occur under spread
@@ -241,21 +191,15 @@ def test_full_size_properties(cfg):
 def _random_batch(seed, n_nodes, n_pods, n_shapes, policy):
     """Mixed shapes: fractional, whole-GPU (count 1..2), -1 sentinel containers, 1..4 containers per pod;
     heterogeneous nodes (G in 1,2,4,8).  Non-monotone rounds: sentinel units ADD 1 to a GPU (gpu.go:36-37)."""
-    import oracle_c as oc
     rng = np.random.default_rng(seed)
-    eg = _egs()
-    e = eg.Egs(policy, n_nodes)
-    o = oc.OracleC(policy)
+    nodes = []
     for n in range(n_nodes):
         g = int(rng.choice([1, 2, 4, 8]))
         m = int(rng.choice([16, 40, 80]))
-        assert o.add_node(100 * g, m * g) == n
-        assert e.node_set_allocatable(n, 100 * g, m * g) == 0
+        rows = None
         if rng.integers(0, 2):
-            core = [int(rng.choice([100, 100, 60, 30, 0])) for _ in range(g)]
-            mem = [int(rng.integers(0, m + 1)) for _ in range(g)]
-            o.set_rows(n, core, mem)
-            assert e.state_load(n, core, mem) == 0
+            rows = ([int(rng.choice([100, 100, 60, 30, 0])) for _ in range(g)], [int(rng.integers(0, m + 1)) for _ in range(g)])
+        nodes.append((g, m, rows))
     shapes = []
     for _ in range(n_shapes):
         c = int(rng.integers(1, 5))
@@ -275,21 +219,16 @@ def _random_batch(seed, n_nodes, n_pods, n_shapes, policy):
     for s in pick:
         units.extend(shapes[int(s)])
         c_off.append(len(units))
-    return e, o, np.array(c_off, np.int32), np.array(units, np.int32)
+    return Cluster(policy, nodes), np.array(c_off, np.int32), np.array(units, np.int32)
 
 
 @pytest.mark.parametrize("policy", [0, 1])
 @pytest.mark.parametrize("seed,n_nodes,n_pods,n_shapes", [(1, 50, 3000, 6), (2, 300, 4000, 12), (3, 2000, 3000, 40), (4, 20, 2000, 3)])
 def test_batch_mixed_shapes_vs_oracle(seed, n_nodes, n_pods, n_shapes, policy):
+    cl, c_off, units = _random_batch(seed, n_nodes, n_pods, n_shapes, policy)
     for mode in (1, 2):
-        e, o, c_off, units = _random_batch(seed, n_nodes, n_pods, n_shapes, policy)
+        e, o = cl.handle(), cl.oracle()
         ref = o.schedule_batch(c_off, units.astype(np.int64))
-        got = e.schedule_batch(c_off, units, mode=mode)
-        for f in FIELDS:
-            assert np.array_equal(ref[f], got[f]), f"mode {mode}: {f} differs first at pod {np.argwhere(ref[f] != got[f])[:1]}"
-        core, mem, gc, _ = e.state_dump()
-        for n in range(n_nodes):
-            rows = o.rows(n)
-            assert [int(x) for x in core[n, :gc[n]]] == [r[0] for r in rows]
-            assert [int(x) for x in mem[n, :gc[n]]] == [r[1] for r in rows]
+        compare_outputs(ref, e.schedule_batch(c_off, units, mode=mode), f"mode {mode}")
+        compare_rows(e, o, range(n_nodes))
         assert (ref["status"] == 3).sum() > 0 or n_nodes > 1000

@@ -9,24 +9,9 @@ import pytest
 
 import egs_oracle as po
 from scenario import CBackend, make_scenario, run_scenario
-from test_shim_double import ShimDoubleBackend, build_double
+from shim_double import ShimDoubleBackend
 
 pytestmark = pytest.mark.gpu
-
-
-class WideShimDouble(ShimDoubleBackend):
-    """The shim double started with the widest node as its second argument; masks are printed as 16-bit integers."""
-
-    def __init__(self, policy, g_max=16):
-        import subprocess
-        self.p = subprocess.Popen([build_double(), str(policy), str(g_max)], stdin=subprocess.PIPE,
-                                  stdout=subprocess.PIPE, text=True)
-        self.n = 0
-        self.g = {}
-
-    @staticmethod
-    def _lists(masks):
-        return [[g for g in range(16) if m >> g & 1] for m in masks]
 
 
 def _wide_scenario(seed):
@@ -57,7 +42,7 @@ def _wide_scenario(seed):
 def test_shim_double_on_wide_nodes_vs_oracle(seed, policy):
     nodes, ops = _wide_scenario(7000 + 2 * seed + policy)
     ref = run_scenario(CBackend(policy), nodes, ops, policy)
-    b = WideShimDouble(policy)
+    b = ShimDoubleBackend(policy, g_max=16)
     try:
         got = run_scenario(b, nodes, ops, policy)
     finally:

@@ -6,12 +6,12 @@ import numpy as np
 import pytest
 
 import oracle_c as oc
+from oracle_harness import Cluster, compare_caches, compare_outputs, compare_rows, egs, oracle_batch, oracle_mut, \
+    pod_request
 
 pytestmark = pytest.mark.gpu
 
-FIELDS = ["node", "status", "alloc_mask", "fit_count", "fit_digest", "score_digest"]
 GS = [1, 2, 8, 9, 10, 12, 16]
-M64 = (1 << 64) - 1
 SHAPES = [
     [(10, 4, 0)], [(50, 8, 0)], [(25, 2, 0)], [(0, 6, 0)], [(-1, -1, 0)],
     [(0, 0, 1)], [(0, 0, 2)], [(0, 0, 9)], [(0, 0, 12)], [(0, 0, 16)],
@@ -20,104 +20,31 @@ SHAPES = [
 ]
 
 
-def _eg():
-    import egs_b200
-    return egs_b200
-
-
-def _req(units, c_off, p):
-    return [tuple(int(x) for x in units[k]) for k in range(int(c_off[p]), int(c_off[p + 1]))]
-
-
 def _cluster(policy, n, seed, gs=GS):
-    """A wide handle and the oracle over the same n nodes of G in `gs` GPUs, about half of them partly used."""
-    eg = _eg()
+    """n nodes of G in `gs` GPUs for a wide handle, about half of them partly used; and the rng that drew them."""
     rng = np.random.default_rng(seed)
-    e = eg.Egs(policy, n, 16)
-    o = oc.OracleC(policy)
-    for i in range(n):
+    nodes = []
+    for _ in range(n):
         G = int(rng.choice(gs)); M = int(rng.choice([16, 32]))
-        assert e.node_set_allocatable(i, 100 * G, M * G) == 0
-        assert o.add_node(100 * G, M * G) == i
+        rows = None
         if rng.integers(0, 2):
             core = [100 if rng.integers(0, 3) == 0 else int(rng.integers(0, 101)) for _ in range(G)]
-            mem = [M if c == 100 else int(rng.integers(0, M + 1)) for c in core]
-            assert e.state_load(i, core, mem) == 0
-            o.set_rows(i, core, mem)
-    return e, o, rng
-
-
-def _check_rows(e, o, n):
-    core, mem, gc, _ = e.state_dump()
-    assert core.shape == (n, 16)
-    for i in range(n):
-        g = int(gc[i])
-        assert [(int(core[i, k]), int(mem[i, k])) for k in range(g)] == o.rows(i), i
-        assert (core[i, g:] == -(1 << 31)).all() and (mem[i, g:] == -(1 << 31)).all()
+            rows = (core, [M if c == 100 else int(rng.integers(0, M + 1)) for c in core])
+        nodes.append((G, M, rows))
+    return Cluster(policy, nodes, 16), rng
 
 
 def _check_caches(e, o, n, shapes, rng):
     """option_dump of every shape on every node against the oracle's cache, and peek on a few nodes."""
-    cap = _eg().capi
+    compare_caches(e, o, shapes, range(n), unfit_check=True)
     for req in shapes:
-        st, sc, am = e.option_dump(req)
-        assert am.dtype == np.uint16
-        for i in range(n):
-            want = o.peek(i, req)
-            if st[i] == 1:
-                assert want == (cap.masks_to_lists(am[i], len(req)), int(sc[i])), (i, req)
-            else:
-                assert want is None, (i, req, st[i])
         for i in rng.choice(n, size=3, replace=False):
             assert e.peek(int(i), req) == o.peek(int(i), req)
 
 
-def _oracle_batch(o, n, c_off, units, uids, muts=(), mut_at=()):
-    """The driver rule on the oracle pod by pod with its own verbs -- filter every node, score the fit ones, bind the
-    first maximal -- so the masks keep all 16 GPUs.  Records muts[j] apply right before pod mut_at[j]."""
-    mix = o.L.egso_mix64
-    P = len(c_off) - 1
-    out = dict(node=np.full(P, -1, np.int32), status=np.zeros(P, np.int32), alloc_mask=np.zeros((P, 4), np.uint16),
-               fit_count=np.zeros(P, np.int32), fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
-    j = 0
-    for p in range(P):
-        while j < len(mut_at) and mut_at[j] == p:
-            _oracle_mut(o, muts[j]); j += 1
-        req = _req(units, c_off, p)
-        ids = np.flatnonzero(o.filter(None, req)).astype(np.int32)
-        out["fit_count"][p] = len(ids)
-        if len(ids) == 0:
-            out["status"][p] = 1
-            continue
-        st, sc = o.score(ids, req)
-        assert st == 0
-        fd = sd = 0
-        for i, s in zip(ids, sc):
-            fd = (fd + mix(2 * int(i) + 1)) & M64
-            sd = (sd + mix(2 * int(i) + 2) * (2 * int(s) + 1)) & M64
-        out["fit_digest"][p], out["score_digest"][p] = fd, sd
-        w = int(ids[int(np.argmax(sc))])
-        st, alloc = o.bind(w, req, int(uids[p]))
-        out["node"][p], out["status"][p] = w, st
-        if st == 0:
-            for c, a in enumerate(alloc):
-                out["alloc_mask"][p, c] = sum(1 << g for g in a)
-    while j < len(mut_at):
-        _oracle_mut(o, muts[j]); j += 1
-    return out
-
-
-def _oracle_mut(o, rec):
-    kind, node, req, alloc, uid = rec
-    if kind == 1:
-        o.forget_pod(node, req, alloc, uid)
-    else:                                   # ADD, and REPLAY of a uid no podsMap holds: the same row update
-        o.add_pod(node, req, alloc, uid)
-
-
 # ---------------------------------------------------------------------------------------------------- hand cases
 def test_ten_gpu_node_from_allocatable_never_uses_gpu_ten_or_above():
-    eg = _eg()
+    eg = egs()
     e = eg.Egs(0, 1, 10)
     o = oc.OracleC(0)
     assert e.node_set_allocatable(0, 1000, 10 * 81920) == 0 and o.add_node(1000, 10 * 81920) == 0
@@ -133,7 +60,7 @@ def test_ten_gpu_node_from_allocatable_never_uses_gpu_ten_or_above():
 
 @pytest.mark.parametrize("policy", [0, 1])
 def test_whole_gpus_and_sentinel_on_a_sixteen_gpu_node(policy):
-    eg = _eg()
+    eg = egs()
     e = eg.Egs(policy, 3, 16)
     for i in range(3):
         assert e.node_set(i, 16, 32) == 0
@@ -154,7 +81,7 @@ def test_whole_gpus_and_sentinel_on_a_sixteen_gpu_node(policy):
 def test_score_without_filter_is_the_reference_panic_on_a_wide_node(policy):
     """Score of a node that fits but has no cached option: the reference dereferences a nil option (node.go:84).  The
     option Assume cached on the way stays, with the oracle's masks on GPUs above 8."""
-    eg = _eg()
+    eg = egs()
     e = eg.Egs(policy, 2, 16)
     o = oc.OracleC(policy)
     for i, g in enumerate((16, 10)):
@@ -171,9 +98,10 @@ def test_score_without_filter_is_the_reference_panic_on_a_wide_node(policy):
 # ---------------------------------------------------------------------------------------------------- verb sequences
 @pytest.mark.parametrize("policy,seed", [(0, 1), (1, 2), (0, 3)])
 def test_seeded_verb_sequences_on_mixed_clusters(policy, seed):
-    eg = _eg(); cap = eg.capi
+    cap = egs().capi
     n = 40
-    e, o, rng = _cluster(policy, n, seed)
+    cl, rng = _cluster(policy, n, seed)
+    e, o = cl.handle(), cl.oracle()
     gc = [o.gpu_count(i) for i in range(n)]
     uid, bound, seen = 1, [], []
     for step in range(160):
@@ -234,8 +162,8 @@ def test_seeded_verb_sequences_on_mixed_clusters(policy, seed):
                     recs.append((cap.EGS_MUT_ADD, node, r, a, uid)); bound.append((node, r, a, uid)); uid += 1
             assert e.mutations_apply(recs) == 0
             for rec in recs:
-                _oracle_mut(o, rec)
-        _check_rows(e, o, n)
+                oracle_mut(o, rec)
+        compare_rows(e, o, range(n))
         _check_caches(e, o, n, seen, rng)
     assert uid > 20
 
@@ -255,47 +183,42 @@ _WEIGHTS /= _WEIGHTS.sum()
 
 def test_oracle_driver_matches_the_oracle_batch():
     """The per-pod oracle driver the batch tests use equals egso_schedule_batch on the GPUs the latter can show."""
-    n = 60
-    _, o1, rng = _cluster(0, n, 21)
-    _, o2, _ = _cluster(0, n, 21)
+    cl, rng = _cluster(0, 60, 21)
     c_off, units = _batch(rng, 300)
     uids = np.arange(1, 301, dtype=np.uint64)
-    a = _oracle_batch(o1, n, c_off, units, uids)
-    b = o2.schedule_batch(c_off, units.astype(np.int64), uids=uids)
-    for f in FIELDS:
-        want = b[f]
-        got = (a[f] & 0xFF).astype(np.uint8) if f == "alloc_mask" else a[f]
-        assert np.array_equal(got, want), f
+    a = oracle_batch(cl.oracle(), c_off, units, uids)
+    b = cl.oracle().schedule_batch(c_off, units.astype(np.int64), uids=uids)
+    compare_outputs(b, dict(a, alloc_mask=(a["alloc_mask"] & 0xFF).astype(np.uint8)), "driver")
 
 
 @pytest.mark.parametrize("policy", [0, 1])
 def test_batches_on_a_mixed_cluster(policy):
     import torch
-    eg = _eg(); cap = eg.capi
+    eg = egs()
     n, P = 120, 400
-    _, o, rng = _cluster(policy, n, 100 + policy)
+    cl, rng = _cluster(policy, n, 100 + policy)
+    o = cl.oracle()
     c_off, units = _batch(rng, P)
     uids = np.arange(1, P + 1, dtype=np.uint64)
-    ref = _oracle_batch(o, n, c_off, units, uids)
+    ref = oracle_batch(o, c_off, units, uids)
     shapes = eg.workloads.shapes_of(eg.workloads.Workload(0, n, 16, 0, policy, None, None, c_off, units))
     shapes = [list(s) for s in shapes]
 
-    def check(e, got):
-        for f in FIELDS:
-            assert np.array_equal(got[f], ref[f]), f"{f} differs at pod {np.argwhere(got[f] != ref[f])[:3]}"
-        _check_rows(e, o, n)
+    def check(e, got, what):
+        compare_outputs(ref, got, what)
+        compare_rows(e, o, range(n))
         _check_caches(e, o, n, shapes, rng)
 
-    e, _, _ = _cluster(policy, n, 100 + policy)
-    check(e, e.schedule_batch(c_off, units, uids=uids))                       # AUTO: the per-pod engine
+    e = cl.handle()
+    check(e, e.schedule_batch(c_off, units, uids=uids), "auto")               # AUTO: the per-pod engine
     assert all(e.pod_known(int(u)) == o.known_pod(int(u)) for u in uids[:50])
 
-    e, _, _ = _cluster(policy, n, 100 + policy)
+    e = cl.handle()
     got = e.schedule_batch_vec(c_off, units, 40, uids=uids)
-    check(e, got)
-    _, o2, _ = _cluster(policy, n, 100 + policy)
+    check(e, got, "vec")
+    o2 = cl.oracle()
     for p in range(40):                                                        # the full vectors, element-wise
-        req = _req(units, c_off, p)
+        req = pod_request(units, c_off, p)
         fit = o2.filter(None, req)
         assert np.array_equal(got["vec_fit"][p], fit), p
         ids = np.flatnonzero(fit).astype(np.int32)
@@ -306,7 +229,7 @@ def test_batches_on_a_mixed_cluster(policy):
         if ref["node"][p] >= 0:
             o2.bind(int(ref["node"][p]), req, int(uids[p]))
 
-    e, _, _ = _cluster(policy, n, 100 + policy)
+    e = cl.handle()
     dev = [torch.zeros(P, dtype=torch.int32, device="cuda"), torch.zeros(P, dtype=torch.int32, device="cuda"),
            torch.zeros(P * 8, dtype=torch.uint8, device="cuda"), torch.zeros(P, dtype=torch.int32, device="cuda"),
            torch.zeros(P, dtype=torch.int64, device="cuda"), torch.zeros(P, dtype=torch.int64, device="cuda")]
@@ -316,18 +239,17 @@ def test_batches_on_a_mixed_cluster(policy):
                alloc_mask=dev[2].cpu().numpy().view("<u2").reshape(P, 4), fit_count=dev[3].cpu().numpy(),
                fit_digest=dev[4].cpu().numpy().view(np.uint64), score_digest=dev[5].cpu().numpy().view(np.uint64))
     lib_uid = 0x8000000000000000                                                # the library numbers these pods
-    _, o3, _ = _cluster(policy, n, 100 + policy)
-    ref3 = _oracle_batch(o3, n, c_off, units, np.arange(lib_uid, lib_uid + P, dtype=np.uint64))
-    for f in FIELDS:
-        assert np.array_equal(got[f], ref3[f]), f
-    _check_rows(e, o3, n)
+    o3 = cl.oracle()
+    compare_outputs(oracle_batch(o3, c_off, units, np.arange(lib_uid, lib_uid + P, dtype=np.uint64)), got, "device")
+    compare_rows(e, o3, range(n))
 
 
 @pytest.mark.parametrize("policy", [0, 1])
 def test_batch_with_mutations_woven_in(policy):
-    eg = _eg(); cap = eg.capi
+    cap = egs().capi
     n, P = 100, 300
-    e, o, rng = _cluster(policy, n, 200 + policy)
+    cl, rng = _cluster(policy, n, 200 + policy)
+    e, o = cl.handle(), cl.oracle()
     gc = [o.gpu_count(i) for i in range(n)]
     c_off, units = _batch(rng, P)
     uids = np.arange(1, P + 1, dtype=np.uint64)
@@ -344,19 +266,18 @@ def test_batch_with_mutations_woven_in(policy):
             a = [sorted(int(x) for x in rng.choice(gc[node], cnt if j % 2 else 1, replace=False))]
             recs.append((cap.EGS_MUT_ADD, node, r, a, 1_000_000 + j))
     got = e.schedule_batch_mut(c_off, units, mut_at, recs, uids=uids)
-    ref = _oracle_batch(o, n, c_off, units, uids, recs, mut_at)
-    for f in FIELDS:
-        assert np.array_equal(got[f], ref[f]), f"{f} differs at pod {np.argwhere(got[f] != ref[f])[:3]}"
-    _check_rows(e, o, n)
+    compare_outputs(oracle_batch(o, c_off, units, uids, recs, mut_at), got, "batch with mutations")
+    compare_rows(e, o, range(n))
     _check_caches(e, o, n, [list(s) for s in SHAPES], rng)
 
 
 # ---------------------------------------------------------------------------------------------------- guards
 def test_guards_of_a_wide_handle():
-    eg = _eg(); cap = eg.capi
+    eg = egs(); cap = eg.capi
     with pytest.raises(cap.EgsError):
         eg.Egs(0, 4, 17)
-    e, o, rng = _cluster(0, 8, 5, gs=[9, 16])
+    cl, _ = _cluster(0, 8, 5, gs=[9, 16])
+    e, o = cl.handle(), cl.oracle()
     assert e.node_set_allocatable(0, 1700, 17 * 16) == cap.EGS_ERR_BAD_ARG
     assert e.node_set(0, 17, 16) == cap.EGS_ERR_BAD_ARG
     assert e.node_set(0, 12, (1 << 25) + 1) == cap.EGS_ERR_OVERFLOW_GUARD
@@ -395,7 +316,7 @@ def test_guards_of_a_wide_handle():
 def test_per_pod_engine_on_a_wide_handle_equals_the_rounds_engine():
     """The same 8-GPU config-4-style cluster and batch: rounds engine on a g_max = 8 handle, per-pod engine on a wide
     handle.  Same outputs (masks widened to u16) and the same rows."""
-    eg = _eg(); cap = eg.capi
+    eg = egs(); cap = eg.capi
     w = eg.workloads.config(4, n_nodes=20_000, n_pods=200_000)
     got = []
     for g_max in (8, 16):
@@ -405,8 +326,7 @@ def test_per_pod_engine_on_a_wide_handle_equals_the_rounds_engine():
         e.close()
     (a, rows_a), (b, rows_b) = got
     assert a["alloc_mask"].dtype == np.uint8 and b["alloc_mask"].dtype == np.uint16
-    for f in FIELDS:
-        assert np.array_equal(a[f].astype(np.uint16) if f == "alloc_mask" else a[f], b[f]), f
+    compare_outputs(a, b, "per-pod engine on a wide handle")
     assert np.array_equal(rows_a[0], rows_b[0][:, :8]) and np.array_equal(rows_a[1], rows_b[1][:, :8])
     assert (rows_b[0][:, 8:] == cap.EGS_PAD).all()
     assert (a["status"] == 0).any()
@@ -416,7 +336,7 @@ def test_device_batch_refuses_a_misaligned_mask_buffer():
     """A wide handle stores each pod's four u16 masks as one 8-byte word: a buffer that is not 8-byte aligned is
     refused before anything runs."""
     import torch
-    eg = _eg(); cap = eg.capi
+    eg = egs(); cap = eg.capi
     e = eg.Egs(0, 4, 16)
     for i in range(4):
         assert e.node_set(i, 16, 32) == 0

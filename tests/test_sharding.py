@@ -7,6 +7,8 @@ import sys
 import numpy as np
 import pytest
 
+from oracle_harness import Cluster, compare_shards, egs, run_sharded
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -35,10 +37,8 @@ def _gloo_worker(rank, world, port, q):
         assert box[0] == bytes(range(128))
         # each rank filters ITS node range with the oracle; per-shard digests must add up (mod 2^64)
         w = egs_b200.workloads.config(1, n_nodes=1000, n_pods=4)
-        o = oracle_c.OracleC(w.policy)
-        for n in range(w.n_nodes):
-            o.add_node(800, 8 * w.mem_total)
-            o.set_rows(n, w.core[n], w.mem[n])
+        cl = Cluster.of_workload(w)
+        o = cl.oracle()
         lo, hi = egs_b200.capi.shard_range(w.n_nodes, rank, world)
         req = [tuple(int(x) for x in w.units[0])]
         ids = np.arange(lo, hi, dtype=np.int32)
@@ -51,11 +51,7 @@ def _gloo_worker(rank, world, port, q):
         t = torch.tensor([int(fit.sum()), fd - (1 << 64) if fd >= 1 << 63 else fd, sd - (1 << 64) if sd >= 1 << 63 else sd],
                          dtype=torch.int64)
         dist.all_reduce(t)                      # int64 wrap-around == addition mod 2^64
-        o2 = oracle_c.OracleC(w.policy)
-        for n in range(w.n_nodes):
-            o2.add_node(800, 8 * w.mem_total)
-            o2.set_rows(n, w.core[n], w.mem[n])
-        full = o2.schedule_batch(w.c_off[:2], w.units64()[:1])
+        full = cl.oracle().schedule_batch(w.c_off[:2], w.units64()[:1])
         assert int(t[0]) == int(full["fit_count"][0])
         assert int(t[1]) & (2**64 - 1) == int(full["fit_digest"][0])
         assert int(t[2]) & (2**64 - 1) == int(full["score_digest"][0])
@@ -99,47 +95,11 @@ def test_sharded_engine_in_process_equals_unsharded(world):
     single-GPU box): an in-process shard group (egs_comm_init_local) replaces NCCL by device-to-device copies of the
     same candidate buffers; kernels, buffers and the replicated resolver are those of the NCCL path.  Every rank's
     outputs must equal the unsharded run bit for bit, and every shard's rows the unsharded rows."""
-    import threading
-    import egs_b200
-    cap = egs_b200.capi
-    F = ["node", "status", "alloc_mask", "fit_count", "fit_digest", "score_digest"]
     # config 4 at full node count, long enough that nearly every round ends on a dry per-shard list (at 8 shards each
     # contributes only 32 candidates per shape): the replicated resolvers must stop at the SAME pod on every rank
     cases = [(4, None, 200000 if world == 8 else 60000, None), (1, None, None, None), (2, 3000, 6000, None), (3, 300, 2000, 0),
              (4, 1000, 3000, 0)]
     for cfg, nn, npods, pol in cases:
-        w = egs_b200.workloads.config(cfg, n_nodes=nn, n_pods=npods, policy=pol)
-        e0 = egs_b200.Egs(w.policy, w.n_nodes)
-        e0.state_load_bulk(0, w.gpus, w.mem_total, w.core, w.mem)
-        ref = e0.schedule_batch(w.c_off, w.units, mode=cap.EGS_MODE_ROUNDS)
-        ref_core, ref_mem, _, _ = e0.state_dump()
-        e0.close()
-        hs = []
-        for r in range(world):
-            e = egs_b200.Egs(w.policy, w.n_nodes)
-            e.shard_set(r, world)
-            hs.append(e)
-        cap.comm_init_local(hs)
-        for e in hs:
-            e.state_load_bulk(0, w.gpus, w.mem_total, w.core, w.mem)
-        outs, errs = [None] * world, []
-
-        def run(r):
-            try:
-                outs[r] = hs[r].schedule_batch(w.c_off, w.units, mode=cap.EGS_MODE_ROUNDS)
-            except Exception as ex:   # pragma: no cover
-                errs.append(repr(ex))
-        th = [threading.Thread(target=run, args=(r,)) for r in range(world)]
-        for t_ in th:
-            t_.start()
-        for t_ in th:
-            t_.join(timeout=600)
-        assert not errs, errs
-        for r in range(world):
-            for f in F:
-                assert np.array_equal(ref[f], outs[r][f]), f"cfg{cfg} world {world} rank {r}: {f} differs"
-            lo, hi = cap.shard_range(w.n_nodes, r, world)
-            core, mem, _, _ = hs[r].state_dump(lo, hi - lo)
-            assert np.array_equal(core, ref_core[lo:hi]) and np.array_equal(mem, ref_mem[lo:hi]), f"rows of shard {r}"
-        for e in hs:
-            e.close()
+        w = egs().workloads.config(cfg, n_nodes=nn, n_pods=npods, policy=pol)
+        ref, rows, ranks = run_sharded(Cluster.of_workload(w).handle, world, w.c_off, w.units)
+        compare_shards(ref, rows, ranks, f"cfg{cfg} world {world}")
