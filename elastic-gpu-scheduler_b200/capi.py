@@ -34,7 +34,7 @@ def mask_dtype(g_max: int):
 SYMBOLS = [
     "egs_create", "egs_destroy", "egs_last_error", "egs_status_string", "egs_unit_from_requests",
     "egs_node_set_allocatable", "egs_node_set", "egs_state_load", "egs_state_load_bulk", "egs_state_dump",
-    "egs_state_snapshot", "egs_state_restore",
+    "egs_state_snapshot", "egs_state_restore", "egs_checkpoint_save", "egs_checkpoint_rollback", "egs_checkpoint_drop",
     "egs_filter", "egs_score", "egs_bind", "egs_option_peek", "egs_option_dump", "egs_pod_apply", "egs_node_replay_pod", "egs_pod_cancel",
     "egs_mutations_apply", "egs_schedule_batch_mut", "egs_pod_known", "egs_pod_released", "egs_schedule_batch", "egs_schedule_batch_vec", "egs_schedule_batch_device",
     "egs_shard_set", "egs_shard_range", "egs_comm_unique_id", "egs_comm_init", "egs_comm_init_local", "egs_profile_evaluate", "egs_profile_get",
@@ -79,6 +79,9 @@ def load(build: bool = True):
     L.egs_state_dump.argtypes = [vp, i32, i32, vp, vp, vp, vp]
     L.egs_state_snapshot.argtypes = [vp]
     L.egs_state_restore.argtypes = [vp]
+    L.egs_checkpoint_save.argtypes = [vp]
+    L.egs_checkpoint_rollback.argtypes = [vp]
+    L.egs_checkpoint_drop.argtypes = [vp]
     L.egs_filter.argtypes = [vp, i32, vp, i32, vp, vp]
     L.egs_score.argtypes = [vp, i32, vp, i32, vp, vp]
     L.egs_bind.argtypes = [vp, i32, i32, vp, u64, vp]
@@ -207,6 +210,18 @@ class Egs:
 
     def restore(self):
         self._ck(self.L.egs_state_restore(self.h), "egs_state_restore")
+
+    def checkpoint_save(self):
+        """Record the complete scheduler state (egs.h), replacing an earlier checkpoint."""
+        self._ck(self.L.egs_checkpoint_save(self.h), "egs_checkpoint_save")
+
+    def checkpoint_rollback(self):
+        """Return exactly to the checkpoint, which stays for the next what-if."""
+        self._ck(self.L.egs_checkpoint_rollback(self.h), "egs_checkpoint_rollback")
+
+    def checkpoint_drop(self):
+        """Forget the checkpoint and free its memory; the current state stays."""
+        self._ck(self.L.egs_checkpoint_drop(self.h), "egs_checkpoint_drop")
 
     def rows(self, node: int):
         core, mem, gc, _ = self.state_dump(node, 1)

@@ -26,6 +26,21 @@ struct PendingBatch {           // results of a batch whose uid bookkeeping is a
   int n; uint64_t uid0; std::vector<uint64_t> uids; int32_t *h_node, *h_status; PinBuf buf; cudaEvent_t done;
 };
 
+struct ShapeCacheEnt { uint64_t h; int slot; };   // open-addressing entry of egs_handle::shape_cache
+
+// egs_checkpoint_save: the complete scheduler state but the PodBook, which keeps its own undo journal.  The device
+// buffers are allocated on the first save and grown when more shapes are interned.
+struct Checkpoint {
+  bool open = false;
+  int32_t *d_core = nullptr, *d_mem = nullptr, *d_mem_total = nullptr;
+  uint8_t *d_st = nullptr; int32_t *d_sc = nullptr; uint8_t *d_al = nullptr; int slot_cap = 0;
+  int n_shapes = 0;                       // shapes interned at the save; later ones are forgotten by the rollback
+  std::vector<int32_t> gpu_count, mem_total;
+  std::vector<char> slot_cold;
+  std::vector<ShapeCacheEnt> shape_cache;
+  uint64_t next_uid = 0;
+};
+
 struct egs_handle {
   int policy = 0, max_nodes = 0, n_pad = 0, g_max = 0, device = 0, n_sm = 0;
   int row_w = EGS_G, mask_b = 1;          // EGS_ROW_WIDTH(g_max), EGS_MASK_BYTES(g_max)
@@ -41,7 +56,7 @@ struct egs_handle {
   std::vector<Shape> shapes;
   std::vector<char> slot_cold;            // option table of the slot holds only OPT_ABSENT (nothing evaluated yet)
   std::unordered_map<std::string, int> shape_ids;
-  struct ShapeCacheEnt { uint64_t h; int slot; };
+  using ShapeCacheEnt = ::ShapeCacheEnt;
   std::vector<ShapeCacheEnt> shape_cache = std::vector<ShapeCacheEnt>(1024, ShapeCacheEnt{0, -1});   // open addressing
   // reference bookkeeping that never reaches the device
   PodBook book;                                                 // podsMap / podMaps / releasedPodMap
@@ -63,6 +78,7 @@ struct egs_handle {
   // profiling
   int64_t k_launches[EGS_K_COUNT] = {0}; double k_ms[EGS_K_COUNT] = {0}; int timing = 0;
   RoundsState rounds;
+  Checkpoint ck;
   std::mutex mu;
   std::string err;
 };
@@ -178,10 +194,15 @@ static inline int intern(egs_handle *h, int C, const egs_unit *u, int *slot) {
   return EGS_OK;
 }
 
-static int intern_slow(egs_handle *h, int C, const egs_unit *u, int *slot) {
-  TRY(check_units(C, u));
+static std::string shape_key(int C, const egs_unit *u) {
   std::string key((const char *)&C, sizeof C);
   key.append((const char *)u, sizeof(egs_unit) * C);
+  return key;
+}
+
+static int intern_slow(egs_handle *h, int C, const egs_unit *u, int *slot) {
+  TRY(check_units(C, u));
+  const std::string key = shape_key(C, u);
   auto it = h->shape_ids.find(key);
   if (it != h->shape_ids.end()) { *slot = it->second; return EGS_OK; }
   int s = (int)h->shapes.size();
@@ -227,6 +248,17 @@ static int pin_get(egs_handle *h, size_t n, PinBuf *out) {
   CK(h, cudaMallocHost(&b.p, b.cap * sizeof(int32_t)));
   *out = b;
   return EGS_OK;
+}
+
+static void checkpoint_free(egs_handle *h) {
+  Checkpoint &k = h->ck;
+  if (k.d_core) {
+    cudaStreamSynchronize(h->stream);             // no copy into these buffers is still in flight
+    void *dev[] = {k.d_core, k.d_mem, k.d_mem_total, k.d_st, k.d_sc, k.d_al};
+    for (void *p : dev) if (p) cudaFree(p);
+  }
+  h->ck = Checkpoint();
+  h->book.drop_checkpoint();
 }
 
 // ------------------------------------------------------------------------------- lifecycle
@@ -278,6 +310,7 @@ extern "C" int egs_destroy(egs_handle *h) {
   for (auto &b : h->pin_pool) cudaFreeHost(b.p);
   h->pin_pool.clear();
   rounds_free(&h->rounds);
+  checkpoint_free(h);
   void *dev[] = {h->d_core, h->d_mem, h->d_mem_total, h->d_st, h->d_sc, h->d_al, h->d_partials, h->d_ticket, h->d_snap_core, h->d_snap_mem, h->d_snap_total,
                  h->d_result, h->d_ids, h->d_fit, h->d_score, h->d_ev_fit, h->d_ev_score, h->d_ev_gpu, h->d_flush,
                  h->d_o_node, h->d_o_status, h->d_o_fit, h->d_o_alloc, h->d_o_fd, h->d_o_sd, h->d_vec_fit, h->d_vec_score, h->d_ops, h->d_group_off};
@@ -464,6 +497,94 @@ extern "C" int egs_state_restore(egs_handle *h) {
   std::fill(h->slot_cold.begin(), h->slot_cold.end(), 1);
   h->h_gpu_count = h->snap_gpu_count; h->h_mem_total = h->snap_mem_total;
   h->book.clear();
+  return EGS_OK;
+}
+
+// Option tables of slots [0, ns) between the handle's arrays and a checkpoint's.  Each array is one contiguous slice
+// per slot (table()), so every array is one copy.
+static int copy_tables(egs_handle *h, int ns, bool save) {
+  Checkpoint &k = h->ck;
+  const size_t np = (size_t)h->n_pad, al_plane = np * EGS_C * h->mask_b;
+  uint8_t *st = save ? k.d_st : h->d_st, *al = save ? k.d_al : h->d_al; int32_t *sc = save ? k.d_sc : h->d_sc;
+  const uint8_t *st0 = save ? h->d_st : k.d_st, *al0 = save ? h->d_al : k.d_al; const int32_t *sc0 = save ? h->d_sc : k.d_sc;
+  if (ns == 0) return EGS_OK;
+  CK(h, cudaMemcpyAsync(st, st0, np * ns, cudaMemcpyDeviceToDevice, h->stream));
+  CK(h, cudaMemcpyAsync(sc, sc0, np * ns * sizeof(int32_t), cudaMemcpyDeviceToDevice, h->stream));
+  CK(h, cudaMemcpyAsync(al, al0, al_plane * ns, cudaMemcpyDeviceToDevice, h->stream));
+  return EGS_OK;
+}
+
+static int copy_rows(egs_handle *h, bool save) {
+  Checkpoint &k = h->ck;
+  const size_t rows = (size_t)h->n_pad * h->row_w * sizeof(int32_t), totals = (size_t)h->n_pad * sizeof(int32_t);
+  CK(h, cudaMemcpyAsync(save ? k.d_core : h->d_core, save ? h->d_core : k.d_core, rows, cudaMemcpyDeviceToDevice, h->stream));
+  CK(h, cudaMemcpyAsync(save ? k.d_mem : h->d_mem, save ? h->d_mem : k.d_mem, rows, cudaMemcpyDeviceToDevice, h->stream));
+  CK(h, cudaMemcpyAsync(save ? k.d_mem_total : h->d_mem_total, save ? h->d_mem_total : k.d_mem_total, totals,
+                        cudaMemcpyDeviceToDevice, h->stream));
+  return EGS_OK;
+}
+
+extern "C" int egs_checkpoint_save(egs_handle *h) {
+  if (!h) return EGS_ERR_BAD_ARG;
+  Guard g(h);
+  TRY(flush_pending(h));                          // batches still pending belong to the saved state
+  Checkpoint &k = h->ck;
+  k.open = false;                                 // an earlier checkpoint is overwritten from here on
+  h->book.drop_checkpoint();
+  const int ns = (int)h->shapes.size();
+  const size_t np = (size_t)h->n_pad, rows = np * h->row_w * sizeof(int32_t);
+  if (!k.d_core) {
+    CK(h, cudaMalloc(&k.d_core, rows));
+    CK(h, cudaMalloc(&k.d_mem, rows));
+    CK(h, cudaMalloc(&k.d_mem_total, np * sizeof(int32_t)));
+  }
+  if (ns > k.slot_cap) {
+    CK(h, cudaStreamSynchronize(h->stream));      // the previous save may still copy into the old buffers
+    if (k.d_st) { cudaFree(k.d_st); cudaFree(k.d_sc); cudaFree(k.d_al); k.d_st = nullptr; k.d_sc = nullptr; k.d_al = nullptr; }
+    k.slot_cap = 0;
+    const int cap = std::max(ns, h->slot_cap);
+    CK(h, cudaMalloc(&k.d_st, np * cap));
+    CK(h, cudaMalloc(&k.d_sc, np * cap * sizeof(int32_t)));
+    CK(h, cudaMalloc(&k.d_al, np * EGS_C * h->mask_b * cap));
+    k.slot_cap = cap;
+  }
+  TRY(copy_rows(h, true));
+  TRY(copy_tables(h, ns, true));
+  k.n_shapes = ns;
+  k.gpu_count = h->h_gpu_count; k.mem_total = h->h_mem_total;
+  k.slot_cold = h->slot_cold;
+  k.shape_cache = h->shape_cache;
+  k.next_uid = h->next_uid;
+  h->book.checkpoint();
+  k.open = true;
+  return EGS_OK;
+}
+
+extern "C" int egs_checkpoint_rollback(egs_handle *h) {
+  if (!h) return EGS_ERR_BAD_ARG;
+  Guard g(h);
+  Checkpoint &k = h->ck;
+  if (!k.open) return fail(h, EGS_ERR_BAD_ARG, "no checkpoint: egs_checkpoint_save first");
+  TRY(discard_pending(h));                        // batches after the save whose results never reached the book
+  const int ns = (int)h->shapes.size();
+  TRY(copy_rows(h, false));
+  TRY(copy_tables(h, k.n_shapes, false));         // the tables may have been reallocated since: slot offsets hold
+  if (ns > k.n_shapes)                            // slots interned since the save read OPT_ABSENT again
+    CK(h, cudaMemsetAsync(h->d_st + (size_t)k.n_shapes * h->n_pad, OPT_ABSENT, (size_t)(ns - k.n_shapes) * h->n_pad, h->stream));
+  for (int s = k.n_shapes; s < ns; s++) h->shape_ids.erase(shape_key(h->shapes[s].C, h->shapes[s].u));
+  h->shapes.resize((size_t)k.n_shapes);
+  h->slot_cold = k.slot_cold;
+  h->shape_cache = k.shape_cache;
+  h->h_gpu_count = k.gpu_count; h->h_mem_total = k.mem_total;
+  h->next_uid = k.next_uid;
+  h->book.rollback();
+  return EGS_OK;
+}
+
+extern "C" int egs_checkpoint_drop(egs_handle *h) {
+  if (!h) return EGS_ERR_BAD_ARG;
+  Guard g(h);
+  checkpoint_free(h);
   return EGS_OK;
 }
 
@@ -1005,6 +1126,7 @@ extern "C" int egs_shard_set(egs_handle *h, int rank, int world) {
   if (!h || world < 1 || world > RD || rank < 0 || rank >= world) return EGS_ERR_BAD_ARG;
   Guard g(h);
   if (is_wide(h)) return fail(h, EGS_ERR_BAD_ARG, "the sharded engine is the rounds engine: it needs g_max <= EGS_MAX_GPUS");
+  checkpoint_free(h);                             // a checkpoint holds for the shard layout it was taken under
   h->rank = rank; h->world = world;
   egs_shard_range(h->max_nodes, rank, world, &h->lo, &h->hi);
   return EGS_OK;

@@ -1,5 +1,6 @@
 // pod_book_on_host.cc -- PodBook (csrc/pod_book.h) behind a C API, so the CPU test suite can check the uid
-// bookkeeping against a model of the reference's three maps (tests/test_pod_book_host.py).  Not part of libegs.
+// bookkeeping against a model of the reference's three maps (tests/test_pod_book_host.py) and its checkpoint journal
+// (tests/test_pod_book_journal_host.py).  Not part of libegs.
 #include "../pod_book.h"
 
 static PodBook *B(void *b) { return (PodBook *)b; }
@@ -28,6 +29,10 @@ int egspb_account(void *b, int kind, int node, uint64_t uid, int fail_apply, int
 }
 void egspb_drop_nodes(void *b, int node0, int n) { B(b)->drop_nodes(node0, n); }
 void egspb_clear(void *b) { B(b)->clear(); }
+void egspb_checkpoint(void *b) { B(b)->checkpoint(); }
+void egspb_rollback(void *b) { B(b)->rollback(); }
+void egspb_drop_checkpoint(void *b) { B(b)->drop_checkpoint(); }
+uint64_t egspb_hash_uid_max(void *b) { return B(b)->hash_uid_max(); }
 int egspb_in_pods_map(void *b, int node, uint64_t uid) { return B(b)->in_pods_map(node, uid) ? 1 : 0; }
 int egspb_in_pod_maps(void *b, uint64_t uid) { return B(b)->in_pod_maps(uid) ? 1 : 0; }
 int egspb_released(void *b, uint64_t uid) { return B(b)->released(uid) ? 1 : 0; }

@@ -116,6 +116,33 @@ int egs_state_dump(egs_handle *h, int node0, int n, int32_t *free_core, int32_t 
 int egs_state_snapshot(egs_handle *h);
 int egs_state_restore(egs_handle *h);
 
+/* Checkpoint of the COMPLETE scheduler state, for dry runs, all-or-nothing admission of a
+ * pod group and what-if evictions (INTEGRATION §3).  Unlike egs_state_restore, which is a
+ * restarted scheduler, a rollback is exact: every call made after it answers as it would
+ * have answered at the save.  The state is
+ *   - the rows, mem_total, and which nodes are set with how many GPUs;
+ *   - the option cache of every shape interned at the save (cached options, stale ones
+ *     included, and "does not fit" memos); shapes interned after the save are forgotten;
+ *   - podsMap, podMaps and releasedPodMap (egs_pod_known / egs_pod_released);
+ *   - the next library-assigned uid, so a dry run and the real run that follows it assign
+ *     the same uids.
+ * Not state: the egs_state_snapshot copy, profile counters and egs_rounds_stats,
+ * egs_last_error, and the shard / communicator setup.
+ * Batches still pending are settled at the save; a rollback discards whatever batch ran
+ * after it.  Costs: two device copies of the rows and of the option tables in use, plus
+ * host work proportional to the uid bookkeeping changed since the save.
+ *
+ * save: records the state, replacing an earlier checkpoint.
+ * rollback: returns to it; the checkpoint stays, so several what-ifs can start from it.
+ *   With no checkpoint: EGS_ERR_BAD_ARG (egs_last_error says so), nothing changes.
+ * drop: forgets it and frees its memory; the current state stays.
+ * egs_destroy frees a checkpoint and egs_shard_set drops it.  On a sharded handle every
+ * rank issues the calls, as with every other call; no collective runs.  One checkpoint
+ * per handle: they do not nest. */
+int egs_checkpoint_save(egs_handle *h);
+int egs_checkpoint_rollback(egs_handle *h);
+int egs_checkpoint_drop(egs_handle *h);
+
 /* ---- verbs (one pod at a time; host buffers) -------------------------------- */
 
 /* Assume: for each candidate node (node_ids == NULL means 0..n-1) cache hit -> fit,
