@@ -68,12 +68,17 @@ def window(w: "Workload", start: int, n_pods: int) -> "Workload":
 
 def shapes_of(w: "Workload"):
     """Distinct request shapes of the batch, in order of first appearance: tuples of (core, mem, count)."""
-    seen, out = set(), []
-    for p in range(w.n_pods):
-        u = tuple(tuple(int(x) for x in w.units[k]) for k in range(int(w.c_off[p]), int(w.c_off[p + 1])))
-        if u not in seen:
-            seen.add(u); out.append(u)
-    return out
+    P = w.n_pods
+    if P == 0:
+        return []
+    n_c = np.diff(w.c_off)
+    pods = np.full((P, int(n_c.max()), 3), np.iinfo(np.int32).min, np.int32)   # one padded row of units per pod
+    for c in range(pods.shape[1]):
+        has = n_c > c
+        pods[has, c] = w.units[w.c_off[:-1][has] + c]
+    _, first = np.unique(pods.reshape(P, -1), axis=0, return_index=True)
+    return [tuple(tuple(int(x) for x in w.units[k]) for k in range(int(w.c_off[p]), int(w.c_off[p + 1])))
+            for p in np.sort(first)]
 
 
 def config(cfg: int, n_nodes: int | None = None, n_pods: int | None = None, policy: int | None = None) -> Workload:

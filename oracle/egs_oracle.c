@@ -421,6 +421,31 @@ int egso_add_node(egso *o, int64_t core_allocatable, int64_t mem_allocatable) {
   for (int i = 0; i < nd->G; i++) { nd->g[i].ca = nd->g[i].ct = CORE_EACH_CARD; nd->g[i].ma = nd->g[i].mt = m; }
   return o->nn - 1;
 }
+/* n nodes of G GPUs each, as n calls of egso_add_node(100 * G, mem_alloc) followed by egso_set_rows with row i of
+ * core / mem ([n][G]; NULL keeps the fresh rows).  Returns the first new node id, or -1 when G is out of range. */
+int egso_add_nodes(egso *o, int n, int G, int64_t mem_alloc, const int64_t *core, const int64_t *mem) {
+  if (G < 1 || G > EGSO_MAX_G || n < 0) return -1;
+  const int first = o->nn;
+  if (o->nn + n > o->nc) {
+    while (o->nn + n > o->nc) o->nc = o->nc ? o->nc * 2 : 64;
+    o->nodes = realloc(o->nodes, o->nc * sizeof(node_t));
+  }
+  for (int i = 0; i < n; i++) {
+    egso_add_node(o, (int64_t)CORE_EACH_CARD * G, mem_alloc);
+    if (core && mem) egso_set_rows(o, first + i, core + (size_t)i * G, mem + (size_t)i * G);
+  }
+  return first;
+}
+/* rows of node_ids[0..n) into [n][width] (cells past a node's GPU count are left untouched) and the GPU counts */
+void egso_get_rows_many(egso *o, int n, const int32_t *node_ids, int width, int64_t *core, int64_t *mem,
+                        int32_t *gpu_count) {
+  for (int i = 0; i < n; i++) {
+    const node_t *nd = &o->nodes[node_ids[i]];
+    const int G = nd->G < width ? nd->G : width;
+    for (int g = 0; g < G; g++) { core[(size_t)i * width + g] = nd->g[g].ca; mem[(size_t)i * width + g] = nd->g[g].ma; }
+    gpu_count[i] = nd->G;
+  }
+}
 int egso_num_nodes(egso *o) { return o->nn; }
 int egso_gpu_count(egso *o, int node) { return o->nodes[node].G; }
 void egso_set_rows(egso *o, int node, const int64_t *core, const int64_t *mem) {

@@ -30,6 +30,11 @@ egso *egso_create(int policy, int faithful);
 void egso_destroy(egso *o);
 /* NewNodeAllocator (node.go:23-59); returns the dense node id, or -1 ("no gpu available"). */
 int egso_add_node(egso *o, int64_t core_allocatable, int64_t mem_allocatable);
+/* TEST SUPPORT, bulk forms of the calls above: n nodes of G GPUs each (egso_add_node(100 * G, mem_alloc) then
+ * egso_set_rows from [n][G] core / mem, NULL = fresh rows), returning the first id; and rows of many nodes. */
+int egso_add_nodes(egso *o, int n, int G, int64_t mem_alloc, const int64_t *core, const int64_t *mem);
+void egso_get_rows_many(egso *o, int n, const int32_t *node_ids, int width, int64_t *core, int64_t *mem,
+                        int32_t *gpu_count);
 int egso_num_nodes(egso *o);
 int egso_gpu_count(egso *o, int node);
 void egso_set_rows(egso *o, int node, const int64_t *core, const int64_t *mem);

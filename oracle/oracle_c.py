@@ -43,6 +43,8 @@ def lib():
         L.egso_create.argtypes = [C.c_int, C.c_int]
         L.egso_destroy.argtypes = [C.c_void_p]
         L.egso_add_node.argtypes = [C.c_void_p, C.c_int64, C.c_int64]
+        L.egso_add_nodes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_void_p]
+        L.egso_get_rows_many.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.egso_num_nodes.argtypes = [C.c_void_p]
         L.egso_gpu_count.argtypes = [C.c_void_p, C.c_int]
         L.egso_set_rows.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
@@ -107,6 +109,27 @@ class OracleC:
 
     def add_node(self, core_alloc: int, mem_alloc: int) -> int:
         return self.L.egso_add_node(self.h, core_alloc, mem_alloc)
+
+    def add_nodes(self, gpus: int, mem_alloc: int, core=None, mem=None) -> int:
+        """len(core) nodes of `gpus` GPUs (add_node(100 * gpus, mem_alloc) each) with rows core / mem [n, gpus]
+        in one call; returns the first new node id."""
+        c = np.ascontiguousarray(core, dtype=np.int64)
+        m = np.ascontiguousarray(mem, dtype=np.int64)
+        assert c.shape == m.shape and c.ndim == 2 and c.shape[1] == gpus
+        first = self.L.egso_add_nodes(self.h, c.shape[0], gpus, mem_alloc, _ptr(c), _ptr(m))
+        assert first >= 0, "egso_add_nodes: GPU count out of range"
+        return first
+
+    def rows_many(self, node_ids, width: int):
+        """Rows of `node_ids` as (core [n, width], mem [n, width], gpu_count [n]); cells past a node's GPU count
+        are 0."""
+        ids = np.ascontiguousarray(node_ids, dtype=np.int32)
+        assert ids.size == 0 or (ids.min() >= 0 and ids.max() < self.n_nodes)
+        core = np.zeros((len(ids), width), np.int64)
+        mem = np.zeros((len(ids), width), np.int64)
+        gc = np.zeros(len(ids), np.int32)
+        self.L.egso_get_rows_many(self.h, len(ids), _ptr(ids), width, _ptr(core), _ptr(mem), _ptr(gc))
+        return core, mem, gc
 
     @property
     def n_nodes(self) -> int:

@@ -20,20 +20,33 @@ def egs():
 
 class Cluster:
     """nodes: [(gpu_count, mem_total per GPU, (core row, mem row) or None)].  The same cluster on a library handle
-    (rows through egs_state_load, or egs_state_load_bulk for a workload) and on the oracle."""
+    (rows through egs_state_load, or egs_state_load_bulk for a workload) and on the oracle.  A cluster of a workload
+    (anything with policy, n_nodes, gpus, mem_total and core / mem [n_nodes, gpus]) is loaded in bulk on both sides,
+    and its node list is only built when asked for."""
 
     def __init__(self, policy, nodes, g_max=8):
-        self.policy, self.nodes, self.g_max = policy, nodes, g_max
+        self.policy, self._nodes, self.g_max = policy, nodes, g_max
         self.workload = None
 
     @classmethod
-    def of_workload(cls, w):
-        cl = cls(w.policy, [(w.gpus, w.mem_total, (w.core[n], w.mem[n])) for n in range(w.n_nodes)])
+    def of_workload(cls, w, g_max=8):
+        cl = cls(w.policy, None, g_max)
         cl.workload = w
         return cl
 
+    @property
+    def nodes(self):
+        if self._nodes is None:
+            w = self.workload
+            self._nodes = [(w.gpus, w.mem_total, (w.core[n], w.mem[n])) for n in range(w.n_nodes)]
+        return self._nodes
+
+    @property
+    def n_nodes(self):
+        return self.workload.n_nodes if self.workload is not None else len(self._nodes)
+
     def handle(self, world=1, rank=0):
-        e = egs().Egs(self.policy, len(self.nodes), self.g_max)
+        e = egs().Egs(self.policy, self.n_nodes, self.g_max)
         if world > 1:
             e.shard_set(rank, world)
         w = self.workload
@@ -48,6 +61,10 @@ class Cluster:
 
     def oracle(self):
         o = oc.OracleC(self.policy)
+        w = self.workload
+        if w is not None:
+            assert o.add_nodes(w.gpus, w.mem_total * w.gpus, w.core, w.mem) == 0
+            return o
         for n, (g, mt, rows) in enumerate(self.nodes):
             assert o.add_node(100 * g, mt * g) == n
             if rows is not None:
@@ -65,11 +82,18 @@ def compare_rows(e, o, nodes):
     """Rows of `nodes`: the library's first gpu_count cells are the oracle's rows and every cell past them is PAD."""
     cap = egs().capi
     core, mem, gc, _ = e.state_dump()
-    assert core.shape[1] == cap.row_width(e.g_max)
-    for n in nodes:
-        g = int(gc[n])
-        assert list(zip(core[n, :g].tolist(), mem[n, :g].tolist())) == o.rows(n), f"rows of node {n}"
-        assert (core[n, g:] == cap.EGS_PAD).all() and (mem[n, g:] == cap.EGS_PAD).all(), f"PAD cells of node {n}"
+    W = core.shape[1]
+    assert W == cap.row_width(e.g_max)
+    nodes = np.unique(np.fromiter(nodes, np.int64))
+    core, mem, gc = core[nodes], mem[nodes], gc[nodes]
+    ocore, omem, ogc = o.rows_many(nodes, W)
+    bad = np.nonzero(gc != ogc)[0]
+    assert bad.size == 0, f"rows of node {int(nodes[bad[0]])}: {gc[bad[0]]} GPUs, the oracle has {ogc[bad[0]]}"
+    live = np.arange(W)[None, :] < ogc[:, None]
+    bad = np.nonzero((live & ((core != ocore) | (mem != omem))).any(1))[0]
+    assert bad.size == 0, f"rows of node {int(nodes[bad[0]])}"
+    bad = np.nonzero((~live & ((core != cap.EGS_PAD) | (mem != cap.EGS_PAD))).any(1))[0]
+    assert bad.size == 0, f"PAD cells of node {int(nodes[bad[0]])}"
 
 
 def compare_caches(e, o, shapes, nodes, unfit_check):
@@ -91,6 +115,57 @@ def compare_caches(e, o, shapes, nodes, unfit_check):
             unfit = nodes[st == 2]
             fits = o.trade_fits(unfit, sh)
             assert not fits.any(), f"shape {sh}: nodes {unfit[fits][:5].tolist()} marked unfit but fit"
+
+
+def conservation(w, out, e):
+    """Size-independent property: final rows == initial rows - sum of successful binds."""
+    core = w.core.astype(np.int64).copy()
+    mem = w.mem.astype(np.int64).copy()
+    ok = out["status"] == 0
+    assert ((out["node"] >= 0) == (out["status"] != 1)).all()
+    for c in range(4):
+        has = ok & (np.diff(w.c_off) > c)
+        pods = np.nonzero(has)[0]
+        m = out["alloc_mask"][pods, c]
+        assert (np.bitwise_count(m) == 1).all()
+        g = np.log2(m.astype(np.float64)).astype(np.int64)
+        u = w.units[w.c_off[pods] + c]
+        np.subtract.at(core, (out["node"][pods], g), u[:, 0])
+        np.subtract.at(mem, (out["node"][pods], g), u[:, 1])
+    dc, dm, _, _ = e.state_dump()
+    assert np.array_equal(dc[:, :w.gpus], core) and np.array_equal(dm[:, :w.gpus], mem)
+    assert (core >= 0).all() and (mem >= 0).all()
+
+
+def late_window(cfg, policy, K, W, n_nodes=None, threads=4, sample=4000):
+    """The GPU engine schedules the first K pods of config `cfg` (at `n_nodes`, default its named size); rows and
+    every option cache are dumped through the ABI and loaded into a FRESH oracle (egso_cache_load); both then schedule
+    pods [K, K+W) and must agree on all six outputs, the final rows and the final caches.  This puts the oracle into
+    the late, full-cluster regime (stale options, bind failures, unfit nodes) that a prefix from an empty cluster
+    never reaches.  Returns the window's outputs and the handle."""
+    eg = egs()
+    full = eg.workloads.config(cfg, n_nodes=n_nodes, n_pods=K + W, policy=policy)
+    e = Cluster.of_workload(full).handle()
+    pre = full.prefix(K)
+    e.schedule_batch(pre.c_off, pre.units, mode=2)
+    core, mem, _, _ = e.state_dump()
+    o = oc.OracleC(full.policy)
+    assert o.add_nodes(full.gpus, full.mem_total * full.gpus, core[:, :full.gpus], mem[:, :full.gpus]) == 0
+    shapes = eg.workloads.shapes_of(full)
+    n_cached = 0
+    for sh in shapes:
+        st, sc, am = e.option_dump(list(sh))
+        assert o.cache_load(list(sh), st == 1, sc, am) == 0
+        n_cached += int((st == 1).sum())
+    assert n_cached > 0
+    win = eg.workloads.window(full, K, W)
+    ref = o.schedule_batch(win.c_off, win.units64(), threads=threads)
+    compare_outputs(ref, e.schedule_batch(win.c_off, win.units, mode=2), f"cfg{cfg} K={K}")
+    rng = np.random.default_rng(K)
+    nodes = set(int(x) for x in rng.integers(0, full.n_nodes, sample)) | set(int(x) for x in ref["node"] if x >= 0)
+    compare_rows(e, o, nodes)
+    compare_caches(e, o, shapes, nodes, unfit_check=True)
+    return ref, e
 
 
 # ------------------------------------------------------------------------------------------------ shard groups

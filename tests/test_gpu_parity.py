@@ -2,9 +2,8 @@
 import numpy as np
 import pytest
 
-import oracle_c as oc
 from ka_vectors import KA0_FINAL, KA0_MEM, KA0_TRACE, TRADE_KA
-from oracle_harness import Cluster, compare_caches, compare_outputs, compare_rows, egs
+from oracle_harness import Cluster, compare_outputs, compare_rows, conservation, egs, late_window
 from scenario import CBackend, GpuBackend, make_scenario, run_scenario
 
 pytestmark = pytest.mark.gpu
@@ -80,52 +79,20 @@ def test_cfg4_prefix(mode):
     _compare_batch(egs().workloads.config(4, n_pods=3000), mode, threads=4)
 
 
-def _late_window(cfg, policy, K, W, threads=4, sample=4000):
-    """The GPU engine schedules the first K pods; rows and every option cache are dumped through the ABI and
-    loaded into a FRESH oracle (egso_cache_load); both then schedule pods [K, K+W) and must agree on all six
-    outputs, the final rows and the final caches.  This puts the oracle into the late, full-cluster regime
-    (stale options, bind failures, unfit nodes) that a prefix from an empty cluster never reaches."""
-    eg = egs()
-    full = eg.workloads.config(cfg, n_pods=K + W, policy=policy)
-    e = Cluster.of_workload(full).handle()
-    pre = full.prefix(K)
-    e.schedule_batch(pre.c_off, pre.units, mode=2)
-    core, mem, _, _ = e.state_dump()
-    o = oc.OracleC(full.policy)
-    for n in range(full.n_nodes):
-        o.add_node(100 * full.gpus, full.mem_total * full.gpus)
-        o.set_rows(n, core[n, :full.gpus], mem[n, :full.gpus])
-    shapes = eg.workloads.shapes_of(full)
-    n_cached = 0
-    for sh in shapes:
-        st, sc, am = e.option_dump(list(sh))
-        assert o.cache_load(list(sh), st == 1, sc, am) == 0
-        n_cached += int((st == 1).sum())
-    assert n_cached > 0
-    win = eg.workloads.window(full, K, W)
-    ref = o.schedule_batch(win.c_off, win.units64(), threads=threads)
-    compare_outputs(ref, e.schedule_batch(win.c_off, win.units, mode=2), f"cfg{cfg} K={K}")
-    rng = np.random.default_rng(K)
-    nodes = set(int(x) for x in rng.integers(0, full.n_nodes, sample)) | set(int(x) for x in ref["node"] if x >= 0)
-    compare_rows(e, o, nodes)
-    compare_caches(e, o, shapes, nodes, unfit_check=True)
-    return ref
-
-
 @pytest.mark.parametrize("K", [250_000, 500_000, 750_000, 900_000, 990_000])
 def test_cfg4_late_windows(K):
     """config 4 at full size, 3000-pod windows deep inside the 1M-pod batch (incl. the > 80 % regime)."""
-    _late_window(4, None, K, 3000)
+    late_window(4, None, K, 3000)
 
 
 @pytest.mark.parametrize("K", [100_000, 400_000])
 def test_cfg3_late_windows(K):
-    _late_window(3, None, K, 1500)
+    late_window(3, None, K, 1500)
 
 
 @pytest.mark.parametrize("K", [50_000, 90_000])
 def test_cfg2_late_windows(K):
-    _late_window(2, None, K, 5000)
+    late_window(2, None, K, 5000)
 
 
 @pytest.mark.parametrize("cfg,n_pods,vec_pods", [(0, None, 8), (1, 10000, 1500), (2, 3000, 600)])
@@ -153,26 +120,6 @@ def test_pressure_small_cluster():
         assert (ref["status"] == 3).sum() + (ref["status"] == 1).sum() > 0, "scenario must exercise failures"
 
 
-def _conservation(w, out, e):
-    """Size-independent property: final rows == initial rows - sum of successful binds."""
-    core = w.core.astype(np.int64).copy()
-    mem = w.mem.astype(np.int64).copy()
-    ok = out["status"] == 0
-    assert ((out["node"] >= 0) == (out["status"] != 1)).all()
-    for c in range(4):
-        has = ok & (np.diff(w.c_off) > c)
-        pods = np.nonzero(has)[0]
-        m = out["alloc_mask"][pods, c]
-        assert (np.bitwise_count(m) == 1).all()
-        g = np.log2(m.astype(np.float64)).astype(np.int64)
-        u = w.units[w.c_off[pods] + c]
-        np.subtract.at(core, (out["node"][pods], g), u[:, 0])
-        np.subtract.at(mem, (out["node"][pods], g), u[:, 1])
-    dc, dm, _, _ = e.state_dump()
-    assert np.array_equal(dc[:, :w.gpus], core) and np.array_equal(dm[:, :w.gpus], mem)
-    assert (core >= 0).all() and (mem >= 0).all()
-
-
 @pytest.mark.parametrize("cfg", [2, 4])
 def test_full_size_properties(cfg):
     """Full BASELINE sizes (cfg2: 10k nodes/100k pods; cfg4: 100k nodes/1M pods): the two
@@ -183,7 +130,7 @@ def test_full_size_properties(cfg):
     e2 = cl.handle()
     b = e2.schedule_batch(w.c_off, w.units, mode=2)
     compare_outputs(a, b, f"config {cfg} rounds against rescan")
-    _conservation(w, b, e2)
+    conservation(w, b, e2)
     assert (b["status"] != 1).all()   # the named clusters have room for every pod (no NOFIT);
     # status 3 (stale cached option, gpu.go:158-168) is reference behaviour and does occur under spread
 
