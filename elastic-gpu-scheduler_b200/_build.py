@@ -98,6 +98,19 @@ def build_devhost(force: bool = False) -> str:
     return LIBDEVHOST
 
 
+LIBRGEOM = os.path.join(LIBDIR, "libegs_rgeom.so")
+
+
+def build_rgeom(force: bool = False) -> str:
+    """The rounds engine's resolver geometry (mw_geometry, csrc/egs_rounds.cuh) behind a C call: CPU-side tests only."""
+    src = os.path.join(CSRC, "host_test", "rounds_geometry_on_host.cu")
+    deps = [src] + _libegs_sources()
+    if force or _stale(LIBRGEOM, deps):
+        os.makedirs(LIBDIR, exist_ok=True)
+        subprocess.check_call([nvcc_path()] + NVCC_FLAGS + ["-o", LIBRGEOM, src])
+    return LIBRGEOM
+
+
 LIBPODBOOK = os.path.join(LIBDIR, "libegs_podbook.so")
 
 
@@ -129,5 +142,6 @@ def build_all(force: bool = False) -> None:
     build_libegs(force)
     build_host(force)
     build_devhost(force)
+    build_rgeom(force)
     build_podbook(force)
     build_shim_double(force)

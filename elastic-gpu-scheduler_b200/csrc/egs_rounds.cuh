@@ -481,6 +481,52 @@ __host__ __device__ __forceinline__ MwTail mw_tail(int ns, int D, int rke, int c
   return t;
 }
 
+// ---- the resolver instance for a round set of ns shapes: f(MwInst16()), f(MwInst32()) or f(MwInst96())
+template <class F>
+static auto mw_dispatch(int ns, F &&f) {
+  if (ns <= MwInst16::NS) return f(MwInst16());
+  if (ns <= MwInst32::NS) return f(MwInst32());
+  return f(MwInst96());
+}
+#define MW_SMEM_MAX 232448   // 227 KB opt-in limit per CTA on sm_90
+
+// Pre-install (DESIGN §3.1): the resolver's prologue fills 3/4 of the tracked table with the top NT / ns merged
+// candidates of every shape (at most half of a list held in shared memory, so no list runs dry at once); the last
+// quarter stays free for first pods and new winners.  Only in the instances with kPreinstall.
+template <class I>
+static void preinstall_geometry(int ns, int rke, int &h, int &cap) {
+  h = 0; cap = 0;
+  if (!I::kPreinstall) return;
+  h = std::max(1, std::min(I::NT / std::max(ns, 1), rke / 2));
+  cap = 3 * I::NT / 4;
+}
+
+// Geometry of the resolver for a round set of ns shapes (1..RSMAX) over D shards:
+//   rkm      list depth k_merge gathers per (shape, shard) -- the instance's RKM, at most 64 above two shards: every
+//            shard contributes its own list, so the resolver holds about as many candidates per shape in total
+//   rke      list entries per (shape, shard) the resolver keeps in shared memory: rkm, or what fits next to MwSmem
+//            (even, so that what follows the lists stays 16-byte aligned); below rkm a list is truncated (`more`)
+//   smem     dynamic shared memory of k_resolve_mw
+//   pre_h, pre_cap   pre-install (preinstall_geometry)
+// batch_rounds refuses a set with rke < 4.  Pure host arithmetic.
+struct MwGeometry { int rkm, rke, pre_h, pre_cap; size_t smem; };
+static inline MwGeometry mw_geometry(int ns, int D) {
+  MwGeometry g;
+  g.rkm = mw_dispatch(ns, [](auto i) { return decltype(i)::RKM; });
+  if (D > 2) g.rkm = std::min(g.rkm, 64);
+  const int cand_bytes = make_layout(ns, g.rkm).cand_bytes;
+  g.rke = g.rkm;
+  mw_dispatch(ns, [&](auto i) {
+    using I = decltype(i);
+    const size_t avail = MW_SMEM_MAX - mw_tail<I>(ns, D, 0, cand_bytes).end;   // all but the lists
+    const size_t per = (size_t)ns * D * 8;
+    if ((size_t)g.rke * per > avail) g.rke = (int)(avail / per) & ~1;
+    g.smem = mw_tail<I>(ns, D, g.rke, cand_bytes).end;
+    preinstall_geometry<I>(ns, g.rke, g.pre_h, g.pre_cap);
+  });
+  return g;
+}
+
 // Ticket hand-over: `turn` in shared memory names the pod whose ticket is open (bookkeeping, and the stop signal);
 // the owner of the next pod SLEEPS in hardware on its own mbarrier (try_wait suspends the warp) and is woken by ONE
 // arrive of the warp that finished the previous pod.  Alternatives (tools/micro/handoff_bench.cu measures the bare
@@ -1307,6 +1353,8 @@ struct RoundsState {
   void *comm = nullptr;             // ncclComm_t
   std::shared_ptr<LocalGroup> local;                    // in-process shard group (instead of NCCL)
   cudaEvent_t ev_ready = nullptr, ev_copied = nullptr;   // own buffer written / peers' buffers copied
+  bool copied = false;              // in-process group: a round ran since egs_comm_init_local, so every peer's
+                                    // ev_copied marks its last copy of this rank's buffer (kept across batches)
   uint8_t *d_pod_sidx = nullptr; int pod_cap = 0;
   uint8_t *d_obs = nullptr; int obs_cap = 0;
   unsigned long long *d_cta_lists = nullptr; AggPart *d_cta_agg = nullptr; int grid = 0, cta_nsc = 0;

@@ -90,28 +90,9 @@ static int rounds_comm_init_local(egs_handle **handles, int world) {
       CK(h, cudaEventCreateWithFlags(&h->rounds.ev_copied, cudaEventDisableTiming));
     }
     h->rounds.local = G;
+    h->rounds.copied = false;                                   // no peer of the new group has copied anything yet
   }
   return EGS_OK;
-}
-
-// ---- the resolver instance for a round set of ns shapes: f(MwInst16()), f(MwInst32()) or f(MwInst96())
-template <class F>
-static auto mw_dispatch(int ns, F &&f) {
-  if (ns <= MwInst16::NS) return f(MwInst16());
-  if (ns <= MwInst32::NS) return f(MwInst32());
-  return f(MwInst96());
-}
-#define MW_SMEM_MAX 232448   // 227 KB opt-in limit per CTA on sm_90
-
-// Pre-install (DESIGN §3.1): the resolver's prologue fills 3/4 of the tracked table with the top NT / ns merged
-// candidates of every shape (at most half of a list held in shared memory, so no list runs dry at once); the last
-// quarter stays free for first pods and new winners.  Only in the instances with kPreinstall.
-template <class I>
-static void preinstall_geometry(int ns, int rke, int &h, int &cap) {
-  h = 0; cap = 0;
-  if (!I::kPreinstall) return;
-  h = std::max(1, std::min(I::NT / std::max(ns, 1), rke / 2));
-  cap = 3 * I::NT / 4;
 }
 
 // k_select grid: enough warps for one 128-node chunk each, at most two CTAs per SM (every CTA then runs in one wave)
@@ -188,11 +169,18 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
   }
   const bool one_set = (int)batch_shapes.size() <= RSMAX;
   const int ns_cfg = one_set ? (int)batch_shapes.size() : RSMAX;
-  int rkm = mw_dispatch(ns_cfg, [](auto i) { return decltype(i)::RKM; });
-  // sharded: every shard contributes its own list; the resolver holds about the same number of candidates per
-  // shape in total, so each shard gathers (and ships) fewer
-  if (h->world > 2) rkm = std::min(rkm, 64);                  // (the resolver keeps what its shared memory holds: rke below)
-  const BufLayout L = make_layout(ns_cfg, rkm);
+  const int D = h->world;
+  const MwGeometry geo = mw_geometry(ns_cfg, D);
+  const BufLayout L = make_layout(ns_cfg, geo.rkm);
+  // in-process group: the peers copy this rank's buffer on THEIR streams in every round, the last round of the
+  // previous batch included, and this rank synchronised only its own stream since.  Everything that rewrites or
+  // frees the buffer -- rounds_ensure's reallocation, every round's k_merge -- waits for those copies.
+  auto wait_peers_copied = [&]() -> int {
+    if (R.local && R.copied)
+      for (egs_handle *peer : R.local->members) if (peer != h) CK(h, cudaStreamWaitEvent(h->stream, peer->rounds.ev_copied, 0));
+    return EGS_OK;
+  };
+  TRY(wait_peers_copied());
   TRY(rounds_ensure(h, P, L));
 
   TableSet tb; tb.st = h->d_st; tb.sc = h->d_sc; tb.al = h->d_al; tb.n_pad = (size_t)h->n_pad; tb.n_slots = (int)h->shapes.size();
@@ -233,17 +221,8 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
   for (int p = 0; p < P; p++) h->slot_cold[slots[p]] = 0;
 
   // ---- resolver geometry
-  const int D = h->world;
-  int rke = rkm, pre_h = 0, pre_cap = 0;
-  size_t smem = 0;
-  mw_dispatch(ns_cfg, [&](auto i) {
-    using I = decltype(i);
-    const size_t avail = MW_SMEM_MAX - mw_tail<I>(ns_cfg, D, 0, L.cand_bytes).end;   // all but the lists
-    const size_t per = (size_t)ns_cfg * D * 8;
-    if ((size_t)rke * per > avail) rke = (int)(avail / per) & ~1;   // even: what follows the lists stays 16-byte aligned
-    smem = mw_tail<I>(ns_cfg, D, rke, L.cand_bytes).end;
-    preinstall_geometry<I>(ns_cfg, rke, pre_h, pre_cap);
-  });
+  const int rke = geo.rke;
+  const size_t smem = geo.smem;
   if (rke < 4) return fail(h, EGS_ERR_BAD_ARG, "rounds: shape set too large for the resolver's shared memory");
   const int nw = std::max(1, std::min(ns_cfg, MW_MAX_WARPS));
 
@@ -256,16 +235,14 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
   ma.out = R.d_bufs + (size_t)h->rank * L.bytes; ma.L = L; ma.ctl = R.d_ctl;
   ra.core = h->d_core; ra.mem = h->d_mem; ra.lo = h->lo; ra.hi = h->hi; ra.policy = h->policy; ra.n_shards = D;
   ra.rd = R.d_rd; ra.tb = tb; ra.obs_pending = R.d_obs; ra.bufs = R.d_bufs; ra.L = L; ra.pod_sidx = R.d_pod_sidx;
-  ra.p0 = -1; ra.p_limit = 0; ra.out = out; ra.ctl = R.d_ctl; ra.rke = rke; ra.nw = nw; ra.pre_h = pre_h; ra.pre_cap = pre_cap;
+  ra.p0 = -1; ra.p_limit = 0; ra.out = out; ra.ctl = R.d_ctl; ra.rke = rke; ra.nw = nw; ra.pre_h = geo.pre_h; ra.pre_cap = geo.pre_cap;
 
   int ns_round = ns_cfg;                                        // grid of k_merge
-  bool local_copied = false;
   auto launch_round = [&]() -> int {
     if (h->timing) CK(h, cudaEventRecord(ev[0], h->stream));
     k_select<<<grid, SEL_THREADS, 0, h->stream>>>(sa);
     if (h->timing) CK(h, cudaEventRecord(ev[1], h->stream));
-    if (local_copied)                                           // peers must have copied my previous buffer before k_merge rewrites it
-      for (egs_handle *peer : R.local->members) if (peer != h) CK(h, cudaStreamWaitEvent(h->stream, peer->rounds.ev_copied, 0));
+    TRY(wait_peers_copied());                                   // peers must have copied my previous buffer before k_merge rewrites it
     k_merge<<<ns_round, 256, 0, h->stream>>>(ma);
     if (h->world > 1 && R.local) {
       // in-process group: wait until no peer still reads my buffer of the previous round (enqueued BEFORE k_merge
@@ -281,7 +258,7 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
       }
       CK(h, cudaEventRecord(R.ev_copied, h->stream));
       if (!G.barrier()) return fail(h, EGS_ERR_COMM, "in-process shard group: a member did not arrive");   // all recorded ev_copied
-      local_copied = true;
+      R.copied = true;
     } else if (h->world > 1)
       NCK(h, nccl_api()->AllGather(R.d_bufs + (size_t)h->rank * L.bytes, R.d_bufs, (size_t)L.bytes, ncclChar, (ncclComm_t)R.comm, h->stream));
     if (h->timing) CK(h, cudaEventRecord(ev[2], h->stream));

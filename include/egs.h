@@ -278,7 +278,17 @@ int egs_schedule_batch_device(egs_handle *h, int mode, int n_pods, const int32_t
  * FULL cluster; the batch loop exchanges the per-shape candidate buffers with ncclAllGather once per
  * round and every rank returns identical per-pod outputs.  After a sharded batch a rank's rows and
  * option tables are current only for its own range, so the single-pod verbs and egs_state_dump must be
- * addressed to the owner of the node.  NCCL is resolved at run time with dlopen("libnccl.so.2"). */
+ * addressed to the owner of the node.  NCCL is resolved at run time with dlopen("libnccl.so.2").
+ *
+ * Which rank gets which call, so that every rank's view of its own range stays the unsharded one:
+ *   - every rank, with the same arguments and in the same order: node loads (egs_node_set_allocatable,
+ *     egs_node_set, egs_state_load, egs_state_load_bulk), the accounting verbs (egs_pod_apply,
+ *     egs_node_replay_pod, egs_pod_cancel), mutation records (egs_mutations_apply), batches
+ *     (egs_schedule_batch, egs_schedule_batch_mut, egs_schedule_batch_device), snapshot / restore and checkpoints;
+ *   - the owner of the node (egs_shard_range) alone: egs_filter, egs_score, egs_bind, egs_option_peek,
+ *     egs_option_dump and egs_state_dump, over node ids of its own range.
+ * A bind's uid enters the owner's pod maps only (egs_pod_known / egs_pod_released of it are the owner's); the uids
+ * of a batch and of accounting verbs and records enter every rank's. */
 int egs_shard_set(egs_handle *h, int rank, int world);
 /* The contiguous node range [lo, hi) egs_shard_set gives rank `rank` of `world` (pure host
  * arithmetic, no handle): boundaries are multiples of 128, the last shard ends at max_nodes. */

@@ -446,6 +446,22 @@ void egso_get_rows_many(egso *o, int n, const int32_t *node_ids, int width, int6
     gpu_count[i] = nd->G;
   }
 }
+/* A node reloaded in place (node.go:23-59 on an update: a new NodeAllocator for an existing node): G, M and fresh
+ * rows as egso_add_node, then the rows core / mem ([G]; NULL keeps the fresh rows).  The node's option cache and
+ * podsMap are emptied; podMaps / releasedPodMap (scheduler level) stay.  -1 when G is out of range (node unchanged). */
+int egso_node_reset(egso *o, int node, int64_t core_allocatable, int64_t mem_allocatable, const int64_t *core,
+                    const int64_t *mem) {
+  const int64_t G = core_allocatable / CORE_EACH_CARD;
+  if (node < 0 || node >= o->nn || G == 0 || G > EGSO_MAX_G) return -1;
+  node_t *nd = &o->nodes[node];
+  free(nd->cache); free(nd->pods);
+  memset(nd, 0, sizeof *nd);
+  nd->G = (int)G;
+  const int64_t m = mem_allocatable / G;
+  for (int i = 0; i < nd->G; i++) { nd->g[i].ca = nd->g[i].ct = CORE_EACH_CARD; nd->g[i].ma = nd->g[i].mt = m; }
+  if (core && mem) egso_set_rows(o, node, core, mem);
+  return 0;
+}
 int egso_num_nodes(egso *o) { return o->nn; }
 int egso_gpu_count(egso *o, int node) { return o->nodes[node].G; }
 void egso_set_rows(egso *o, int node, const int64_t *core, const int64_t *mem) {

@@ -35,6 +35,10 @@ int egso_add_node(egso *o, int64_t core_allocatable, int64_t mem_allocatable);
 int egso_add_nodes(egso *o, int n, int G, int64_t mem_alloc, const int64_t *core, const int64_t *mem);
 void egso_get_rows_many(egso *o, int n, const int32_t *node_ids, int width, int64_t *core, int64_t *mem,
                         int32_t *gpu_count);
+/* A node reloaded in place: a new NodeAllocator for an existing id (fresh rows, then core / mem [G] unless NULL);
+ * its option cache and podsMap are emptied, podMaps / releasedPodMap stay.  0, or -1 (G out of range). */
+int egso_node_reset(egso *o, int node, int64_t core_allocatable, int64_t mem_allocatable, const int64_t *core,
+                    const int64_t *mem);
 int egso_num_nodes(egso *o);
 int egso_gpu_count(egso *o, int node);
 void egso_set_rows(egso *o, int node, const int64_t *core, const int64_t *mem);

@@ -45,6 +45,7 @@ def lib():
         L.egso_add_node.argtypes = [C.c_void_p, C.c_int64, C.c_int64]
         L.egso_add_nodes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_void_p]
         L.egso_get_rows_many.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.egso_node_reset.argtypes = [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]
         L.egso_num_nodes.argtypes = [C.c_void_p]
         L.egso_gpu_count.argtypes = [C.c_void_p, C.c_int]
         L.egso_set_rows.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
@@ -130,6 +131,15 @@ class OracleC:
         gc = np.zeros(len(ids), np.int32)
         self.L.egso_get_rows_many(self.h, len(ids), _ptr(ids), width, _ptr(core), _ptr(mem), _ptr(gc))
         return core, mem, gc
+
+    def node_reset(self, node: int, core_alloc: int, mem_alloc: int, core=None, mem=None) -> int:
+        """Reload an existing node (egs_node_set_allocatable, or one node of egs_state_load_bulk when core / mem
+        are given): fresh rows of the new size, then core / mem; its option cache and podsMap are emptied."""
+        if core is None:
+            return self.L.egso_node_reset(self.h, node, core_alloc, mem_alloc, None, None)
+        c = np.ascontiguousarray(core, dtype=np.int64)
+        m = np.ascontiguousarray(mem, dtype=np.int64)
+        return self.L.egso_node_reset(self.h, node, core_alloc, mem_alloc, _ptr(c), _ptr(m))
 
     @property
     def n_nodes(self) -> int:
