@@ -124,6 +124,19 @@ def build_podbook(force: bool = False) -> str:
     return LIBPODBOOK
 
 
+LIBBUFFERS = os.path.join(LIBDIR, "libegs_buffers.so")
+
+
+def build_buffers(force: bool = False) -> str:
+    """The buffer owner (csrc/buffers.h) over a fake allocator behind a small C API: CPU-side tests only."""
+    src = os.path.join(CSRC, "host_test", "buffers_on_host.cc")
+    deps = [src, os.path.join(CSRC, "buffers.h")]
+    if force or _stale(LIBBUFFERS, deps):
+        os.makedirs(LIBDIR, exist_ok=True)
+        subprocess.check_call([nvcc_path()] + NVCC_FLAGS + ["-o", LIBBUFFERS, src])
+    return LIBBUFFERS
+
+
 SHIM_DOUBLE = os.path.join(ROOT, "integration", "_build", "shim_double")
 
 
@@ -144,4 +157,5 @@ def build_all(force: bool = False) -> None:
     build_devhost(force)
     build_rgeom(force)
     build_podbook(force)
+    build_buffers(force)
     build_shim_double(force)

@@ -13,29 +13,48 @@
 #include <unordered_set>
 #include <vector>
 
+#include "buffers.h"
 #include "egs_kernels.cuh"
 #include "egs_rounds.cuh"
 #include "pod_book.h"
 
 struct Shape { int C; egs_unit u[EGS_C]; };
 
-// Pinned host buffer holding (node[n], status[n]) of a batch.  Recycled through egs_handle::pin_pool: cudaMallocHost /
-// cudaFreeHost cost milliseconds and synchronise the device -- too much for a small batch on the extender's path.
-struct PinBuf { int32_t *p = nullptr; size_t cap = 0; };   // cap in int32 elements
+// Pinned host buffer holding (node[n], status[n]) of a batch.  Recycled through egs_handle::pin_pool: allocating and
+// freeing pinned memory cost milliseconds and synchronise the device -- too much for a small batch on the extender's path.
+using PinBuf = PinnedBuf<int32_t>;
 struct PendingBatch {           // results of a batch whose uid bookkeeping is applied lazily
   int n; uint64_t uid0; std::vector<uint64_t> uids; int32_t *h_node, *h_status; PinBuf buf; cudaEvent_t done;
 };
 
 struct ShapeCacheEnt { uint64_t h; int slot; };   // open-addressing entry of egs_handle::shape_cache
 
+// The rows of every node: free_core / free_mem / mem_total on the device and the host's gpu_count / mem_total, which
+// also say which nodes are set.  A snapshot and a checkpoint each hold one; its device buffers are allocated on the
+// first save.
+struct RowImage {
+  DeviceBuf<int32_t> d_core, d_mem, d_mem_total;
+  std::vector<int32_t> h_gpu_count, h_mem_total;
+  int save(egs_handle *h);
+  int load(egs_handle *h) const;
+};
+
+// The option tables of `slots` slots: state, score and masks, each array one contiguous slice per slot (table()).  The
+// handle's live tables and a checkpoint's copy.
+struct OptTables {
+  DeviceBuf<uint8_t> st; DeviceBuf<int32_t> sc; DeviceBuf<uint8_t> al;
+  int slots = 0;
+  int grow(egs_handle *h, int cap);                      // keeps every slot held; the new slots' states read OPT_ABSENT
+  int copy_from(egs_handle *h, const OptTables &o, int n);   // slots [0, n) of o
+};
+
 // egs_checkpoint_save: the complete scheduler state but the PodBook, which keeps its own undo journal.  The device
 // buffers are allocated on the first save and grown when more shapes are interned.
 struct Checkpoint {
   bool open = false;
-  int32_t *d_core = nullptr, *d_mem = nullptr, *d_mem_total = nullptr;
-  uint8_t *d_st = nullptr; int32_t *d_sc = nullptr; uint8_t *d_al = nullptr; int slot_cap = 0;
+  RowImage rows;
+  OptTables tables;
   int n_shapes = 0;                       // shapes interned at the save; later ones are forgotten by the rollback
-  std::vector<int32_t> gpu_count, mem_total;
   std::vector<char> slot_cold;
   std::vector<ShapeCacheEnt> shape_cache;
   uint64_t next_uid = 0;
@@ -46,13 +65,10 @@ struct egs_handle {
   int row_w = EGS_G, mask_b = 1;          // EGS_ROW_WIDTH(g_max), EGS_MASK_BYTES(g_max)
   int rank = 0, world = 1, lo = 0, hi = 0;
   cudaStream_t stream = nullptr;
-  int32_t *d_core = nullptr, *d_mem = nullptr, *d_mem_total = nullptr;
-  int32_t *d_snap_core = nullptr, *d_snap_mem = nullptr, *d_snap_total = nullptr;
-  std::vector<int32_t> snap_gpu_count, snap_mem_total;
+  DeviceBuf<int32_t> d_core, d_mem, d_mem_total;
   std::vector<int32_t> h_gpu_count, h_mem_total;
-  // option tables
-  int slot_cap = 0;
-  uint8_t *d_st = nullptr; int32_t *d_sc = nullptr; uint8_t *d_al = nullptr;
+  RowImage snap;
+  OptTables tables;
   std::vector<Shape> shapes;
   std::vector<char> slot_cold;            // option table of the slot holds only OPT_ABSENT (nothing evaluated yet)
   std::unordered_map<std::string, int> shape_ids;
@@ -64,17 +80,17 @@ struct egs_handle {
   std::vector<PinBuf> pin_pool;                                 // idle pinned result buffers (at most PIN_POOL_MAX)
   uint64_t next_uid = 0x8000000000000000ull;
   // scratch
-  Partial *d_partials = nullptr; unsigned int *d_ticket = nullptr; int32_t *d_result = nullptr;
-  int32_t *h_result = nullptr;                                  // pinned
-  int32_t *d_ids = nullptr; uint8_t *d_fit = nullptr; int32_t *d_score = nullptr; size_t gather_cap = 0;
-  void *h_stage = nullptr; size_t h_stage_cap = 0;              // pinned staging
+  DeviceBuf<Partial> d_partials; DeviceBuf<unsigned int> d_ticket; DeviceBuf<int32_t> d_result;
+  PinnedBuf<int32_t> h_result;
+  DeviceBuf<int32_t> d_ids; DeviceBuf<uint8_t> d_fit; DeviceBuf<int32_t> d_score;
+  PinnedBuf<char> h_stage;                                      // staging
   // eval scratch (profile)
-  uint8_t *d_ev_fit = nullptr; int32_t *d_ev_score = nullptr; uint8_t *d_ev_gpu = nullptr; void *d_flush = nullptr;
+  DeviceBuf<uint8_t> d_ev_fit; DeviceBuf<int32_t> d_ev_score; DeviceBuf<uint8_t> d_ev_gpu; DeviceBuf<char> d_flush;
   // batch outputs
-  int32_t *d_o_node = nullptr, *d_o_status = nullptr, *d_o_fit = nullptr; uint8_t *d_o_alloc = nullptr;
-  unsigned long long *d_o_fd = nullptr, *d_o_sd = nullptr; int out_cap = 0;
-  void *d_ops = nullptr; int32_t *d_group_off = nullptr; size_t ops_cap = 0;   // egs_mutations_apply: ApplyOp<row_w>[]
-  uint8_t *d_vec_fit = nullptr; int32_t *d_vec_score = nullptr; size_t vec_cap = 0; int vec_pods = 0;   // egs_schedule_batch_vec
+  DeviceBuf<int32_t> d_o_node, d_o_status, d_o_fit; DeviceBuf<uint8_t> d_o_alloc;
+  DeviceBuf<unsigned long long> d_o_fd, d_o_sd;
+  DeviceBuf<char> d_ops; DeviceBuf<int32_t> d_group_off;       // egs_mutations_apply: ApplyOp<row_w>[]
+  DeviceBuf<uint8_t> d_vec_fit; DeviceBuf<int32_t> d_vec_score; int vec_pods = 0;   // egs_schedule_batch_vec
   // profiling
   int64_t k_launches[EGS_K_COUNT] = {0}; double k_ms[EGS_K_COUNT] = {0}; int timing = 0;
   RoundsState rounds;
@@ -110,41 +126,32 @@ static void put_masks(const egs_handle *h, uint64_t masks, uint8_t *out) {
 }
 
 static int ensure_stage(egs_handle *h, size_t bytes) {
-  if (bytes <= h->h_stage_cap) return EGS_OK;
-  if (h->h_stage) cudaFreeHost(h->h_stage);
-  h->h_stage = nullptr; h->h_stage_cap = 0;
-  size_t cap = std::max(bytes, (size_t)1 << 20);
-  CK(h, cudaMallocHost(&h->h_stage, cap));
-  h->h_stage_cap = cap;
+  if (bytes > h->h_stage.cap()) CK(h, grow(h->stream, false, to(h->h_stage, std::max(bytes, (size_t)1 << 20))));
   return EGS_OK;
 }
 
 static OptTable table(egs_handle *h, int slot) {
   OptTable t;
   t.plane = (size_t)h->n_pad;
-  t.st = h->d_st + (size_t)slot * h->n_pad;
-  t.sc = h->d_sc + (size_t)slot * h->n_pad;
-  t.al = h->d_al + (size_t)slot * EGS_C * h->n_pad * h->mask_b;
+  t.st = h->tables.st + (size_t)slot * h->n_pad;
+  t.sc = h->tables.sc + (size_t)slot * h->n_pad;
+  t.al = h->tables.al + (size_t)slot * EGS_C * h->n_pad * h->mask_b;
   return t;
 }
 
-static int grow_slots(egs_handle *h, int need) {
-  if (need <= h->slot_cap) return EGS_OK;
-  int cap = std::max(need, std::max(16, h->slot_cap * 2));
-  uint8_t *st; int32_t *sc; uint8_t *al;
-  size_t np = (size_t)h->n_pad, al_plane = np * EGS_C * h->mask_b;
-  CK(h, cudaMalloc(&st, np * cap));
-  CK(h, cudaMalloc(&sc, np * cap * sizeof(int32_t)));
-  CK(h, cudaMalloc(&al, al_plane * cap));
-  CK(h, cudaMemsetAsync(st, OPT_ABSENT, np * cap, h->stream));
-  if (h->slot_cap) {
-    CK(h, cudaMemcpyAsync(st, h->d_st, np * h->slot_cap, cudaMemcpyDeviceToDevice, h->stream));
-    CK(h, cudaMemcpyAsync(sc, h->d_sc, np * h->slot_cap * sizeof(int32_t), cudaMemcpyDeviceToDevice, h->stream));
-    CK(h, cudaMemcpyAsync(al, h->d_al, al_plane * h->slot_cap, cudaMemcpyDeviceToDevice, h->stream));
-    CK(h, cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_st); cudaFree(h->d_sc); cudaFree(h->d_al);
-  }
-  h->d_st = st; h->d_sc = sc; h->d_al = al; h->slot_cap = cap;
+int OptTables::grow(egs_handle *h, int cap) {
+  const size_t np = (size_t)h->n_pad, al_plane = np * EGS_C * h->mask_b;
+  CK(h, ::grow(h->stream, true, to(st, np * cap), to(sc, np * cap), to(al, al_plane * cap)));
+  CK(h, cudaMemsetAsync(st + np * slots, OPT_ABSENT, np * (cap - slots), h->stream));
+  slots = cap;
+  return EGS_OK;
+}
+
+int OptTables::copy_from(egs_handle *h, const OptTables &o, int n) {
+  const size_t np = (size_t)h->n_pad, al_plane = np * EGS_C * h->mask_b;
+  CK(h, st.copy_from(o.st, np * n, h->stream));
+  CK(h, sc.copy_from(o.sc, np * n, h->stream));
+  CK(h, al.copy_from(o.al, al_plane * n, h->stream));
   return EGS_OK;
 }
 
@@ -206,7 +213,7 @@ static int intern_slow(egs_handle *h, int C, const egs_unit *u, int *slot) {
   auto it = h->shape_ids.find(key);
   if (it != h->shape_ids.end()) { *slot = it->second; return EGS_OK; }
   int s = (int)h->shapes.size();
-  TRY(grow_slots(h, s + 1));
+  if (s + 1 > h->tables.slots) TRY(h->tables.grow(h, std::max(s + 1, h->tables.slots * 2)));
   Shape sh; sh.C = C; memset(sh.u, 0, sizeof sh.u); memcpy(sh.u, u, sizeof(egs_unit) * C);
   h->shapes.push_back(sh);
   h->slot_cold.push_back(1);
@@ -219,16 +226,16 @@ static bool is_single(int C, const egs_unit *u) { return C == 1 && u[0].count ==
 
 constexpr size_t PIN_POOL_MAX = 4;
 static void pin_put(egs_handle *h, PinBuf b) {
-  if (!b.p) return;
-  if (h->pin_pool.size() < PIN_POOL_MAX) h->pin_pool.push_back(b); else cudaFreeHost(b.p);
+  if (b && h->pin_pool.size() < PIN_POOL_MAX) h->pin_pool.push_back(std::move(b));
 }
 
-static int flush_pending(egs_handle *h) {
+// Waits for the batches in flight and moves their results into the book (apply), or drops them.
+static int settle_pending(egs_handle *h, bool apply) {
   for (auto &b : h->pending) {
     CK(h, cudaEventSynchronize(b.done));
-    if (b.uids.empty()) h->book.add_run(b.uid0, b.n, b.h_node, b.h_status);     // library-assigned uids
-    else h->book.add_batch(b.uids.data(), b.n, b.h_node, b.h_status);
-    pin_put(h, b.buf); cudaEventDestroy(b.done);
+    if (apply && b.uids.empty()) h->book.add_run(b.uid0, b.n, b.h_node, b.h_status);     // library-assigned uids
+    else if (apply) h->book.add_batch(b.uids.data(), b.n, b.h_node, b.h_status);
+    pin_put(h, std::move(b.buf)); cudaEventDestroy(b.done);
   }
   h->pending.clear();
   return EGS_OK;
@@ -242,23 +249,23 @@ struct Guard {
 static int pin_get(egs_handle *h, size_t n, PinBuf *out) {
   int best = -1;                                                // smallest idle buffer that is large enough
   for (size_t i = 0; i < h->pin_pool.size(); i++)
-    if (h->pin_pool[i].cap >= n && (best < 0 || h->pin_pool[i].cap < h->pin_pool[(size_t)best].cap)) best = (int)i;
-  if (best >= 0) { *out = h->pin_pool[(size_t)best]; h->pin_pool.erase(h->pin_pool.begin() + best); return EGS_OK; }
-  PinBuf b; b.cap = std::max(n, (size_t)4096);
-  CK(h, cudaMallocHost(&b.p, b.cap * sizeof(int32_t)));
-  *out = b;
+    if (h->pin_pool[i].cap() >= n && (best < 0 || h->pin_pool[i].cap() < h->pin_pool[(size_t)best].cap())) best = (int)i;
+  if (best >= 0) { *out = std::move(h->pin_pool[(size_t)best]); h->pin_pool.erase(h->pin_pool.begin() + best); return EGS_OK; }
+  CK(h, grow(h->stream, false, to(*out, std::max(n, (size_t)4096))));
   return EGS_OK;
 }
 
 static void checkpoint_free(egs_handle *h) {
-  Checkpoint &k = h->ck;
-  if (k.d_core) {
-    cudaStreamSynchronize(h->stream);             // no copy into these buffers is still in flight
-    void *dev[] = {k.d_core, k.d_mem, k.d_mem_total, k.d_st, k.d_sc, k.d_al};
-    for (void *p : dev) if (p) cudaFree(p);
-  }
+  if (h->ck.rows.d_core) cudaStreamSynchronize(h->stream);   // no copy into the checkpoint's buffers is still in flight
   h->ck = Checkpoint();
   h->book.drop_checkpoint();
+}
+
+// The handle and everything it owns; the stream goes last.
+static void free_handle(egs_handle *h) {
+  cudaStream_t s = h->stream;
+  delete h;
+  if (s) cudaStreamDestroy(s);
 }
 
 // ------------------------------------------------------------------------------- lifecycle
@@ -277,27 +284,22 @@ extern "C" int egs_create(int policy, int max_nodes, int g_max, int device, egs_
     CK(h, cudaSetDevice(device));
     CK(h, cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device));
     CK(h, cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    size_t rows = (size_t)h->n_pad * h->row_w * sizeof(int32_t);
-    CK(h, cudaMalloc(&h->d_core, rows));
-    CK(h, cudaMalloc(&h->d_mem, rows));
-    CK(h, cudaMalloc(&h->d_mem_total, (size_t)h->n_pad * sizeof(int32_t)));
+    const size_t cells = (size_t)h->n_pad * h->row_w;
+    CK(h, grow(h->stream, false, to(h->d_core, cells), to(h->d_mem, cells), to(h->d_mem_total, h->n_pad)));
     CK(h, cudaMemsetAsync(h->d_mem_total, 0, (size_t)h->n_pad * sizeof(int32_t), h->stream));
     // EGS_PAD == 0x80000000: fill through a pinned pattern-free path (memset is per byte)
-    std::vector<int32_t> pad((size_t)h->n_pad * h->row_w, EGS_PAD);
-    CK(h, cudaMemcpy(h->d_core, pad.data(), rows, cudaMemcpyHostToDevice));
-    CK(h, cudaMemcpy(h->d_mem, pad.data(), rows, cudaMemcpyHostToDevice));
+    std::vector<int32_t> pad(cells, EGS_PAD);
+    CK(h, cudaMemcpy(h->d_core, pad.data(), cells * sizeof(int32_t), cudaMemcpyHostToDevice));
+    CK(h, cudaMemcpy(h->d_mem, pad.data(), cells * sizeof(int32_t), cudaMemcpyHostToDevice));
     int nblk = (h->n_pad + PASS_THREADS - 1) / PASS_THREADS;
-    CK(h, cudaMalloc(&h->d_partials, sizeof(Partial) * (size_t)nblk));
-    CK(h, cudaMalloc(&h->d_ticket, sizeof(unsigned int) * 4));
+    CK(h, grow(h->stream, false, to(h->d_partials, nblk), to(h->d_ticket, 4), to(h->d_result, 16), to(h->h_result, 16)));
     CK(h, cudaMemsetAsync(h->d_ticket, 0, sizeof(unsigned int) * 4, h->stream));
-    CK(h, cudaMalloc(&h->d_result, sizeof(int32_t) * 16));
-    CK(h, cudaMallocHost(&h->h_result, sizeof(int32_t) * 16));
-    TRY(grow_slots(h, 16));
+    TRY(h->tables.grow(h, 16));
     CK(h, cudaStreamSynchronize(h->stream));
     return EGS_OK;
   };
   int rc = boot();
-  if (rc != EGS_OK) { fprintf(stderr, "egs_create: %s\n", h->err.c_str()); delete h; return rc; }
+  if (rc != EGS_OK) { fprintf(stderr, "egs_create: %s\n", h->err.c_str()); free_handle(h); return rc; }
   *out = h;
   return EGS_OK;
 }
@@ -306,19 +308,9 @@ extern "C" int egs_destroy(egs_handle *h) {
   if (!h) return EGS_ERR_BAD_ARG;
   cudaSetDevice(h->device);
   cudaStreamSynchronize(h->stream);
-  flush_pending(h);
-  for (auto &b : h->pin_pool) cudaFreeHost(b.p);
-  h->pin_pool.clear();
+  settle_pending(h, true);
   rounds_free(&h->rounds);
-  checkpoint_free(h);
-  void *dev[] = {h->d_core, h->d_mem, h->d_mem_total, h->d_st, h->d_sc, h->d_al, h->d_partials, h->d_ticket, h->d_snap_core, h->d_snap_mem, h->d_snap_total,
-                 h->d_result, h->d_ids, h->d_fit, h->d_score, h->d_ev_fit, h->d_ev_score, h->d_ev_gpu, h->d_flush,
-                 h->d_o_node, h->d_o_status, h->d_o_fit, h->d_o_alloc, h->d_o_fd, h->d_o_sd, h->d_vec_fit, h->d_vec_score, h->d_ops, h->d_group_off};
-  for (void *p : dev) if (p) cudaFree(p);
-  if (h->h_result) cudaFreeHost(h->h_result);
-  if (h->h_stage) cudaFreeHost(h->h_stage);
-  cudaStreamDestroy(h->stream);
-  delete h;
+  free_handle(h);
   return EGS_OK;
 }
 
@@ -359,10 +351,15 @@ extern "C" int egs_unit_from_requests(int64_t core, int64_t mem, egs_unit *out) 
 }
 
 // ------------------------------------------------------------------------------- node cache
+static int check_node(const egs_handle *h, int node) {
+  if (node < 0 || node >= h->max_nodes) return EGS_ERR_BAD_ARG;
+  return h->h_gpu_count[node] == 0 ? EGS_ERR_NO_NODE : EGS_OK;
+}
+
 static int reset_nodes(egs_handle *h, int node0, int n, int full) {
   int ns = (int)h->shapes.size();
   if (ns == 0 || n <= 0) return EGS_OK;
-  k_node_reset<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_st, (size_t)h->n_pad, ns, node0, n, full);
+  k_node_reset<<<(n + 255) / 256, 256, 0, h->stream>>>(h->tables.st, (size_t)h->n_pad, ns, node0, n, full);
   CK(h, cudaGetLastError());
   return EGS_OK;
 }
@@ -376,7 +373,7 @@ static int load_rows(egs_handle *h, int node0, int n, int gpu_count, int mem_tot
   size_t cells = (size_t)n * W;
   TRY(ensure_stage(h, cells * 2 * sizeof(int32_t) + (size_t)n * sizeof(int32_t)));
   CK(h, cudaStreamSynchronize(h->stream));   // staging buffer reuse
-  int32_t *sc = (int32_t *)h->h_stage, *sm = sc + cells, *st = sm + cells;
+  int32_t *sc = (int32_t *)h->h_stage.get(), *sm = sc + cells, *st = sm + cells;
   for (int i = 0; i < n; i++) {
     for (int g = 0; g < W; g++) {
       int32_t cv = EGS_PAD, mv = EGS_PAD;
@@ -398,20 +395,10 @@ static int load_rows(egs_handle *h, int node0, int n, int gpu_count, int mem_tot
   return EGS_OK;
 }
 
-// wait for in-flight batches and drop their bookkeeping without applying it
-static int discard_pending(egs_handle *h) {
-  for (auto &b : h->pending) {
-    CK(h, cudaEventSynchronize(b.done));
-    pin_put(h, b.buf); cudaEventDestroy(b.done);
-  }
-  h->pending.clear();
-  return EGS_OK;
-}
-
 extern "C" int egs_node_set(egs_handle *h, int node_id, int gpu_count, int mem_total_per_gpu) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  TRY(flush_pending(h));
+  TRY(settle_pending(h, true));
   TRY(load_rows(h, node_id, 1, gpu_count, mem_total_per_gpu, nullptr, nullptr, true));
   h->book.drop_nodes(node_id, 1);
   return EGS_OK;
@@ -430,8 +417,7 @@ extern "C" int egs_node_set_allocatable(egs_handle *h, int node_id, int64_t core
 extern "C" int egs_state_load(egs_handle *h, int node_id, const int32_t *free_core, const int32_t *free_mem) {
   if (!h || !free_core || !free_mem) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  if (node_id < 0 || node_id >= h->max_nodes) return EGS_ERR_BAD_ARG;
-  if (h->h_gpu_count[node_id] == 0) return EGS_ERR_NO_NODE;
+  TRY(check_node(h, node_id));
   return load_rows(h, node_id, 1, h->h_gpu_count[node_id], h->h_mem_total[node_id], free_core, free_mem, false);
 }
 
@@ -440,7 +426,7 @@ extern "C" int egs_state_load_bulk(egs_handle *h, int node0, int n, int gpu_coun
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
   // pending batch results only feed podsMap/podMaps; podMaps (scheduler level) survives a node reload
-  TRY(flush_pending(h));
+  TRY(settle_pending(h, true));
   TRY(load_rows(h, node0, n, gpu_count, mem_total, free_core, free_mem, true));
   h->book.drop_nodes(node0, n);
   return EGS_OK;
@@ -453,7 +439,7 @@ extern "C" int egs_state_dump(egs_handle *h, int node0, int n, int32_t *free_cor
   if (node0 < 0 || n < 0 || node0 + n > h->max_nodes) return EGS_ERR_BAD_ARG;
   size_t cells = (size_t)n * h->row_w;
   TRY(ensure_stage(h, cells * 2 * sizeof(int32_t)));
-  int32_t *sc = (int32_t *)h->h_stage, *sm = sc + cells;
+  int32_t *sc = (int32_t *)h->h_stage.get(), *sm = sc + cells;
   CK(h, cudaMemcpyAsync(sc, h->d_core + (size_t)node0 * h->row_w, cells * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaMemcpyAsync(sm, h->d_mem + (size_t)node0 * h->row_w, cells * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaStreamSynchronize(h->stream));
@@ -466,19 +452,29 @@ extern "C" int egs_state_dump(egs_handle *h, int node0, int n, int32_t *free_cor
   return EGS_OK;
 }
 
+int RowImage::save(egs_handle *h) {
+  const size_t cells = (size_t)h->n_pad * h->row_w;
+  if (!d_core) CK(h, grow(h->stream, false, to(d_core, cells), to(d_mem, cells), to(d_mem_total, h->n_pad)));
+  CK(h, d_core.copy_from(h->d_core, cells, h->stream));
+  CK(h, d_mem.copy_from(h->d_mem, cells, h->stream));
+  CK(h, d_mem_total.copy_from(h->d_mem_total, h->n_pad, h->stream));
+  h_gpu_count = h->h_gpu_count; h_mem_total = h->h_mem_total;
+  return EGS_OK;
+}
+
+int RowImage::load(egs_handle *h) const {
+  const size_t cells = (size_t)h->n_pad * h->row_w;
+  CK(h, h->d_core.copy_from(d_core, cells, h->stream));
+  CK(h, h->d_mem.copy_from(d_mem, cells, h->stream));
+  CK(h, h->d_mem_total.copy_from(d_mem_total, h->n_pad, h->stream));
+  h->h_gpu_count = h_gpu_count; h->h_mem_total = h_mem_total;
+  return EGS_OK;
+}
+
 extern "C" int egs_state_snapshot(egs_handle *h) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  const size_t rows = (size_t)h->n_pad * h->row_w * sizeof(int32_t);
-  if (!h->d_snap_core) {
-    CK(h, cudaMalloc(&h->d_snap_core, rows));
-    CK(h, cudaMalloc(&h->d_snap_mem, rows));
-    CK(h, cudaMalloc(&h->d_snap_total, (size_t)h->n_pad * sizeof(int32_t)));
-  }
-  CK(h, cudaMemcpyAsync(h->d_snap_core, h->d_core, rows, cudaMemcpyDeviceToDevice, h->stream));
-  CK(h, cudaMemcpyAsync(h->d_snap_mem, h->d_mem, rows, cudaMemcpyDeviceToDevice, h->stream));
-  CK(h, cudaMemcpyAsync(h->d_snap_total, h->d_mem_total, (size_t)h->n_pad * sizeof(int32_t), cudaMemcpyDeviceToDevice, h->stream));
-  h->snap_gpu_count = h->h_gpu_count; h->snap_mem_total = h->h_mem_total;
+  TRY(h->snap.save(h));
   CK(h, cudaStreamSynchronize(h->stream));
   return EGS_OK;
 }
@@ -486,72 +482,28 @@ extern "C" int egs_state_snapshot(egs_handle *h) {
 extern "C" int egs_state_restore(egs_handle *h) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  if (!h->d_snap_core) return fail(h, EGS_ERR_BAD_ARG, "no snapshot");
-  TRY(discard_pending(h));
-  const size_t rows = (size_t)h->n_pad * h->row_w * sizeof(int32_t);
-  CK(h, cudaMemcpyAsync(h->d_core, h->d_snap_core, rows, cudaMemcpyDeviceToDevice, h->stream));
-  CK(h, cudaMemcpyAsync(h->d_mem, h->d_snap_mem, rows, cudaMemcpyDeviceToDevice, h->stream));
-  CK(h, cudaMemcpyAsync(h->d_mem_total, h->d_snap_total, (size_t)h->n_pad * sizeof(int32_t), cudaMemcpyDeviceToDevice, h->stream));
+  if (!h->snap.d_core) return fail(h, EGS_ERR_BAD_ARG, "no snapshot");
+  TRY(settle_pending(h, false));
+  TRY(h->snap.load(h));
   if (!h->shapes.empty())
-    CK(h, cudaMemsetAsync(h->d_st, OPT_ABSENT, (size_t)h->n_pad * h->shapes.size(), h->stream));
+    CK(h, cudaMemsetAsync(h->tables.st, OPT_ABSENT, (size_t)h->n_pad * h->shapes.size(), h->stream));
   std::fill(h->slot_cold.begin(), h->slot_cold.end(), 1);
-  h->h_gpu_count = h->snap_gpu_count; h->h_mem_total = h->snap_mem_total;
   h->book.clear();
-  return EGS_OK;
-}
-
-// Option tables of slots [0, ns) between the handle's arrays and a checkpoint's.  Each array is one contiguous slice
-// per slot (table()), so every array is one copy.
-static int copy_tables(egs_handle *h, int ns, bool save) {
-  Checkpoint &k = h->ck;
-  const size_t np = (size_t)h->n_pad, al_plane = np * EGS_C * h->mask_b;
-  uint8_t *st = save ? k.d_st : h->d_st, *al = save ? k.d_al : h->d_al; int32_t *sc = save ? k.d_sc : h->d_sc;
-  const uint8_t *st0 = save ? h->d_st : k.d_st, *al0 = save ? h->d_al : k.d_al; const int32_t *sc0 = save ? h->d_sc : k.d_sc;
-  if (ns == 0) return EGS_OK;
-  CK(h, cudaMemcpyAsync(st, st0, np * ns, cudaMemcpyDeviceToDevice, h->stream));
-  CK(h, cudaMemcpyAsync(sc, sc0, np * ns * sizeof(int32_t), cudaMemcpyDeviceToDevice, h->stream));
-  CK(h, cudaMemcpyAsync(al, al0, al_plane * ns, cudaMemcpyDeviceToDevice, h->stream));
-  return EGS_OK;
-}
-
-static int copy_rows(egs_handle *h, bool save) {
-  Checkpoint &k = h->ck;
-  const size_t rows = (size_t)h->n_pad * h->row_w * sizeof(int32_t), totals = (size_t)h->n_pad * sizeof(int32_t);
-  CK(h, cudaMemcpyAsync(save ? k.d_core : h->d_core, save ? h->d_core : k.d_core, rows, cudaMemcpyDeviceToDevice, h->stream));
-  CK(h, cudaMemcpyAsync(save ? k.d_mem : h->d_mem, save ? h->d_mem : k.d_mem, rows, cudaMemcpyDeviceToDevice, h->stream));
-  CK(h, cudaMemcpyAsync(save ? k.d_mem_total : h->d_mem_total, save ? h->d_mem_total : k.d_mem_total, totals,
-                        cudaMemcpyDeviceToDevice, h->stream));
   return EGS_OK;
 }
 
 extern "C" int egs_checkpoint_save(egs_handle *h) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  TRY(flush_pending(h));                          // batches still pending belong to the saved state
+  TRY(settle_pending(h, true));                   // batches still pending belong to the saved state
   Checkpoint &k = h->ck;
   k.open = false;                                 // an earlier checkpoint is overwritten from here on
   h->book.drop_checkpoint();
   const int ns = (int)h->shapes.size();
-  const size_t np = (size_t)h->n_pad, rows = np * h->row_w * sizeof(int32_t);
-  if (!k.d_core) {
-    CK(h, cudaMalloc(&k.d_core, rows));
-    CK(h, cudaMalloc(&k.d_mem, rows));
-    CK(h, cudaMalloc(&k.d_mem_total, np * sizeof(int32_t)));
-  }
-  if (ns > k.slot_cap) {
-    CK(h, cudaStreamSynchronize(h->stream));      // the previous save may still copy into the old buffers
-    if (k.d_st) { cudaFree(k.d_st); cudaFree(k.d_sc); cudaFree(k.d_al); k.d_st = nullptr; k.d_sc = nullptr; k.d_al = nullptr; }
-    k.slot_cap = 0;
-    const int cap = std::max(ns, h->slot_cap);
-    CK(h, cudaMalloc(&k.d_st, np * cap));
-    CK(h, cudaMalloc(&k.d_sc, np * cap * sizeof(int32_t)));
-    CK(h, cudaMalloc(&k.d_al, np * EGS_C * h->mask_b * cap));
-    k.slot_cap = cap;
-  }
-  TRY(copy_rows(h, true));
-  TRY(copy_tables(h, ns, true));
+  if (ns > k.tables.slots) TRY(k.tables.grow(h, std::max(ns, h->tables.slots)));
+  TRY(k.rows.save(h));
+  TRY(k.tables.copy_from(h, h->tables, ns));
   k.n_shapes = ns;
-  k.gpu_count = h->h_gpu_count; k.mem_total = h->h_mem_total;
   k.slot_cold = h->slot_cold;
   k.shape_cache = h->shape_cache;
   k.next_uid = h->next_uid;
@@ -565,17 +517,16 @@ extern "C" int egs_checkpoint_rollback(egs_handle *h) {
   Guard g(h);
   Checkpoint &k = h->ck;
   if (!k.open) return fail(h, EGS_ERR_BAD_ARG, "no checkpoint: egs_checkpoint_save first");
-  TRY(discard_pending(h));                        // batches after the save whose results never reached the book
+  TRY(settle_pending(h, false));                  // batches after the save whose results never reached the book
   const int ns = (int)h->shapes.size();
-  TRY(copy_rows(h, false));
-  TRY(copy_tables(h, k.n_shapes, false));         // the tables may have been reallocated since: slot offsets hold
+  TRY(k.rows.load(h));
+  TRY(h->tables.copy_from(h, k.tables, k.n_shapes));   // the tables may have been reallocated since: slot offsets hold
   if (ns > k.n_shapes)                            // slots interned since the save read OPT_ABSENT again
-    CK(h, cudaMemsetAsync(h->d_st + (size_t)k.n_shapes * h->n_pad, OPT_ABSENT, (size_t)(ns - k.n_shapes) * h->n_pad, h->stream));
+    CK(h, cudaMemsetAsync(h->tables.st + (size_t)k.n_shapes * h->n_pad, OPT_ABSENT, (size_t)(ns - k.n_shapes) * h->n_pad, h->stream));
   for (int s = k.n_shapes; s < ns; s++) h->shape_ids.erase(shape_key(h->shapes[s].C, h->shapes[s].u));
   h->shapes.resize((size_t)k.n_shapes);
   h->slot_cold = k.slot_cold;
   h->shape_cache = k.shape_cache;
-  h->h_gpu_count = k.gpu_count; h->h_mem_total = k.mem_total;
   h->next_uid = k.next_uid;
   h->book.rollback();
   return EGS_OK;
@@ -589,18 +540,6 @@ extern "C" int egs_checkpoint_drop(egs_handle *h) {
 }
 
 // ------------------------------------------------------------------------------- verbs
-static int ensure_gather(egs_handle *h, size_t n) {
-  if (n <= h->gather_cap) return EGS_OK;
-  if (h->d_ids) { cudaFree(h->d_ids); cudaFree(h->d_fit); cudaFree(h->d_score); }
-  h->d_ids = nullptr; h->gather_cap = 0;
-  size_t cap = std::max(n, (size_t)4096);
-  CK(h, cudaMalloc(&h->d_ids, cap * sizeof(int32_t)));
-  CK(h, cudaMalloc(&h->d_fit, cap));
-  CK(h, cudaMalloc(&h->d_score, cap * sizeof(int32_t)));
-  h->gather_cap = cap;
-  return EGS_OK;
-}
-
 static int gather(egs_handle *h, bool score, int n, const int32_t *node_ids, int C, const egs_unit *units,
                   uint8_t *out_fit, int32_t *out_score) {
   if (n < 0 || (n > 0 && !(score ? (void *)out_score : (void *)out_fit))) return EGS_ERR_BAD_ARG;
@@ -608,7 +547,10 @@ static int gather(egs_handle *h, bool score, int n, const int32_t *node_ids, int
   TRY(intern(h, C, units, &slot));
   if (n == 0) return EGS_OK;
   h->slot_cold[slot] = 0;
-  TRY(ensure_gather(h, (size_t)n));
+  if ((size_t)n > h->d_ids.cap()) {
+    const size_t cap = std::max((size_t)n, (size_t)4096);
+    CK(h, grow(h->stream, false, to(h->d_ids, cap), to(h->d_fit, cap), to(h->d_score, cap)));
+  }
   TRY(ensure_stage(h, (size_t)n * sizeof(int32_t)));
   GatherArgs a;
   a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total;
@@ -664,15 +606,14 @@ extern "C" int egs_score(egs_handle *h, int n, const int32_t *node_ids, int n_co
 // res[0] had entry, res[1] status, res[2] score; *masks the option's packed masks
 static int bind_or_peek(egs_handle *h, int consume, int node_id, int C, const egs_unit *units, uint64_t uid,
                         int32_t *res, uint64_t *masks) {
-  if (node_id < 0 || node_id >= h->max_nodes) return EGS_ERR_BAD_ARG;
-  if (h->h_gpu_count[node_id] == 0) return EGS_ERR_NO_NODE;
+  TRY(check_node(h, node_id));
   int slot;
   TRY(intern(h, C, units, &slot));
-  TRY(flush_pending(h));
+  TRY(settle_pending(h, true));
   BindArgs a;
   a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total; a.node = node_id;
   a.req = make_req(C, units); a.t = table(h, slot);
-  a.all_st = h->d_st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
+  a.all_st = h->tables.st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
   const bool known = consume && h->book.in_pods_map(node_id, uid);
   a.skip_transact = known ? 1 : 0; a.consume = consume; a.result = h->d_result;
   by_width(h, [&](auto W) -> int {
@@ -724,7 +665,7 @@ extern "C" int egs_option_dump(egs_handle *h, int n_containers, const egs_unit *
   const size_t sn = (size_t)n, mb = (size_t)h->mask_b;
   TRY(ensure_stage(h, sn * (1 + 4 + EGS_C * mb)));
   CK(h, cudaStreamSynchronize(h->stream));
-  char *s = (char *)h->h_stage;
+  char *s = h->h_stage.get();
   int32_t *hs = (int32_t *)s; uint8_t *hst = (uint8_t *)(hs + sn); uint8_t *hal = hst + sn;
   CK(h, cudaMemcpyAsync(hs, t.sc + node0, 4 * sn, cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaMemcpyAsync(hst, t.st + node0, sn, cudaMemcpyDeviceToHost, h->stream));
@@ -750,7 +691,7 @@ static int apply_lists(egs_handle *h, int cancel, int node_id, int C, const egs_
     ApplyArgs<G> a; memset(&a, 0, sizeof a);
     a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total;
     a.op.node = node_id; a.op.cancel = cancel; a.op.req = make_req<ReqW>(C, units);
-    a.all_st = h->d_st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
+    a.all_st = h->tables.st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
     for (int c = 0; c < C; c++) {
       int n = alloc_off ? alloc_off[c + 1] - alloc_off[c] : 0;
       if (n < 0 || n > G || (n > 0 && !alloc_idx)) return EGS_ERR_BAD_ARG;
@@ -772,10 +713,9 @@ extern "C" int egs_pod_apply(egs_handle *h, int node_id, int n_containers, const
                              const int32_t *alloc_off, const int32_t *alloc_idx, uint64_t uid) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  if (node_id < 0 || node_id >= h->max_nodes) return EGS_ERR_BAD_ARG;
-  if (h->h_gpu_count[node_id] == 0) return EGS_ERR_NO_NODE;
+  TRY(check_node(h, node_id));
   TRY(check_units(n_containers, units, EGS_MAX_CONTAINERS_APPLY));
-  TRY(flush_pending(h));
+  TRY(settle_pending(h, true));
   return h->book.account(EGS_MUT_ADD, node_id, uid,
                          [&](int cancel) { return apply_lists(h, cancel, node_id, n_containers, units, alloc_off, alloc_idx); });
 }
@@ -785,10 +725,9 @@ extern "C" int egs_node_replay_pod(egs_handle *h, int node_id, int n_containers,
                                    const int32_t *alloc_off, const int32_t *alloc_idx, uint64_t uid) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  if (node_id < 0 || node_id >= h->max_nodes) return EGS_ERR_BAD_ARG;
-  if (h->h_gpu_count[node_id] == 0) return EGS_ERR_NO_NODE;
+  TRY(check_node(h, node_id));
   TRY(check_units(n_containers, units, EGS_MAX_CONTAINERS_APPLY));
-  TRY(flush_pending(h));
+  TRY(settle_pending(h, true));
   return h->book.account(EGS_MUT_REPLAY, node_id, uid,
                          [&](int cancel) { return apply_lists(h, cancel, node_id, n_containers, units, alloc_off, alloc_idx); });
 }
@@ -798,10 +737,9 @@ extern "C" int egs_pod_cancel(egs_handle *h, int node_id, int n_containers, cons
                               const int32_t *alloc_off, const int32_t *alloc_idx, uint64_t uid) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  TRY(flush_pending(h));
+  TRY(settle_pending(h, true));
   if (node_id >= 0) {
-    if (node_id >= h->max_nodes) return EGS_ERR_BAD_ARG;
-    if (h->h_gpu_count[node_id] == 0) return EGS_ERR_NO_NODE;
+    TRY(check_node(h, node_id));
     TRY(check_units(n_containers, units, EGS_MAX_CONTAINERS_APPLY));
   }
   return h->book.account(EGS_MUT_FORGET, node_id, uid,
@@ -819,8 +757,7 @@ static int mutations_apply_locked(egs_handle *h, int n, const egs_mutation *ops)
     const egs_mutation &m = ops[i];
     if (m.kind < EGS_MUT_ADD || m.kind > EGS_MUT_REPLAY) return EGS_ERR_BAD_ARG;
     if (m.node_id < 0) { if (m.kind != EGS_MUT_FORGET) return EGS_ERR_BAD_ARG; continue; }
-    if (m.node_id >= h->max_nodes) return EGS_ERR_BAD_ARG;
-    if (h->h_gpu_count[m.node_id] == 0) return EGS_ERR_NO_NODE;
+    TRY(check_node(h, m.node_id));
     TRY(check_units(m.n_containers, m.units, EGS_MAX_CONTAINERS_APPLY));
     for (int c = 0; c < m.n_containers; c++) {
       if (m.n_idx[c] < 0 || m.n_idx[c] > EGS_MAX_GPUS) return fail(h, EGS_ERR_BAD_ARG, "a mutation record holds at most EGS_MAX_GPUS indices per container");
@@ -854,25 +791,22 @@ static int mutations_rows(egs_handle *h, int n, const egs_mutation *ops) {
   const size_t nd = dev.size();
   TRY(ensure_stage(h, nd * sizeof(Op) + (nd + 1) * sizeof(int32_t)));
   CK(h, cudaStreamSynchronize(h->stream));
-  Op *so = (Op *)h->h_stage; int32_t *sg = (int32_t *)(so + nd);
+  Op *so = (Op *)h->h_stage.get(); int32_t *sg = (int32_t *)(so + nd);
   int ng = 0;
   for (size_t i = 0; i < nd; i++) {
     so[i] = dev[order[i]];
     if (i == 0 || so[i].node != so[i - 1].node) sg[ng++] = (int32_t)i;
   }
   sg[ng] = (int32_t)nd;
-  if (nd > h->ops_cap) {
-    if (h->d_ops) { cudaFree(h->d_ops); cudaFree(h->d_group_off); h->d_ops = nullptr; h->d_group_off = nullptr; h->ops_cap = 0; }
+  if (nd * sizeof(Op) > h->d_ops.cap()) {
     const size_t cap = std::max(nd, (size_t)1024);
-    CK(h, cudaMalloc(&h->d_ops, cap * sizeof(Op)));
-    CK(h, cudaMalloc(&h->d_group_off, (cap + 1) * sizeof(int32_t)));
-    h->ops_cap = cap;
+    CK(h, grow(h->stream, false, to(h->d_ops, cap * sizeof(Op)), to(h->d_group_off, cap + 1)));
   }
   CK(h, cudaMemcpyAsync(h->d_ops, so, nd * sizeof(Op), cudaMemcpyHostToDevice, h->stream));
   CK(h, cudaMemcpyAsync(h->d_group_off, sg, (size_t)(ng + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
   ApplyManyArgs<G> ka;
-  ka.core = h->d_core; ka.mem = h->d_mem; ka.mem_total = h->d_mem_total; ka.ops = (const Op *)h->d_ops; ka.group_off = h->d_group_off; ka.n_groups = ng;
-  ka.all_st = h->d_st; ka.slot_stride = (size_t)h->n_pad; ka.n_slots = (int)h->shapes.size();
+  ka.core = h->d_core; ka.mem = h->d_mem; ka.mem_total = h->d_mem_total; ka.ops = (const Op *)h->d_ops.get(); ka.group_off = h->d_group_off; ka.n_groups = ng;
+  ka.all_st = h->tables.st; ka.slot_stride = (size_t)h->n_pad; ka.n_slots = (int)h->shapes.size();
   k_apply_many<G><<<(ng + 127) / 128, 128, 0, h->stream>>>(ka);
   CK(h, cudaGetLastError());
   return EGS_OK;
@@ -881,14 +815,14 @@ static int mutations_rows(egs_handle *h, int n, const egs_mutation *ops) {
 extern "C" int egs_mutations_apply(egs_handle *h, int n, const egs_mutation *ops) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  TRY(flush_pending(h));
+  TRY(settle_pending(h, true));
   return mutations_apply_locked(h, n, ops);
 }
 
 extern "C" int egs_pod_known(egs_handle *h, uint64_t uid) {
   if (!h) return 0;
   Guard g(h);
-  if (flush_pending(h) != EGS_OK) return 0;
+  if (settle_pending(h, true) != EGS_OK) return 0;
   return h->book.in_pod_maps(uid) ? 1 : 0;
 }
 extern "C" int egs_pod_released(egs_handle *h, uint64_t uid) {
@@ -899,18 +833,10 @@ extern "C" int egs_pod_released(egs_handle *h, uint64_t uid) {
 
 // ------------------------------------------------------------------------------- batch loop
 static int ensure_out(egs_handle *h, int P) {
-  if (P <= h->out_cap) return EGS_OK;
-  void *old[] = {h->d_o_node, h->d_o_status, h->d_o_fit, h->d_o_alloc, h->d_o_fd, h->d_o_sd};
-  for (void *p : old) if (p) cudaFree(p);
-  h->out_cap = 0;
-  int cap = std::max(P, 1024);
-  CK(h, cudaMalloc(&h->d_o_node, sizeof(int32_t) * (size_t)cap));
-  CK(h, cudaMalloc(&h->d_o_status, sizeof(int32_t) * (size_t)cap));
-  CK(h, cudaMalloc(&h->d_o_fit, sizeof(int32_t) * (size_t)cap));
-  CK(h, cudaMalloc(&h->d_o_alloc, (size_t)cap * EGS_C * h->mask_b));
-  CK(h, cudaMalloc(&h->d_o_fd, sizeof(unsigned long long) * (size_t)cap));
-  CK(h, cudaMalloc(&h->d_o_sd, sizeof(unsigned long long) * (size_t)cap));
-  h->out_cap = cap;
+  if ((size_t)P <= h->d_o_node.cap()) return EGS_OK;
+  const size_t cap = (size_t)std::max(P, 1024);
+  CK(h, grow(h->stream, false, to(h->d_o_node, cap), to(h->d_o_status, cap), to(h->d_o_fit, cap),
+             to(h->d_o_alloc, cap * EGS_C * h->mask_b), to(h->d_o_fd, cap), to(h->d_o_sd, cap)));
   return EGS_OK;
 }
 
@@ -925,7 +851,7 @@ static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_un
     PassArgs a;
     a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total; a.core_w = h->d_core; a.mem_w = h->d_mem;
     a.n = h->max_nodes; a.policy = h->policy; a.req = make_req(C, u); a.t = table(h, slots[p]);
-    a.all_st = h->d_st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
+    a.all_st = h->tables.st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
     a.vec_fit = p < h->vec_pods ? h->d_vec_fit + (size_t)p * h->max_nodes : nullptr;
     a.vec_score = p < h->vec_pods ? h->d_vec_score + (size_t)p * h->max_nodes : nullptr;
     a.partials = h->d_partials; a.ticket = h->d_ticket;
@@ -962,7 +888,7 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
     TRY(intern(h, C, units + c_off[p], &slots[p]));
   }
   if (uids) {                                    // pods awaiting scheduling must be unknown and distinct
-    TRY(flush_pending(h));
+    TRY(settle_pending(h, true));
     std::unordered_set<uint64_t> seen; seen.reserve((size_t)P * 2);
     for (int p = 0; p < P; p++) {
       if (!seen.insert(uids[p]).second || h->book.in_pod_maps(uids[p])) return fail(h, EGS_ERR_BAD_ARG, "duplicate or known uid");
@@ -981,7 +907,7 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
   if (mode == EGS_MODE_AUTO) mode = is_wide(h) ? EGS_MODE_RESCAN : EGS_MODE_ROUNDS;
   int batch_rc = EGS_OK, n_done = P;
   if (mode == EGS_MODE_RESCAN) TRY(batch_rescan(h, P, c_off, units, slots, dev));
-  else if (mode == EGS_MODE_ROUNDS) batch_rc = batch_rounds(h, P, c_off, units, slots, dev, &n_done);
+  else if (mode == EGS_MODE_ROUNDS) batch_rc = batch_rounds(h, P, slots, dev, &n_done);
   else return EGS_ERR_BAD_ARG;
 
   // lazy uid bookkeeping: async copy of (node, status), applied on the next uid-dependent verb.  A batch that
@@ -990,7 +916,7 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
     PendingBatch pb; pb.n = n_done; pb.uid0 = h->next_uid;
     if (uids) pb.uids.assign(uids, uids + n_done); else h->next_uid += (uint64_t)n_done;
     TRY(pin_get(h, 2 * (size_t)n_done, &pb.buf));
-    pb.h_node = pb.buf.p; pb.h_status = pb.buf.p + n_done;
+    pb.h_node = pb.buf; pb.h_status = pb.buf + n_done;
     CK(h, cudaMemcpyAsync(pb.h_node, dev.node, sizeof(int32_t) * (size_t)n_done, cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaMemcpyAsync(pb.h_status, dev.status, sizeof(int32_t) * (size_t)n_done, cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaEventCreateWithFlags(&pb.done, cudaEventDisableTiming));
@@ -1003,7 +929,7 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
     size_t sp = (size_t)P;
     const size_t ab = (size_t)EGS_C * h->mask_b;   // alloc bytes per pod
     TRY(ensure_stage(h, sp * (4 + 4 + 4 + ab + 8 + 8)));
-    char *s = (char *)h->h_stage;
+    char *s = h->h_stage.get();
     int32_t *hn = (int32_t *)s, *hs = hn + sp, *hf = hs + sp;
     unsigned long long *hfd = (unsigned long long *)(hf + sp), *hsd = hfd + sp;
     uint8_t *ha = (uint8_t *)(hsd + sp);
@@ -1026,14 +952,24 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
   return EGS_OK;
 }
 
+// The caller's six per-pod outputs from pod p on; each may be null.
+static PodOut pod_out(const egs_handle *h, int32_t *node, int32_t *status, uint8_t *alloc, int32_t *fit_count,
+                      uint64_t *fit_digest, uint64_t *score_digest, int p = 0) {
+  PodOut o;
+  o.node = node ? node + p : nullptr; o.status = status ? status + p : nullptr;
+  o.alloc = alloc ? alloc + (size_t)p * EGS_C * h->mask_b : nullptr; o.fit_count = fit_count ? fit_count + p : nullptr;
+  o.fit_digest = fit_digest ? (unsigned long long *)fit_digest + p : nullptr;
+  o.score_digest = score_digest ? (unsigned long long *)score_digest + p : nullptr;
+  return o;
+}
+
 extern "C" int egs_schedule_batch(egs_handle *h, int mode, int n_pods, const int32_t *c_off, const egs_unit *units,
                                   const uint64_t *uids, int32_t *out_node, int32_t *out_status,
                                   uint8_t *out_alloc_mask, int32_t *out_fit_count, uint64_t *out_fit_digest,
                                   uint64_t *out_score_digest) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  PodOut o; o.node = out_node; o.status = out_status; o.alloc = out_alloc_mask; o.fit_count = out_fit_count;
-  o.fit_digest = (unsigned long long *)out_fit_digest; o.score_digest = (unsigned long long *)out_score_digest;
+  const PodOut o = pod_out(h, out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest);
   return batch_common(h, mode, n_pods, c_off, units, uids, o, false);
 }
 
@@ -1052,17 +988,13 @@ extern "C" int egs_schedule_batch_mut(egs_handle *h, int mode, int n_pods, const
     int j1 = j;
     while (j1 < n_mut && mut_at[j1] == p) j1++;
     if (j1 > j) {
-      TRY(flush_pending(h));
+      TRY(settle_pending(h, true));
       TRY(mutations_apply_locked(h, j1 - j, muts + j));
       j = j1;
     }
     if (p >= n_pods) break;
     const int q = j < n_mut ? mut_at[j] : n_pods;                // next mutation point (> p)
-    PodOut o;
-    o.node = out_node ? out_node + p : nullptr; o.status = out_status ? out_status + p : nullptr;
-    o.alloc = out_alloc_mask ? out_alloc_mask + (size_t)p * EGS_C * h->mask_b : nullptr; o.fit_count = out_fit_count ? out_fit_count + p : nullptr;
-    o.fit_digest = out_fit_digest ? (unsigned long long *)out_fit_digest + p : nullptr;
-    o.score_digest = out_score_digest ? (unsigned long long *)out_score_digest + p : nullptr;
+    const PodOut o = pod_out(h, out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest, p);
     // the segment's pods as a batch of its own: offsets rebased
     std::vector<int32_t> off((size_t)(q - p) + 1);
     for (int i = p; i <= q; i++) off[(size_t)(i - p)] = c_off[i] - c_off[p];
@@ -1081,14 +1013,8 @@ extern "C" int egs_schedule_batch_vec(egs_handle *h, int n_pods, const int32_t *
   if (h->world > 1) return fail(h, EGS_ERR_BAD_ARG, "egs_schedule_batch_vec is single-shard");
   vec_pods = std::min(vec_pods, n_pods);
   const size_t cells = (size_t)vec_pods * h->max_nodes;
-  if (cells > h->vec_cap) {
-    if (h->d_vec_fit) { cudaFree(h->d_vec_fit); cudaFree(h->d_vec_score); h->d_vec_fit = nullptr; h->d_vec_score = nullptr; h->vec_cap = 0; }
-    CK(h, cudaMalloc(&h->d_vec_fit, cells));
-    CK(h, cudaMalloc(&h->d_vec_score, cells * sizeof(int32_t)));
-    h->vec_cap = cells;
-  }
-  PodOut o; o.node = out_node; o.status = out_status; o.alloc = out_alloc_mask; o.fit_count = out_fit_count;
-  o.fit_digest = (unsigned long long *)out_fit_digest; o.score_digest = (unsigned long long *)out_score_digest;
+  if (cells > h->d_vec_fit.cap()) CK(h, grow(h->stream, false, to(h->d_vec_fit, cells), to(h->d_vec_score, cells)));
+  const PodOut o = pod_out(h, out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest);
   h->vec_pods = vec_pods;
   const int rc = batch_common(h, EGS_MODE_RESCAN, n_pods, c_off, units, uids, o, false);
   h->vec_pods = 0;
@@ -1108,8 +1034,7 @@ extern "C" int egs_schedule_batch_device(egs_handle *h, int mode, int n_pods, co
   Guard g(h);
   if ((uintptr_t)d_out_alloc_mask % ((uintptr_t)EGS_C * h->mask_b))     // one packed word per pod (write_pod_out)
     return fail(h, EGS_ERR_BAD_ARG, "d_out_alloc_mask must be aligned to EGS_MAX_CONTAINERS * EGS_MASK_BYTES(g_max)");
-  PodOut o; o.node = d_out_node; o.status = d_out_status; o.alloc = d_out_alloc_mask; o.fit_count = d_out_fit_count;
-  o.fit_digest = (unsigned long long *)d_out_fit_digest; o.score_digest = (unsigned long long *)d_out_score_digest;
+  const PodOut o = pod_out(h, d_out_node, d_out_status, d_out_alloc_mask, d_out_fit_count, d_out_fit_digest, d_out_score_digest);
   return batch_common(h, mode, n_pods, h_c_off, h_units, nullptr, o, true);
 }
 
@@ -1146,13 +1071,9 @@ extern "C" int egs_profile_evaluate(egs_handle *h, int n_containers, const egs_u
   Guard g(h);
   TRY(check_units(n_containers, units));
   const size_t np = (size_t)h->n_pad;
-  if (!h->d_ev_fit) {
-    CK(h, cudaMalloc(&h->d_ev_fit, np));
-    CK(h, cudaMalloc(&h->d_ev_score, np * sizeof(int32_t)));
-    CK(h, cudaMalloc(&h->d_ev_gpu, np * EGS_C * h->mask_b));
-  }
+  if (!h->d_ev_fit) CK(h, grow(h->stream, false, to(h->d_ev_fit, np), to(h->d_ev_score, np), to(h->d_ev_gpu, np * EGS_C * h->mask_b)));
   const size_t flush_bytes = (size_t)256 << 20;
-  if (flush_l2 && !h->d_flush) CK(h, cudaMalloc(&h->d_flush, flush_bytes));
+  if (flush_l2 && !h->d_flush) CK(h, grow(h->stream, false, to(h->d_flush, flush_bytes)));
   EvalArgs a;
   a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total; a.lo = 0; a.n = h->max_nodes; a.policy = h->policy;
   a.req = make_req(n_containers, units); a.fit = h->d_ev_fit; a.score = h->d_ev_score; a.gpu = h->d_ev_gpu; a.plane = np;

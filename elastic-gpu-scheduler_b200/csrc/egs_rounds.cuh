@@ -33,6 +33,7 @@
 #include <memory>
 #include <mutex>
 #include <vector>
+#include "buffers.h"
 #include "egs_kernels.cuh"
 
 #define OPT_NEW 3
@@ -1355,20 +1356,19 @@ struct RoundsState {
   cudaEvent_t ev_ready = nullptr, ev_copied = nullptr;   // own buffer written / peers' buffers copied
   bool copied = false;              // in-process group: a round ran since egs_comm_init_local, so every peer's
                                     // ev_copied marks its last copy of this rank's buffer (kept across batches)
-  uint8_t *d_pod_sidx = nullptr; int pod_cap = 0;
-  uint8_t *d_obs = nullptr; int obs_cap = 0;
-  unsigned long long *d_cta_lists = nullptr; AggPart *d_cta_agg = nullptr; int grid = 0, cta_nsc = 0;
-  char *d_bufs = nullptr; size_t bufs_cap = 0;      // [RD] candidate buffers; own shard written at index `rank`
-  RoundDesc *d_rd = nullptr; RoundDesc *h_rd = nullptr;
-  RoundCtl *d_ctl = nullptr; RoundCtl *h_ctl = nullptr;
+  DeviceBuf<uint8_t> d_pod_sidx;
+  DeviceBuf<uint8_t> d_obs;
+  DeviceBuf<unsigned long long> d_cta_lists; DeviceBuf<AggPart> d_cta_agg; int grid = 0, cta_nsc = 0;
+  DeviceBuf<char> d_bufs;                           // [RD] candidate buffers; own shard written at index `rank`
+  DeviceBuf<RoundDesc> d_rd; PinnedBuf<RoundDesc> h_rd;
+  DeviceBuf<RoundCtl> d_ctl; PinnedBuf<RoundCtl> h_ctl;
   int64_t rounds = 0, pods = 0, tracked = 0; int64_t stops[4] = {0, 0, 0, 0};
   long long prof[RPROF] = {0};
 };
 
 static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_unit *units,
                         const std::vector<int> &slots, PodOut out);
-static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_unit *units,
-                        const std::vector<int> &slots, PodOut out, int *n_done);
+static int batch_rounds(egs_handle *h, int P, const std::vector<int> &slots, PodOut out, int *n_done);
 static void rounds_free(RoundsState *r);
 static int rounds_comm_unique_id(uint8_t out_id[128]);
 static int rounds_comm_init(egs_handle *h, const uint8_t id[128]);

@@ -40,15 +40,11 @@ static NcclApi *nccl_api() {
     }                                                                                    \
   } while (0)
 
+// The NCCL comm and the events; the buffers go with the handle.
 static void rounds_free(RoundsState *r) {
   if (r->comm && nccl_api()) nccl_api()->CommDestroy((ncclComm_t)r->comm);
-  void *dev[] = {r->d_pod_sidx, r->d_obs, r->d_cta_lists, r->d_cta_agg, r->d_bufs, r->d_rd, r->d_ctl};
-  for (void *p : dev) if (p) cudaFree(p);
   if (r->ev_ready) cudaEventDestroy(r->ev_ready);
   if (r->ev_copied) cudaEventDestroy(r->ev_copied);
-  if (r->h_rd) cudaFreeHost(r->h_rd);
-  if (r->h_ctl) cudaFreeHost(r->h_ctl);
-  *r = RoundsState();
 }
 
 static int rounds_comm_unique_id(uint8_t out_id[128]) {
@@ -104,56 +100,34 @@ static int select_grid(const egs_handle *h) {
 static int rounds_ensure(egs_handle *h, int P, const BufLayout &L) {
   RoundsState &R = h->rounds;
   if (!R.d_ctl) {
-    CK(h, cudaMalloc(&R.d_ctl, sizeof(RoundCtl)));
-    CK(h, cudaMallocHost(&R.h_ctl, sizeof(RoundCtl)));
-    CK(h, cudaMalloc(&R.d_rd, sizeof(RoundDesc)));
-    CK(h, cudaMallocHost(&R.h_rd, sizeof(RoundDesc)));
+    CK(h, grow(h->stream, false, to(R.d_ctl, 1), to(R.h_ctl, 1), to(R.d_rd, 1), to(R.h_rd, 1)));
     for (int ns : {MwInst16::NS, MwInst32::NS, MwInst96::NS})
       CK(h, mw_dispatch(ns, [](auto i) {
         return cudaFuncSetAttribute(k_resolve_mw<decltype(i)>, cudaFuncAttributeMaxDynamicSharedMemorySize, MW_SMEM_MAX);
       }));
   }
   const size_t need = (size_t)L.bytes * RD;
-  if (need > R.bufs_cap) {
-    if (R.d_bufs) { CK(h, cudaStreamSynchronize(h->stream)); cudaFree(R.d_bufs); R.d_bufs = nullptr; R.bufs_cap = 0; }
-    CK(h, cudaMalloc(&R.d_bufs, need));
+  if (need > R.d_bufs.cap()) {
+    CK(h, grow(h->stream, false, to(R.d_bufs, need)));
     CK(h, cudaMemsetAsync(R.d_bufs, 0, need, h->stream));
-    R.bufs_cap = need;
   }
   const int grid = select_grid(h);
   if (grid > R.grid || L.nsc > R.cta_nsc) {
-    if (R.d_cta_lists) { CK(h, cudaStreamSynchronize(h->stream)); cudaFree(R.d_cta_lists); cudaFree(R.d_cta_agg); R.d_cta_lists = nullptr; }
     const int g = std::max(grid, R.grid), n = std::max(L.nsc, R.cta_nsc);
-    CK(h, cudaMalloc(&R.d_cta_lists, sizeof(unsigned long long) * (size_t)g * n * RK));
-    CK(h, cudaMalloc(&R.d_cta_agg, sizeof(AggPart) * (size_t)g * n));
+    CK(h, grow(h->stream, false, to(R.d_cta_lists, (size_t)g * n * RK), to(R.d_cta_agg, (size_t)g * n)));
     R.grid = g; R.cta_nsc = n;
   }
-  if (P + 8 > R.pod_cap) {
-    if (R.d_pod_sidx) { CK(h, cudaStreamSynchronize(h->stream)); cudaFree(R.d_pod_sidx); }
-    R.pod_cap = 0;
-    CK(h, cudaMalloc(&R.d_pod_sidx, (size_t)P + 8));
-    R.pod_cap = P + 8;
-  }
-  const int ns = (int)h->shapes.size();
-  if (ns > R.obs_cap) {
-    const int cap = std::max(ns, 4096);
-    uint8_t *n;
-    CK(h, cudaMalloc(&n, (size_t)cap));
-    CK(h, cudaMemsetAsync(n, 0, (size_t)cap, h->stream));
-    if (R.d_obs) {
-      CK(h, cudaMemcpyAsync(n, R.d_obs, (size_t)R.obs_cap, cudaMemcpyDeviceToDevice, h->stream));
-      CK(h, cudaStreamSynchronize(h->stream));
-      cudaFree(R.d_obs);
-    }
-    R.d_obs = n; R.obs_cap = cap;
+  if ((size_t)P + 8 > R.d_pod_sidx.cap()) CK(h, grow(h->stream, false, to(R.d_pod_sidx, (size_t)P + 8)));
+  const size_t ns = h->shapes.size(), old = R.d_obs.cap();
+  if (ns > old) {                                               // the flags of the slots held so far are kept
+    CK(h, grow(h->stream, true, to(R.d_obs, std::max(ns, (size_t)4096))));
+    CK(h, cudaMemsetAsync(R.d_obs + old, 0, R.d_obs.cap() - old, h->stream));
   }
   return EGS_OK;
 }
 
 // Runs the batch; *n_done = pods resolved (== P unless an error stopped the loop).
-static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_unit *units,
-                        const std::vector<int> &slots, PodOut out, int *n_done) {
-  (void)c_off; (void)units;
+static int batch_rounds(egs_handle *h, int P, const std::vector<int> &slots, PodOut out, int *n_done) {
   RoundsState &R = h->rounds;
   *n_done = 0;
   if (h->world > 1 && !R.comm && !R.local) return fail(h, EGS_ERR_COMM, "sharded handle without egs_comm_init");
@@ -183,7 +157,7 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
   TRY(wait_peers_copied());
   TRY(rounds_ensure(h, P, L));
 
-  TableSet tb; tb.st = h->d_st; tb.sc = h->d_sc; tb.al = h->d_al; tb.n_pad = (size_t)h->n_pad; tb.n_slots = (int)h->shapes.size();
+  TableSet tb; tb.st = h->tables.st; tb.sc = h->tables.sc; tb.al = h->tables.al; tb.n_pad = (size_t)h->n_pad; tb.n_slots = (int)h->shapes.size();
   const int grid = select_grid(h);
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   if (h->timing) for (auto &e : ev) CK(h, cudaEventCreate(&e));
@@ -282,7 +256,7 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
   // staging: pod -> shape index, round descriptor, control block
   TRY(ensure_stage(h, (size_t)P + 8));
   CK(h, cudaStreamSynchronize(h->stream));
-  uint8_t *h_sidx = (uint8_t *)h->h_stage;
+  uint8_t *h_sidx = (uint8_t *)h->h_stage.get();
   RoundCtl ctl0; memset(&ctl0, 0, sizeof ctl0);
   std::vector<int> set_idx(h->shapes.size(), -1);
   int rc = EGS_OK;
@@ -366,7 +340,8 @@ static int batch_rounds(egs_handle *h, int P, const int32_t *c_off, const egs_un
   // no OPT_NEW may outlive the batch -- also after an error, so that the handle stays consistent
   const int n = h->hi - h->lo;
   if (n > 0) k_rounds_finalize<<<(n + 255) / 256, 256, 0, h->stream>>>(tb, R.d_obs, h->lo, h->hi);   // a shard may be empty
-  k_clear_u8<<<(R.obs_cap + 255) / 256, 256, 0, h->stream>>>(R.d_obs, R.obs_cap);
+  const int n_obs = (int)R.d_obs.cap();
+  k_clear_u8<<<(n_obs + 255) / 256, 256, 0, h->stream>>>(R.d_obs, n_obs);
   if (rc != EGS_OK) return rc;
   CK(h, cudaGetLastError());
   return EGS_OK;
