@@ -30,9 +30,14 @@ def mask_dtype(g_max: int):
     """One GPU mask of a handle created with `g_max` (EGS_MASK_BYTES little-endian bytes)."""
     return np.dtype("<u2") if g_max > EGS_MAX_GPUS else np.dtype(np.uint8)
 
+
+def masks_per_pod(c_max: int) -> int:
+    """EGS_MASKS_PER_POD: GPU masks per pod / node of a handle created for pods of up to `c_max` containers."""
+    return 8 if c_max > EGS_MAX_CONTAINERS else EGS_MAX_CONTAINERS
+
 # every symbol include/egs.h declares
 SYMBOLS = [
-    "egs_create", "egs_destroy", "egs_last_error", "egs_status_string", "egs_unit_from_requests",
+    "egs_create", "egs_create_ex", "egs_destroy", "egs_last_error", "egs_status_string", "egs_unit_from_requests",
     "egs_node_set_allocatable", "egs_node_set", "egs_state_load", "egs_state_load_bulk", "egs_state_dump",
     "egs_state_snapshot", "egs_state_restore", "egs_checkpoint_save", "egs_checkpoint_rollback", "egs_checkpoint_drop",
     "egs_filter", "egs_score", "egs_bind", "egs_option_peek", "egs_option_dump", "egs_pod_apply", "egs_node_replay_pod", "egs_pod_cancel",
@@ -68,6 +73,7 @@ def load(build: bool = True):
     L = C.CDLL(path)
     vp, i32, i64, u64 = C.c_void_p, C.c_int, C.c_int64, C.c_uint64
     L.egs_create.argtypes = [i32, i32, i32, i32, C.POINTER(vp)]
+    L.egs_create_ex.argtypes = [i32, i32, i32, i32, i32, C.POINTER(vp)]
     L.egs_destroy.argtypes = [vp]
     L.egs_last_error.argtypes = [vp]; L.egs_last_error.restype = C.c_char_p
     L.egs_status_string.argtypes = [i32]; L.egs_status_string.restype = C.c_char_p
@@ -144,6 +150,7 @@ def units_array(req: Sequence[Tuple[int, int, int]]) -> np.ndarray:
 
 
 def masks_to_lists(masks, n_containers: int):
+    """GPU index lists of the first n_containers masks (up to 8 planes of up to 16 GPUs)."""
     return [[g for g in range(EGS_MAX_GPUS_WIDE) if (int(masks[c]) >> g) & 1] for c in range(n_containers)]
 
 
@@ -156,16 +163,20 @@ def _alloc_arrays(alloc):
 
 
 class Egs:
-    """One libegs handle == one device.  Method names follow the C ABI."""
+    """One libegs handle == one device.  Method names follow the C ABI.  c_max > 4 makes a sidecar handle
+    (egs_create_ex): pods of up to c_max containers, 8 masks per pod."""
 
-    def __init__(self, policy: int, max_nodes: int, g_max: int = 8, device: int = 0):
+    def __init__(self, policy: int, max_nodes: int, g_max: int = 8, device: int = 0, c_max: int = EGS_MAX_CONTAINERS):
         self.L = load()
         self.h = C.c_void_p()
-        st = self.L.egs_create(policy, max_nodes, g_max, device, C.byref(self.h))
+        if c_max == EGS_MAX_CONTAINERS:
+            st = self.L.egs_create(policy, max_nodes, g_max, device, C.byref(self.h))
+        else:
+            st = self.L.egs_create_ex(policy, max_nodes, g_max, c_max, device, C.byref(self.h))
         if st != EGS_OK:
             raise EgsError(st, "egs_create", "(is a CUDA device visible?)")
-        self.max_nodes, self.g_max, self.policy = max_nodes, g_max, policy
-        self.row_w, self.mask_dtype = row_width(g_max), mask_dtype(g_max)
+        self.max_nodes, self.g_max, self.policy, self.c_max = max_nodes, g_max, policy, c_max
+        self.row_w, self.mask_dtype, self.n_masks = row_width(g_max), mask_dtype(g_max), masks_per_pod(c_max)
 
     def close(self):
         if getattr(self, "h", None):
@@ -245,13 +256,13 @@ class Egs:
         return st, out[:n]
 
     def bind(self, node: int, req, uid: int):
-        masks = np.zeros(4, self.mask_dtype)
+        masks = np.zeros(self.n_masks, self.mask_dtype)
         st = self.L.egs_bind(self.h, node, len(req), _p(units_array(req)), uid, _p(masks))
         return st, (masks_to_lists(masks, len(req)) if st == EGS_OK else None)
 
     def peek(self, node: int, req):
         valid, score = C.c_int32(0), C.c_int32(0)
-        masks = np.zeros(4, self.mask_dtype)
+        masks = np.zeros(self.n_masks, self.mask_dtype)
         self._ck(self.L.egs_option_peek(self.h, node, len(req), _p(units_array(req)), C.byref(valid),
                                         C.byref(score), _p(masks)), "egs_option_peek")
         if not valid.value:
@@ -259,10 +270,11 @@ class Egs:
         return masks_to_lists(masks, len(req)), score.value
 
     def option_dump(self, req, node0: int = 0, n: Optional[int] = None):
-        """Option cache of request `req` on nodes [node0, node0+n): (state u8, score i32, alloc_mask [n,4] of
-        mask_dtype: u8, or u16 on a wide handle)."""
+        """Option cache of request `req` on nodes [node0, node0+n): (state u8, score i32, alloc_mask [n, n_masks] of
+        mask_dtype: u8, or u16 on a wide handle; n_masks is 4, or 8 on a sidecar handle)."""
         n = self.max_nodes - node0 if n is None else n
-        st = np.zeros(max(n, 1), np.uint8); sc = np.zeros(max(n, 1), np.int32); am = np.zeros((max(n, 1), 4), self.mask_dtype)
+        st = np.zeros(max(n, 1), np.uint8); sc = np.zeros(max(n, 1), np.int32)
+        am = np.zeros((max(n, 1), self.n_masks), self.mask_dtype)
         self._ck(self.L.egs_option_dump(self.h, len(req), _p(units_array(req)), node0, n, _p(st), _p(sc), _p(am)),
                  "egs_option_dump")
         return st[:n], sc[:n], am[:n]
@@ -284,7 +296,7 @@ class Egs:
         c_off = np.ascontiguousarray(c_off, np.int32); units = np.ascontiguousarray(units, np.int32)
         at = np.ascontiguousarray(mut_at, np.int32); a = mutations_array(records)
         out = dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
-                   alloc_mask=np.zeros((P, 4), self.mask_dtype), fit_count=np.zeros(P, np.int32),
+                   alloc_mask=np.zeros((P, self.n_masks), self.mask_dtype), fit_count=np.zeros(P, np.int32),
                    fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
         u = None if uids is None else np.ascontiguousarray(uids, np.uint64)
         self._ck(self.L.egs_schedule_batch_mut(self.h, mode, P, _p(c_off), _p(units), _p(u), len(records), _p(at), _p(a),
@@ -305,7 +317,7 @@ class Egs:
         c_off = np.ascontiguousarray(c_off, np.int32)
         units = np.ascontiguousarray(units, np.int32)
         out = dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
-                   alloc_mask=np.zeros((P, 4), self.mask_dtype), fit_count=np.zeros(P, np.int32),
+                   alloc_mask=np.zeros((P, self.n_masks), self.mask_dtype), fit_count=np.zeros(P, np.int32),
                    fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
         u = None if uids is None else np.ascontiguousarray(uids, np.uint64)
         self._ck(self.L.egs_schedule_batch(self.h, mode, P, _p(c_off), _p(units), _p(u), _p(out["node"]),
@@ -320,7 +332,7 @@ class Egs:
         units = np.ascontiguousarray(units, np.int32)
         vec_pods = min(vec_pods, P)
         out = dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
-                   alloc_mask=np.zeros((P, 4), self.mask_dtype), fit_count=np.zeros(P, np.int32),
+                   alloc_mask=np.zeros((P, self.n_masks), self.mask_dtype), fit_count=np.zeros(P, np.int32),
                    fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64),
                    vec_fit=np.zeros((max(vec_pods, 1), self.max_nodes), np.uint8),
                    vec_score=np.zeros((max(vec_pods, 1), self.max_nodes), np.int32))

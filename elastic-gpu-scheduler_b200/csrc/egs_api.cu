@@ -18,7 +18,7 @@
 #include "egs_rounds.cuh"
 #include "pod_book.h"
 
-struct Shape { int C; egs_unit u[EGS_C]; };
+struct Shape { int C; egs_unit u[EGS_CA]; };
 
 // Pinned host buffer holding (node[n], status[n]) of a batch.  Recycled through egs_handle::pin_pool: allocating and
 // freeing pinned memory cost milliseconds and synchronise the device -- too much for a small batch on the extender's path.
@@ -63,6 +63,7 @@ struct Checkpoint {
 struct egs_handle {
   int policy = 0, max_nodes = 0, n_pad = 0, g_max = 0, device = 0, n_sm = 0;
   int row_w = EGS_G, mask_b = 1;          // EGS_ROW_WIDTH(g_max), EGS_MASK_BYTES(g_max)
+  int c_max = EGS_C, planes = EGS_C;      // largest pod Traded, EGS_MASKS_PER_POD(c_max)
   int rank = 0, world = 1, lo = 0, hi = 0;
   cudaStream_t stream = nullptr;
   DeviceBuf<int32_t> d_core, d_mem, d_mem_total;
@@ -83,6 +84,7 @@ struct egs_handle {
   DeviceBuf<Partial> d_partials; DeviceBuf<unsigned int> d_ticket; DeviceBuf<int32_t> d_result;
   PinnedBuf<int32_t> h_result;
   DeviceBuf<int32_t> d_ids; DeviceBuf<uint8_t> d_fit; DeviceBuf<int32_t> d_score;
+  DeviceBuf<int32_t> d_miss; DeviceBuf<unsigned long long> d_keys; int leaf_grid = 0;   // leaf-split Trade (sidecar)
   PinnedBuf<char> h_stage;                                      // staging
   // eval scratch (profile)
   DeviceBuf<uint8_t> d_ev_fit; DeviceBuf<int32_t> d_ev_score; DeviceBuf<uint8_t> d_ev_gpu; DeviceBuf<char> d_flush;
@@ -111,17 +113,20 @@ struct egs_handle {
 
 static int fail(egs_handle *h, int code, const char *msg) { h->err = msg; return code; }
 
-// The one place the row width picks a kernel instantiation: f(std::integral_constant<int, G>()) with G the handle's
-// row width, 8 or 16.
+// The one place the handle's geometry picks a kernel instantiation: f(Geo<G, NP>()) with G the row width and NP the
+// mask planes per pod -- (8, 4), (16, 4) on a wide handle, or (8, 8) on a sidecar handle.
+template <int G_, int NP_> struct Geo { static constexpr int G = G_, NP = NP_; };
 template <class F>
-static int by_width(const egs_handle *h, F &&f) {
-  return h->row_w == 16 ? f(std::integral_constant<int, 16>()) : f(std::integral_constant<int, EGS_G>());
+static int by_geometry(const egs_handle *h, F &&f) {
+  if (h->row_w == 16) return f(Geo<16, EGS_C>());
+  return h->planes == EGS_CA ? f(Geo<EGS_G, EGS_CA>()) : f(Geo<EGS_G, EGS_C>());
 }
 static bool is_wide(const egs_handle *h) { return h->row_w > EGS_G; }
+static bool is_sidecar(const egs_handle *h) { return h->planes > EGS_C; }
 
-// Packed option masks (container c at bits [G*c, G*c + G)) -> EGS_MAX_CONTAINERS little-endian masks of mask_b bytes.
+// Packed option masks (container c at bits [G*c, G*c + G)) -> EGS_MASKS_PER_POD little-endian masks of mask_b bytes.
 static void put_masks(const egs_handle *h, uint64_t masks, uint8_t *out) {
-  for (int c = 0; c < EGS_C; c++)
+  for (int c = 0; c < h->planes; c++)
     for (int b = 0; b < h->mask_b; b++) out[c * h->mask_b + b] = (uint8_t)(masks >> (h->row_w * c + 8 * b));
 }
 
@@ -135,12 +140,12 @@ static OptTable table(egs_handle *h, int slot) {
   t.plane = (size_t)h->n_pad;
   t.st = h->tables.st + (size_t)slot * h->n_pad;
   t.sc = h->tables.sc + (size_t)slot * h->n_pad;
-  t.al = h->tables.al + (size_t)slot * EGS_C * h->n_pad * h->mask_b;
+  t.al = h->tables.al + (size_t)slot * h->planes * h->n_pad * h->mask_b;
   return t;
 }
 
 int OptTables::grow(egs_handle *h, int cap) {
-  const size_t np = (size_t)h->n_pad, al_plane = np * EGS_C * h->mask_b;
+  const size_t np = (size_t)h->n_pad, al_plane = np * h->planes * h->mask_b;
   CK(h, ::grow(h->stream, true, to(st, np * cap), to(sc, np * cap), to(al, al_plane * cap)));
   CK(h, cudaMemsetAsync(st + np * slots, OPT_ABSENT, np * (cap - slots), h->stream));
   slots = cap;
@@ -148,7 +153,7 @@ int OptTables::grow(egs_handle *h, int cap) {
 }
 
 int OptTables::copy_from(egs_handle *h, const OptTables &o, int n) {
-  const size_t np = (size_t)h->n_pad, al_plane = np * EGS_C * h->mask_b;
+  const size_t np = (size_t)h->n_pad, al_plane = np * h->planes * h->mask_b;
   CK(h, st.copy_from(o.st, np * n, h->stream));
   CK(h, sc.copy_from(o.sc, np * n, h->stream));
   CK(h, al.copy_from(o.al, al_plane * n, h->stream));
@@ -180,7 +185,7 @@ static int intern_slow(egs_handle *h, int C, const egs_unit *u, int *slot);
 
 // hot entry: one hash + one probe per pod (a batch of 10^6 pods re-uses a handful of shapes)
 static inline int intern(egs_handle *h, int C, const egs_unit *u, int *slot) {
-  if (C >= 1 && C <= EGS_C && u) {
+  if (C >= 1 && C <= h->c_max && u) {
     const uint64_t hv = shape_hash(C, u);
     const size_t mask = h->shape_cache.size() - 1;
     for (size_t i = hv & mask, n = 0; n < 8; i = (i + 1) & mask, n++) {
@@ -208,7 +213,7 @@ static std::string shape_key(int C, const egs_unit *u) {
 }
 
 static int intern_slow(egs_handle *h, int C, const egs_unit *u, int *slot) {
-  TRY(check_units(C, u));
+  TRY(check_units(C, u, h->c_max));
   const std::string key = shape_key(C, u);
   auto it = h->shape_ids.find(key);
   if (it != h->shape_ids.end()) { *slot = it->second; return EGS_OK; }
@@ -223,6 +228,56 @@ static int intern_slow(egs_handle *h, int C, const egs_unit *u, int *slot) {
 }
 
 static bool is_single(int C, const egs_unit *u) { return C == 1 && u[0].count == 0 && u[0].core >= 0 && u[0].mem >= 0; }
+
+// Digit width of the leaf space on this handle: every node has at most g_max GPUs (trade_leaf_space).
+static int leaf_bits(const egs_handle *h) { return h->g_max <= 1 ? 0 : h->g_max <= 2 ? 1 : h->g_max <= 4 ? 2 : 3; }
+static int n_branch(int C, const egs_unit *u) {
+  int n = 0;
+  for (int i = 0; i < C; i++) n += u[i].count == 0 ? 1 : 0;
+  return n;
+}
+// Shapes whose leaf space has more than 2^LEAF_SPLIT_LOG2 leaves are Traded by the leaf-split kernels; smaller ones
+// by the one-thread DFS inside k_pass / k_gather_*.  2^12 = 8^4 is the DFS's worst case on a handle without sidecars.
+constexpr int LEAF_SPLIT_LOG2 = 12;
+static bool leaf_split(const egs_handle *h, int C, const egs_unit *u) {
+  return is_sidecar(h) && leaf_bits(h) * n_branch(C, u) > LEAF_SPLIT_LOG2;
+}
+
+// The leaf-split Trade of every candidate of slot `slot` whose option is absent (k_trade_probe, k_trade_leaves,
+// k_trade_commit; egs_kernels.cuh), enqueued on the stream.  d_ids == nullptr: nodes [0, n).  With d_score the probe is
+// also Score's read of the cache and the commit raises d_panic.
+static int trade_misses(egs_handle *h, int slot, int C, const egs_unit *u, const int32_t *d_ids, int n,
+                        int32_t *d_score, int *d_panic) {
+  if (n <= 0) return EGS_OK;
+  if ((size_t)n > h->d_miss.cap()) {
+    const size_t cap = std::max((size_t)n, (size_t)h->n_pad);
+    CK(h, grow(h->stream, false, to(h->d_miss, cap), to(h->d_keys, cap)));
+  }
+  if (!h->leaf_grid) {
+    int per_sm = 0;
+    CK(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_trade_leaves, LEAF_THREADS, 0));
+    h->leaf_grid = std::max(per_sm, 1) * h->n_sm;
+  }
+  unsigned int *d_n = reinterpret_cast<unsigned int *>(h->d_ticket.get()) + 1;   // ticket[0] belongs to k_pass
+  CK(h, cudaMemsetAsync(d_n, 0, sizeof(unsigned int), h->stream));
+  const OptTable t = table(h, slot);
+  ProbeArgs pa;
+  pa.st = t.st; pa.sc = t.sc; pa.ids = d_ids; pa.n = n; pa.n_nodes = h->max_nodes;
+  pa.miss = h->d_miss; pa.n_miss = d_n; pa.keys = h->d_keys; pa.out_score = d_score;
+  const int grid = (n + 255) / 256;
+  k_trade_probe<<<grid, 256, 0, h->stream>>>(pa);
+  LeafArgs la;
+  la.core = h->d_core; la.mem = h->d_mem; la.mem_total = h->d_mem_total;
+  la.policy = h->policy; la.bits = leaf_bits(h); la.nbranch = n_branch(C, u);
+  const int nleaf = 1 << (la.bits * la.nbranch);
+  la.tiles = (nleaf + LEAF_THREADS * LEAF_CHUNK - 1) / (LEAF_THREADS * LEAF_CHUNK);
+  la.req = make_req<ReqW>(C, u);
+  la.miss = h->d_miss; la.n_miss = d_n; la.keys = h->d_keys;
+  k_trade_leaves<<<h->leaf_grid, LEAF_THREADS, 0, h->stream>>>(la);
+  k_trade_commit<<<grid, 256, 0, h->stream>>>(la, t, d_panic);
+  CK(h, cudaGetLastError());
+  return EGS_OK;
+}
 
 constexpr size_t PIN_POOL_MAX = 4;
 static void pin_put(egs_handle *h, PinBuf b) {
@@ -270,13 +325,20 @@ static void free_handle(egs_handle *h) {
 
 // ------------------------------------------------------------------------------- lifecycle
 extern "C" int egs_create(int policy, int max_nodes, int g_max, int device, egs_handle **out) {
+  return egs_create_ex(policy, max_nodes, g_max, EGS_MAX_CONTAINERS, device, out);
+}
+
+extern "C" int egs_create_ex(int policy, int max_nodes, int g_max, int c_max, int device, egs_handle **out) {
   if (!out || max_nodes < 1 || g_max < 1 || g_max > EGS_MAX_GPUS_WIDE || (policy != EGS_BINPACK && policy != EGS_SPREAD))
     return EGS_ERR_BAD_ARG;
+  if (c_max < 1 || c_max > EGS_MAX_CONTAINERS_APPLY) return EGS_ERR_BAD_ARG;
+  if (c_max > EGS_MAX_CONTAINERS && g_max > EGS_MAX_GPUS) return EGS_ERR_BAD_ARG;   // 128-bit masks, 2^32 leaves
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1 || device < 0 || device >= ndev) return EGS_ERR_CUDA;
   egs_handle *h = new egs_handle();
   h->policy = policy; h->max_nodes = max_nodes; h->g_max = g_max; h->device = device;
   h->row_w = EGS_ROW_WIDTH(g_max); h->mask_b = EGS_MASK_BYTES(g_max);
+  h->c_max = std::max(c_max, EGS_MAX_CONTAINERS); h->planes = EGS_MASKS_PER_POD(c_max);
   h->n_pad = (max_nodes + 1023) / 1024 * 1024;
   h->lo = 0; h->hi = max_nodes;
   h->h_gpu_count.assign(max_nodes, 0); h->h_mem_total.assign(max_nodes, 0);
@@ -552,25 +614,35 @@ static int gather(egs_handle *h, bool score, int n, const int32_t *node_ids, int
     CK(h, grow(h->stream, false, to(h->d_ids, cap), to(h->d_fit, cap), to(h->d_score, cap)));
   }
   TRY(ensure_stage(h, (size_t)n * sizeof(int32_t)));
-  GatherArgs a;
-  a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total;
-  a.n = n; a.n_nodes = h->max_nodes; a.policy = h->policy; a.req = make_req(C, units); a.t = table(h, slot);
-  a.ids = nullptr; a.out_fit = h->d_fit; a.out_score = h->d_score; a.panic_flag = h->d_result + 8;
+  const int32_t *d_ids = nullptr;
   if (node_ids) {
     CK(h, cudaStreamSynchronize(h->stream));
     memcpy(h->h_stage, node_ids, (size_t)n * sizeof(int32_t));
     CK(h, cudaMemcpyAsync(h->d_ids, h->h_stage, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
-    a.ids = h->d_ids;
+    d_ids = h->d_ids;
   }
-  const bool single = is_single(C, units);
+  const bool single = is_single(C, units), split = leaf_split(h, C, units);
   const int grid = (n + 255) / 256;
+  // the arguments in the geometry's request type
+  auto args = [&](auto W) {
+    GatherArgsT<ReqOf<decltype(W)::NP>> a;
+    a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total;
+    a.n = n; a.n_nodes = h->max_nodes; a.policy = h->policy; a.req = make_req<ReqOf<decltype(W)::NP>>(C, units);
+    a.t = table(h, slot); a.ids = d_ids; a.out_fit = h->d_fit; a.out_score = h->d_score; a.panic_flag = h->d_result + 8;
+    return a;
+  };
   if (score) {
     CK(h, cudaMemsetAsync(h->d_result + 8, 0, sizeof(int32_t), h->stream));
-    by_width(h, [&](auto W) -> int {
-      constexpr int G = decltype(W)::value;
-      if (single) k_gather_score<G, true><<<grid, 256, 0, h->stream>>>(a); else k_gather_score<G, false><<<grid, 256, 0, h->stream>>>(a);
-      return EGS_OK;
-    });
+    if (split) {                                   // the probe is Score's read; the commit raises the panic flag
+      TRY(trade_misses(h, slot, C, units, d_ids, n, h->d_score, h->d_result + 8));
+    } else {
+      by_geometry(h, [&](auto W) -> int {
+        constexpr int G = decltype(W)::G, NP = decltype(W)::NP;
+        if (single) k_gather_score<G, NP, true><<<grid, 256, 0, h->stream>>>(args(W));
+        else k_gather_score<G, NP, false><<<grid, 256, 0, h->stream>>>(args(W));
+        return EGS_OK;
+      });
+    }
     CK(h, cudaGetLastError());
     CK(h, cudaMemcpyAsync(h->h_stage, h->d_score, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaMemcpyAsync(h->h_result, h->d_result + 8, sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
@@ -578,9 +650,11 @@ static int gather(egs_handle *h, bool score, int n, const int32_t *node_ids, int
     memcpy(out_score, h->h_stage, (size_t)n * sizeof(int32_t));
     return h->h_result[0] ? EGS_ERR_PANIC : EGS_OK;
   }
-  by_width(h, [&](auto W) -> int {
-    constexpr int G = decltype(W)::value;
-    if (single) k_gather_filter<G, true><<<grid, 256, 0, h->stream>>>(a); else k_gather_filter<G, false><<<grid, 256, 0, h->stream>>>(a);
+  if (split) TRY(trade_misses(h, slot, C, units, d_ids, n, nullptr, nullptr));   // k_gather_filter then only reads
+  by_geometry(h, [&](auto W) -> int {
+    constexpr int G = decltype(W)::G, NP = decltype(W)::NP;
+    if (single) k_gather_filter<G, NP, true><<<grid, 256, 0, h->stream>>>(args(W));
+    else k_gather_filter<G, NP, false><<<grid, 256, 0, h->stream>>>(args(W));
     return EGS_OK;
   });
   CK(h, cudaGetLastError());
@@ -610,15 +684,15 @@ static int bind_or_peek(egs_handle *h, int consume, int node_id, int C, const eg
   int slot;
   TRY(intern(h, C, units, &slot));
   TRY(settle_pending(h, true));
-  BindArgs a;
-  a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total; a.node = node_id;
-  a.req = make_req(C, units); a.t = table(h, slot);
-  a.all_st = h->tables.st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
   const bool known = consume && h->book.in_pods_map(node_id, uid);
-  a.skip_transact = known ? 1 : 0; a.consume = consume; a.result = h->d_result;
-  by_width(h, [&](auto W) -> int {
-    constexpr int G = decltype(W)::value;
-    k_bind<G><<<1, 1, 0, h->stream>>>(a);
+  by_geometry(h, [&](auto W) -> int {
+    constexpr int G = decltype(W)::G, NP = decltype(W)::NP;
+    BindArgsT<ReqOf<NP>> a;
+    a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total; a.node = node_id;
+    a.req = make_req<ReqOf<NP>>(C, units); a.t = table(h, slot);
+    a.all_st = h->tables.st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
+    a.skip_transact = known ? 1 : 0; a.consume = consume; a.result = h->d_result;
+    k_bind<G, NP><<<1, 1, 0, h->stream>>>(a);
     return EGS_OK;
   });
   CK(h, cudaGetLastError());
@@ -626,7 +700,7 @@ static int bind_or_peek(egs_handle *h, int consume, int node_id, int C, const eg
   CK(h, cudaStreamSynchronize(h->stream));
   const int32_t *r = h->h_result;
   res[0] = r[0]; res[1] = r[1]; res[2] = r[3];
-  *masks = (uint32_t)r[2] | (is_wide(h) ? (uint64_t)(uint32_t)r[4] << 32 : 0);
+  *masks = (uint32_t)r[2] | (h->row_w * h->planes > 32 ? (uint64_t)(uint32_t)r[4] << 32 : 0);   // a 64-bit packed word
   if (consume) h->book.record_bind(node_id, uid, res[0] != 0, known, res[1]);
   return EGS_OK;
 }
@@ -663,13 +737,14 @@ extern "C" int egs_option_dump(egs_handle *h, int n_containers, const egs_unit *
   if (n == 0) return EGS_OK;
   const OptTable t = table(h, slot);
   const size_t sn = (size_t)n, mb = (size_t)h->mask_b;
-  TRY(ensure_stage(h, sn * (1 + 4 + EGS_C * mb)));
+  const int np = h->planes;
+  TRY(ensure_stage(h, sn * (1 + 4 + np * mb)));
   CK(h, cudaStreamSynchronize(h->stream));
   char *s = h->h_stage.get();
   int32_t *hs = (int32_t *)s; uint8_t *hst = (uint8_t *)(hs + sn); uint8_t *hal = hst + sn;
   CK(h, cudaMemcpyAsync(hs, t.sc + node0, 4 * sn, cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaMemcpyAsync(hst, t.st + node0, sn, cudaMemcpyDeviceToHost, h->stream));
-  for (int c = 0; c < EGS_C; c++)
+  for (int c = 0; c < np; c++)
     CK(h, cudaMemcpyAsync(hal + (size_t)c * sn * mb, t.al + ((size_t)c * t.plane + node0) * mb, sn * mb, cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaStreamSynchronize(h->stream));
   for (size_t i = 0; i < sn; i++) {
@@ -677,17 +752,17 @@ extern "C" int egs_option_dump(egs_handle *h, int n_containers, const egs_unit *
     if (out_state) out_state[i] = hst[i] == OPT_CACHED ? 1 : hst[i] == OPT_UNFIT ? 2 : 0;
     if (out_score) out_score[i] = cached ? hs[i] : 0;
     if (out_alloc_mask)
-      for (int c = 0; c < EGS_C; c++)
+      for (int c = 0; c < np; c++)
         for (size_t b = 0; b < mb; b++)
-          out_alloc_mask[(i * EGS_C + c) * mb + b] = (cached && c < n_containers) ? hal[((size_t)c * sn + i) * mb + b] : 0;
+          out_alloc_mask[(i * np + c) * mb + b] = (cached && c < n_containers) ? hal[((size_t)c * sn + i) * mb + b] : 0;
   }
   return EGS_OK;
 }
 
 static int apply_lists(egs_handle *h, int cancel, int node_id, int C, const egs_unit *units,
                        const int32_t *alloc_off, const int32_t *alloc_idx) {
-  return by_width(h, [&](auto W) -> int {
-    constexpr int G = decltype(W)::value;
+  return by_geometry(h, [&](auto W) -> int {
+    constexpr int G = decltype(W)::G;
     ApplyArgs<G> a; memset(&a, 0, sizeof a);
     a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total;
     a.op.node = node_id; a.op.cancel = cancel; a.op.req = make_req<ReqW>(C, units);
@@ -764,7 +839,7 @@ static int mutations_apply_locked(egs_handle *h, int n, const egs_mutation *ops)
       for (int j = 0; j < m.n_idx[c]; j++) if (m.idx[c][j] < 0 || m.idx[c][j] >= h->h_gpu_count[m.node_id]) return EGS_ERR_BAD_ARG;
     }
   }
-  return by_width(h, [&](auto W) -> int { return mutations_rows<decltype(W)::value>(h, n, ops); });
+  return by_geometry(h, [&](auto W) -> int { return mutations_rows<decltype(W)::G>(h, n, ops); });
 }
 
 // passes 2 and 3 of mutations_apply_locked on a handle of row width G
@@ -836,7 +911,7 @@ static int ensure_out(egs_handle *h, int P) {
   if ((size_t)P <= h->d_o_node.cap()) return EGS_OK;
   const size_t cap = (size_t)std::max(P, 1024);
   CK(h, grow(h->stream, false, to(h->d_o_node, cap), to(h->d_o_status, cap), to(h->d_o_fit, cap),
-             to(h->d_o_alloc, cap * EGS_C * h->mask_b), to(h->d_o_fd, cap), to(h->d_o_sd, cap)));
+             to(h->d_o_alloc, cap * h->planes * h->mask_b), to(h->d_o_fd, cap), to(h->d_o_sd, cap)));
   return EGS_OK;
 }
 
@@ -848,18 +923,20 @@ static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_un
   for (int p = 0; p < P; p++) {
     const int C = c_off[p + 1] - c_off[p];
     const egs_unit *u = units + c_off[p];
-    PassArgs a;
-    a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total; a.core_w = h->d_core; a.mem_w = h->d_mem;
-    a.n = h->max_nodes; a.policy = h->policy; a.req = make_req(C, u); a.t = table(h, slots[p]);
-    a.all_st = h->tables.st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
-    a.vec_fit = p < h->vec_pods ? h->d_vec_fit + (size_t)p * h->max_nodes : nullptr;
-    a.vec_score = p < h->vec_pods ? h->d_vec_score + (size_t)p * h->max_nodes : nullptr;
-    a.partials = h->d_partials; a.ticket = h->d_ticket;
-    a.pod = p; a.out = out;
-    by_width(h, [&](auto W) -> int {
-      constexpr int G = decltype(W)::value;
-      if (is_single(C, u)) k_pass<G, true><<<grid, PASS_THREADS, 0, h->stream>>>(a);
-      else k_pass<G, false><<<grid, PASS_THREADS, 0, h->stream>>>(a);
+    // a shape past the one-thread DFS is Traded on every node without an option first: k_pass then only reads caches
+    if (leaf_split(h, C, u)) TRY(trade_misses(h, slots[p], C, u, nullptr, h->max_nodes, nullptr, nullptr));
+    by_geometry(h, [&](auto W) -> int {
+      constexpr int G = decltype(W)::G, NP = decltype(W)::NP;
+      PassArgsT<ReqOf<NP>> a;
+      a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total; a.core_w = h->d_core; a.mem_w = h->d_mem;
+      a.n = h->max_nodes; a.policy = h->policy; a.req = make_req<ReqOf<NP>>(C, u); a.t = table(h, slots[p]);
+      a.all_st = h->tables.st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
+      a.vec_fit = p < h->vec_pods ? h->d_vec_fit + (size_t)p * h->max_nodes : nullptr;
+      a.vec_score = p < h->vec_pods ? h->d_vec_score + (size_t)p * h->max_nodes : nullptr;
+      a.partials = h->d_partials; a.ticket = h->d_ticket;
+      a.pod = p; a.out = out;
+      if (is_single(C, u)) k_pass<G, NP, true><<<grid, PASS_THREADS, 0, h->stream>>>(a);
+      else k_pass<G, NP, false><<<grid, PASS_THREADS, 0, h->stream>>>(a);
       return EGS_OK;
     });
     if ((p & 1023) == 0) CK(h, cudaGetLastError());
@@ -869,10 +946,14 @@ static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_un
   return EGS_OK;
 }
 
-// A wide handle has no rounds engine: EGS_MODE_ROUNDS is refused before the batch touches anything, and
+// Wide and sidecar handles have no rounds engine: EGS_MODE_ROUNDS is refused before the batch touches anything, and
 // EGS_MODE_AUTO runs the per-pod engine there.
+static bool per_pod_only(const egs_handle *h) { return is_wide(h) || is_sidecar(h); }
 static int refuse_wide_rounds(egs_handle *h, int mode) {
-  return is_wide(h) && mode == EGS_MODE_ROUNDS ? fail(h, EGS_ERR_BAD_ARG, "EGS_MODE_ROUNDS needs g_max <= EGS_MAX_GPUS") : EGS_OK;
+  if (mode != EGS_MODE_ROUNDS) return EGS_OK;
+  if (is_wide(h)) return fail(h, EGS_ERR_BAD_ARG, "EGS_MODE_ROUNDS needs g_max <= EGS_MAX_GPUS");
+  if (is_sidecar(h)) return fail(h, EGS_ERR_BAD_ARG, "EGS_MODE_ROUNDS needs c_max <= EGS_MAX_CONTAINERS");
+  return EGS_OK;
 }
 
 static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, const egs_unit *units,
@@ -884,7 +965,7 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
   std::vector<int> slots((size_t)P);
   for (int p = 0; p < P; p++) {
     const int C = c_off[p + 1] - c_off[p];
-    if (C < 1 || C > EGS_C) return EGS_ERR_BAD_ARG;
+    if (C < 1 || C > h->c_max) return EGS_ERR_BAD_ARG;
     TRY(intern(h, C, units + c_off[p], &slots[p]));
   }
   if (uids) {                                    // pods awaiting scheduling must be unknown and distinct
@@ -904,7 +985,7 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
     if (!dev.node) dev.node = h->d_o_node;          // uid bookkeeping needs node + status
     if (!dev.status) dev.status = h->d_o_status;
   }
-  if (mode == EGS_MODE_AUTO) mode = is_wide(h) ? EGS_MODE_RESCAN : EGS_MODE_ROUNDS;
+  if (mode == EGS_MODE_AUTO) mode = per_pod_only(h) ? EGS_MODE_RESCAN : EGS_MODE_ROUNDS;
   int batch_rc = EGS_OK, n_done = P;
   if (mode == EGS_MODE_RESCAN) TRY(batch_rescan(h, P, c_off, units, slots, dev));
   else if (mode == EGS_MODE_ROUNDS) batch_rc = batch_rounds(h, P, slots, dev, &n_done);
@@ -927,7 +1008,7 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
 
   if (!device_out) {
     size_t sp = (size_t)P;
-    const size_t ab = (size_t)EGS_C * h->mask_b;   // alloc bytes per pod
+    const size_t ab = (size_t)h->planes * h->mask_b;   // alloc bytes per pod
     TRY(ensure_stage(h, sp * (4 + 4 + 4 + ab + 8 + 8)));
     char *s = h->h_stage.get();
     int32_t *hn = (int32_t *)s, *hs = hn + sp, *hf = hs + sp;
@@ -957,7 +1038,7 @@ static PodOut pod_out(const egs_handle *h, int32_t *node, int32_t *status, uint8
                       uint64_t *fit_digest, uint64_t *score_digest, int p = 0) {
   PodOut o;
   o.node = node ? node + p : nullptr; o.status = status ? status + p : nullptr;
-  o.alloc = alloc ? alloc + (size_t)p * EGS_C * h->mask_b : nullptr; o.fit_count = fit_count ? fit_count + p : nullptr;
+  o.alloc = alloc ? alloc + (size_t)p * h->planes * h->mask_b : nullptr; o.fit_count = fit_count ? fit_count + p : nullptr;
   o.fit_digest = fit_digest ? (unsigned long long *)fit_digest + p : nullptr;
   o.score_digest = score_digest ? (unsigned long long *)score_digest + p : nullptr;
   return o;
@@ -1032,8 +1113,8 @@ extern "C" int egs_schedule_batch_device(egs_handle *h, int mode, int n_pods, co
                                          uint64_t *d_out_fit_digest, uint64_t *d_out_score_digest) {
   if (!h) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  if ((uintptr_t)d_out_alloc_mask % ((uintptr_t)EGS_C * h->mask_b))     // one packed word per pod (write_pod_out)
-    return fail(h, EGS_ERR_BAD_ARG, "d_out_alloc_mask must be aligned to EGS_MAX_CONTAINERS * EGS_MASK_BYTES(g_max)");
+  if ((uintptr_t)d_out_alloc_mask % ((uintptr_t)h->planes * h->mask_b))     // one packed word per pod (write_pod_out)
+    return fail(h, EGS_ERR_BAD_ARG, "d_out_alloc_mask must be aligned to EGS_MASKS_PER_POD(c_max) * EGS_MASK_BYTES(g_max)");
   const PodOut o = pod_out(h, d_out_node, d_out_status, d_out_alloc_mask, d_out_fit_count, d_out_fit_digest, d_out_score_digest);
   return batch_common(h, mode, n_pods, h_c_off, h_units, nullptr, o, true);
 }
@@ -1051,6 +1132,7 @@ extern "C" int egs_shard_set(egs_handle *h, int rank, int world) {
   if (!h || world < 1 || world > RD || rank < 0 || rank >= world) return EGS_ERR_BAD_ARG;
   Guard g(h);
   if (is_wide(h)) return fail(h, EGS_ERR_BAD_ARG, "the sharded engine is the rounds engine: it needs g_max <= EGS_MAX_GPUS");
+  if (is_sidecar(h)) return fail(h, EGS_ERR_BAD_ARG, "the sharded engine is the rounds engine: it needs c_max <= EGS_MAX_CONTAINERS");
   checkpoint_free(h);                             // a checkpoint holds for the shard layout it was taken under
   h->rank = rank; h->world = world;
   egs_shard_range(h->max_nodes, rank, world, &h->lo, &h->hi);
@@ -1069,6 +1151,8 @@ extern "C" int egs_profile_evaluate(egs_handle *h, int n_containers, const egs_u
                                     int flush_l2, float *out_ms_per_launch) {
   if (!h || iters < 1 || !out_ms_per_launch) return EGS_ERR_BAD_ARG;
   Guard g(h);
+  if (n_containers > EGS_C && n_containers <= h->c_max)
+    return fail(h, EGS_ERR_BAD_ARG, "egs_profile_evaluate takes at most EGS_MAX_CONTAINERS containers");
   TRY(check_units(n_containers, units));
   const size_t np = (size_t)h->n_pad;
   if (!h->d_ev_fit) CK(h, grow(h->stream, false, to(h->d_ev_fit, np), to(h->d_ev_score, np), to(h->d_ev_gpu, np * EGS_C * h->mask_b)));
@@ -1085,8 +1169,8 @@ extern "C" int egs_profile_evaluate(egs_handle *h, int n_containers, const egs_u
   if (is_wide(h)) items = 1;                      // a 16-wide row already keeps 8 loads of 16 B in flight per thread
   const int grid = (h->max_nodes + 256 * items - 1) / (256 * items);
   auto launch = [&]() {
-    by_width(h, [&](auto W) -> int {
-      constexpr int G = decltype(W)::value;
+    by_geometry(h, [&](auto W) -> int {
+      constexpr int G = decltype(W)::G;
       if (!single) k_evaluate<G, false, 1><<<(h->max_nodes + 255) / 256, 256, 0, h->stream>>>(a);
       else if constexpr (G == EGS_G) {
         if (items == 1) k_evaluate<G, true, 1><<<grid, 256, 0, h->stream>>>(a);

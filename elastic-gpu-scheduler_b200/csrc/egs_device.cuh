@@ -41,13 +41,15 @@
 
 // GPURequest (allocate.go:20) for one pod, by value in kernel params / shared memory.
 struct Req {
+  static constexpr int NC = EGS_C;   // containers the type holds: the option masks of a pod are NC planes
   int C;
   int core[EGS_C];
   int mem[EGS_C];
   int cnt[EGS_C];
 };
 #define EGS_CA EGS_MAX_CONTAINERS_APPLY
-struct ReqW { int C; int core[EGS_CA], mem[EGS_CA], cnt[EGS_CA]; };   // a pod as AddPod / ForgetPod see it (up to 8 containers)
+// a pod as AddPod / ForgetPod see it, and as a sidecar handle (c_max > 4) Trades it: up to 8 containers
+struct ReqW { static constexpr int NC = EGS_CA; int C; int core[EGS_CA], mem[EGS_CA], cnt[EGS_CA]; };
 
 // Req or ReqW from C units (C within the type's bound, checked by the caller); unused containers are zero.
 template <class R = Req>
@@ -81,13 +83,19 @@ __host__ __device__ __forceinline__ uint64_t cand_key(int32_t score, uint32_t no
 __host__ __device__ __forceinline__ uint32_t key_node(uint64_t key) { return 0xFFFFFFFFu - (uint32_t)key; }
 __host__ __device__ __forceinline__ int32_t key_score(uint64_t key) { return (int32_t)(key >> 32); }
 
-// Per row width G: the GPU mask of one container (Mask) and the masks of a pod's EGS_C containers packed into one
-// word (Packed: container k at bits [G*k, G*k + G)), and LG = log2(G) for the folded Trade keys.
+// Per row width G: the GPU mask of one container (Mask), and LG = log2(G) for the folded Trade keys.
 template <int G> struct RowWidth;
-template <> struct RowWidth<8> { typedef uint8_t Mask; typedef uint32_t Packed; static constexpr int LG = 3; };
-template <> struct RowWidth<16> { typedef uint16_t Mask; typedef uint64_t Packed; static constexpr int LG = 4; };
+template <> struct RowWidth<8> { typedef uint8_t Mask; static constexpr int LG = 3; };
+template <> struct RowWidth<16> { typedef uint16_t Mask; static constexpr int LG = 4; };
 template <int G> using MaskT = typename RowWidth<G>::Mask;
-template <int G> using PackedT = typename RowWidth<G>::Packed;
+// Per geometry (row width G, NP mask planes per pod): the masks of a pod's NP containers packed into one word
+// (container k at bits [G*k, G*k + G)).  Three geometries exist: (8, 4) and (16, 4), and (8, 8) on a sidecar handle.
+template <int G, int NP> struct Geometry;
+template <> struct Geometry<8, EGS_C> { typedef uint32_t Packed; typedef Req R; };
+template <> struct Geometry<16, EGS_C> { typedef uint64_t Packed; typedef Req R; };
+template <> struct Geometry<8, EGS_CA> { typedef uint64_t Packed; typedef ReqW R; };
+template <int G, int NP = EGS_C> using PackedT = typename Geometry<G, NP>::Packed;
+template <int NP> using ReqOf = typename Geometry<EGS_G, NP>::R;
 
 // G/4 16-byte read-only loads per array: one node's row (4*G B core + 4*G B mem), all issued before any use.
 template <int G>
@@ -177,16 +185,16 @@ EGS_HD int trade_lane_key(const int (&c)[EGS_G], const int (&m)[EGS_G], int gl, 
 }
 
 // ---------------------------------------------------------------------------------------------
-// General Trade: up to EGS_C containers, whole-GPU units, sentinel units.  Depth-first over
-// the containers exactly as gpu.go:72-123.  Cold path: rows live in local memory.
+// General Trade: up to R::NC containers (4, or 8 on a sidecar handle), whole-GPU units, sentinel units.  Depth-first
+// over the containers exactly as gpu.go:72-123.  Cold path: rows live in local memory.
 // ---------------------------------------------------------------------------------------------
-template <int G>
+template <int G, class R>
 struct TradeCtx {
-  typedef PackedT<G> P;
+  typedef PackedT<G, R::NC> P;
   int c[G], m[G];
   int mem_total, policy;
-  const Req *r;
-  P masks;              // 4 x Mask: GPUs chosen per container on the current DFS path
+  const R *r;
+  P masks;              // R::NC x Mask: GPUs chosen per container on the current DFS path
   int best;
   P best_masks;
   bool found;
@@ -197,8 +205,8 @@ struct TradeCtx {
 #else
 #define EGS_HD_NOINLINE __host__ __device__ inline
 #endif
-template <int G>
-EGS_HD_NOINLINE void trade_leaf(TradeCtx<G> &t) {  // gpu.go:73-93
+template <int G, class R>
+EGS_HD_NOINLINE void trade_leaf(TradeCtx<G, R> &t) {  // gpu.go:73-93
   int s = 0;
   if (t.policy == EGS_BINPACK) {
     // rateIndexes: containers holding exactly one GPU (gpu.go:76-83); k = distinct GPUs (rater.go:19-30)
@@ -225,10 +233,10 @@ EGS_HD_NOINLINE void trade_leaf(TradeCtx<G> &t) {  // gpu.go:73-93
   t.best_masks = t.masks;
 }
 
-template <int G, int CI>
-EGS_HD_NOINLINE void trade_dfs(TradeCtx<G> &t) {
-  typedef PackedT<G> P;
-  if constexpr (CI == EGS_C) {
+template <int G, class R, int CI>
+EGS_HD_NOINLINE void trade_dfs(TradeCtx<G, R> &t) {
+  typedef PackedT<G, R::NC> P;
+  if constexpr (CI == R::NC) {
     trade_leaf(t);
   } else {
     if (CI == t.r->C) { trade_leaf(t); return; }
@@ -243,7 +251,7 @@ EGS_HD_NOINLINE void trade_dfs(TradeCtx<G> &t) {
 #pragma unroll 1
       for (int g = 0; g < G; g++) if ((fm >> g) & 1u) { t.c[g] = 0; t.m[g] = 0; }          // Add gpu.go:32-34
       t.masks = keep | ((P)fm << (G * CI));
-      trade_dfs<G, CI + 1>(t);
+      trade_dfs<G, R, CI + 1>(t);
 #pragma unroll 1
       for (int g = 0; g < G; g++) if ((fm >> g) & 1u) { t.c[g] = EGS_CORE_PER_GPU; t.m[g] = t.mem_total; }  // Sub gpu.go:42-44
       t.masks = keep;
@@ -254,21 +262,21 @@ EGS_HD_NOINLINE void trade_dfs(TradeCtx<G> &t) {
       if (!(t.c[g] >= rc && t.m[g] >= rm)) continue;
       t.c[g] -= rc; t.m[g] -= rm;
       t.masks = keep | (((P)1u << g) << (G * CI));
-      trade_dfs<G, CI + 1>(t);
+      trade_dfs<G, R, CI + 1>(t);
       t.c[g] += rc; t.m[g] += rm;
     }
     t.masks = keep;
   }
 }
 
-template <int G>
+template <int G, class R>
 EGS_HD bool trade_general(const int (&c)[G], const int (&m)[G], int mem_total,
-                          const Req &r, int policy, int &score, PackedT<G> &masks) {
-  TradeCtx<G> t;
+                          const R &r, int policy, int &score, PackedT<G, R::NC> &masks) {
+  TradeCtx<G, R> t;
 #pragma unroll
   for (int g = 0; g < G; g++) { t.c[g] = c[g]; t.m[g] = m[g]; }
   t.mem_total = mem_total; t.policy = policy; t.r = &r; t.masks = 0; t.best = 0; t.best_masks = 0; t.found = false;
-  trade_dfs<G, 0>(t);
+  trade_dfs<G, R, 0>(t);
   score = t.best; masks = t.best_masks;
   return t.found;
 }
@@ -281,8 +289,61 @@ EGS_HD bool trade_general(const int (&c)[G], const int (&m)[G], int mem_total,
 // lexicographic order with the FIRST branching container most significant, and "the last maximal leaf wins"
 // (gpu.go:85) == the maximal (score, leaf index).  Digits are `bits` wide; a digit that names a GPU the node does
 // not have meets a PAD row and fails CanAllocate like any other infeasible choice.
-// Returns the leaf's score (>= 0) and its Allocated masks, or -1 when the leaf is infeasible.
+// Returns the leaf's score (>= 0) and its Allocated masks, or -1 when the leaf is infeasible.  The template takes
+// ReqW and 64-bit masks (up to 8 containers, the leaf-split Trade of a sidecar handle); the overload after it is the
+// same evaluation on Req and 32-bit masks (the resolver), kept as a plain function because the resolver kernels
+// compile to a different register assignment when it is a template instance.
+// With `fail`, an infeasible leaf also reports how many of its leading digits already make it infeasible: every leaf
+// that shares those digits is infeasible too (trade_leaf_next skips them).  0 means no leaf of the node is feasible.
 // ---------------------------------------------------------------------------------------------
+template <class R, class P>
+EGS_HD int trade_leaf_eval(const int (&c0)[EGS_G], const int (&m0)[EGS_G], int mem_total, const R &r, int policy,
+                           int bits, int nbranch, int leaf, P &masks_out, int *fail = nullptr) {
+  int c[EGS_G], m[EGS_G];
+#pragma unroll
+  for (int g = 0; g < EGS_G; g++) { c[g] = c0[g]; m[g] = m0[g]; }
+  P masks = 0;
+  uint32_t used = 0;
+  int j = 0;                                                  // index among the branching containers
+  for (int i = 0; i < r.C; i++) {
+    if (r.cnt[i] > 0) {                                       // gpu.go:95-109 with GetFreeGPUs gpu.go:193-202
+      uint32_t fm = 0; int nf = 0;
+#pragma unroll
+      for (int g = 0; g < EGS_G; g++) {
+        const bool fr = nf < r.cnt[i] && c[g] == EGS_CORE_PER_GPU && m[g] == mem_total;
+        fm |= fr ? (1u << g) : 0u; nf += fr ? 1 : 0;
+      }
+      if (nf < r.cnt[i]) { if (fail) *fail = j; return -1; }  // decided by the digits taken so far
+#pragma unroll
+      for (int g = 0; g < EGS_G; g++) { const bool t = (fm >> g) & 1u; c[g] = t ? 0 : c[g]; m[g] = t ? 0 : m[g]; }   // Add gpu.go:32-34
+      masks |= (P)fm << (8 * i);
+      if (EGS_POPC(fm) == 1) used |= fm;
+    } else {                                                  // gpu.go:110-122
+      const int gi = (leaf >> (bits * (nbranch - 1 - j))) & ((1 << bits) - 1);
+      j++;
+      int cg = EGS_PAD, mg = EGS_PAD;
+#pragma unroll
+      for (int g = 0; g < EGS_G; g++) { cg = g == gi ? c[g] : cg; mg = g == gi ? m[g] : mg; }
+      if (!(cg >= r.core[i] && mg >= r.mem[i])) { if (fail) *fail = j; return -1; }   // CanAllocate gpu.go:55 (PAD rows fail)
+#pragma unroll
+      for (int g = 0; g < EGS_G; g++) { c[g] -= g == gi ? r.core[i] : 0; m[g] -= g == gi ? r.mem[i] : 0; }
+      masks |= (P)(1u << gi) << (8 * i);
+      used |= 1u << gi;
+    }
+  }
+  masks_out = masks;
+  if (policy != EGS_BINPACK) return 0;                        // Spread.Rate rater.go:56-59
+  const int k = EGS_POPC(used);                               // rater.go:19-30
+  int cmin = INT32_MAX, cmax = INT32_MIN, mmin = INT32_MAX, mmax = INT32_MIN;
+#pragma unroll
+  for (int g = 0; g < EGS_G; g++) {
+    const bool real = c0[g] != EGS_PAD;
+    cmin = real ? EGS_MIN(cmin, c[g]) : cmin; cmax = real ? EGS_MAX(cmax, c[g]) : cmax;
+    mmin = real ? EGS_MIN(mmin, m[g]) : mmin; mmax = real ? EGS_MAX(mmax, m[g]) : mmax;
+  }
+  const int range = (mmax + cmax - mmin - cmin) / 2;
+  return range / (k + 1) * 100;
+}
 EGS_HD int trade_leaf_eval(const int (&c0)[EGS_G], const int (&m0)[EGS_G], int mem_total, const Req &r, int policy,
                            int bits, int nbranch, int leaf, uint32_t &masks_out) {
   int c[EGS_G], m[EGS_G];
@@ -329,8 +390,15 @@ EGS_HD int trade_leaf_eval(const int (&c0)[EGS_G], const int (&m0)[EGS_G], int m
   const int range = (mmax + cmax - mmin - cmin) / 2;
   return range / (k + 1) * 100;
 }
+// The first leaf after `leaf` that does not share its first `fail` digits (trade_leaf_eval's report): nleaf when
+// fail == 0.
+EGS_HD int trade_leaf_next(int leaf, int fail, int bits, int nbranch) {
+  const int sh = bits * (nbranch - fail);
+  return ((leaf >> sh) + 1) << sh;
+}
 // geometry of the leaf space of request r on a node with the given rows
-EGS_HD void trade_leaf_space(const int (&c0)[EGS_G], const Req &r, int &bits, int &nbranch, int &nleaf) {
+template <class R>
+EGS_HD void trade_leaf_space(const int (&c0)[EGS_G], const R &r, int &bits, int &nbranch, int &nleaf) {
   int gcount = 0;
 #pragma unroll
   for (int g = 0; g < EGS_G; g++) gcount += c0[g] != EGS_PAD ? 1 : 0;
@@ -346,13 +414,13 @@ __host__ __device__ __forceinline__ bool req_is_single(const Req &r) {
 }
 
 // Trade dispatch.  `masks` packs one G-bit GPU mask per container.
-template <int G>
+template <int G, class R>
 EGS_HD bool trade_any(const int (&c)[G], const int (&m)[G], int mem_total,
-                      const Req &r, bool single, int policy, int &score, PackedT<G> &masks) {
+                      const R &r, bool single, int policy, int &score, PackedT<G, R::NC> &masks) {
   if (single) {
     int g;
     bool ok = trade_single(c, m, r.core[0], r.mem[0], policy, score, g);
-    masks = (PackedT<G>)1u << g;
+    masks = (PackedT<G, R::NC>)1u << g;
     return ok;
   }
   return trade_general(c, m, mem_total, r, policy, score, masks);
@@ -360,9 +428,9 @@ EGS_HD bool trade_any(const int (&c)[G], const int (&m)[G], int mem_total,
 
 // GPUs.Transact gpu.go:153-175 on the node's rows in global memory (one thread).
 // Returns true on success; on failure the Adds already made stay (no rollback).
-template <int G>
-EGS_HD bool transact_row(int32_t *core, int32_t *mem, int mem_total, const Req &r,
-                         PackedT<G> masks) {
+template <int G, class R>
+EGS_HD bool transact_row(int32_t *core, int32_t *mem, int mem_total, const R &r,
+                         PackedT<G, R::NC> masks) {
   for (int i = 0; i < r.C; i++) {
     uint32_t mk = (uint32_t)(masks >> (G * i)) & ((1u << G) - 1u);
     if (r.cnt[i] > 0) {

@@ -11,8 +11,11 @@
 //                ForgetPod in one launch.
 // Each reference step these kernels share is written once: Assume (assume_option), Allocate
 // (allocate_option), and the AddPod / ForgetPod row update (apply_op, egs_device.cuh).
-// Every kernel here is a template on the row width G (8, or 16 on a handle with g_max > 8); the rounds engine
-// (egs_rounds.cuh) uses the 8-wide instantiations only.
+//   k_trade_probe / k_trade_leaves / k_trade_commit : the leaf-split Trade of a sidecar handle (c_max > 4) for shapes
+//                whose leaf space is larger than one thread should walk; the kernels above then only read caches.
+// Every kernel here is a template on the geometry: row width G (8, or 16 on a handle with g_max > 8) and, where masks
+// or requests are involved, NP mask planes per pod (4, or 8 on a sidecar handle).  The rounds engine (egs_rounds.cuh)
+// uses the (8, 4) instantiations only.
 #pragma once
 #include "egs_device.cuh"
 
@@ -21,7 +24,7 @@
 struct OptTable {            // option cache of ONE request shape (slot)
   uint8_t *st;               // [N_pad]  OPT_*
   int32_t *sc;               // [N_pad]  option.Score
-  uint8_t *al;               // [EGS_C][N_pad] MaskT<G> GPU mask per container (option.Allocated)
+  uint8_t *al;               // [NP][N_pad] MaskT<G> GPU mask per container (option.Allocated)
   size_t plane;              // N_pad
 };
 
@@ -29,28 +32,29 @@ struct Partial { unsigned long long key, fd, sd; int fit; int pad; };
 
 struct PodOut {              // per-pod outputs of the batch loop (device pointers, may be null)
   int32_t *node, *status, *fit_count;
-  uint8_t *alloc;            // [P][EGS_C] MaskT<G>
+  uint8_t *alloc;            // [P][NP] MaskT<G>
   unsigned long long *fit_digest, *score_digest;
 };
 
-// The six per-pod outputs of pod p; `masks` packs the EGS_C alloc masks of the pod (one MaskT<G> per container).
-template <int G>
+// The six per-pod outputs of pod p; `masks` packs the NP alloc masks of the pod (one MaskT<G> per container).
+template <int G, int NP = EGS_C>
 __device__ __forceinline__ void write_pod_out(const PodOut &o, int p, int node, int status, int fit, unsigned long long fd,
-                                              unsigned long long sd, PackedT<G> masks) {
-  static_assert(EGS_C * sizeof(MaskT<G>) == sizeof(PackedT<G>), "alloc row == one packed word");
+                                              unsigned long long sd, PackedT<G, NP> masks) {
+  static_assert(NP * sizeof(MaskT<G>) == sizeof(PackedT<G, NP>), "alloc row == one packed word");
   if (o.node) o.node[p] = node;
   if (o.status) o.status[p] = status;
   if (o.fit_count) o.fit_count[p] = fit;
   if (o.fit_digest) o.fit_digest[p] = fd;
   if (o.score_digest) o.score_digest[p] = sd;
-  if (o.alloc) reinterpret_cast<PackedT<G> *>(o.alloc)[p] = masks;
+  if (o.alloc) reinterpret_cast<PackedT<G, NP> *>(o.alloc)[p] = masks;
 }
 
-struct PassArgs {
+template <class R>
+struct PassArgsT {
   const int32_t *core, *mem, *mem_total;   // rows are written by the bind in the last block
   int32_t *core_w, *mem_w;
   int n, policy;
-  Req req;
+  R req;
   OptTable t;
   uint8_t *all_st; size_t slot_stride; int n_slots;   // every slot's state plane (UNFIT memo reset)
   uint8_t *vec_fit; int32_t *vec_score;    // optional full vectors
@@ -101,13 +105,13 @@ __device__ __forceinline__ void memo_reset(uint8_t *all_st, size_t slot_stride, 
 // (node.go:64-66); no entry -> Trade (node.go:67-71): the option is cached, or the failure memoised as UNFIT (the
 // reference caches nothing then and re-Trades with the same outcome).  Returns the state after Assume; `score` is
 // set when it is OPT_CACHED.  The fast Trade ignores mem_total, so SINGLE does not load it.
-template <int G, bool SINGLE>
+template <int G, bool SINGLE, class R>
 __device__ __forceinline__ uint8_t assume_option(const OptTable &t, size_t i, const int32_t *core, const int32_t *mem,
-                                                 const int32_t *mem_total, const Req &req, int policy, int &score) {
+                                                 const int32_t *mem_total, const R &req, int policy, int &score) {
   uint8_t st = t.st[i];
   if (st == OPT_CACHED) { score = t.sc[i]; return st; }
   if (st != OPT_ABSENT) return st;
-  int c[G], m[G]; PackedT<G> masks;
+  int c[G], m[G]; PackedT<G, R::NC> masks;
   load_row(core, mem, i, c, m);
   if (trade_any(c, m, SINGLE ? 0 : mem_total[i], req, SINGLE, policy, score, masks)) {
     st = OPT_CACHED;
@@ -121,20 +125,20 @@ __device__ __forceinline__ uint8_t assume_option(const OptTable &t, size_t i, co
 }
 
 // GPU masks of node w's option, one MaskT<G> per container.
-template <int G>
-__device__ __forceinline__ PackedT<G> option_masks(const OptTable &t, size_t w, int C) {
-  PackedT<G> masks = 0;
-  for (int c = 0; c < C; c++) masks |= (PackedT<G>)reinterpret_cast<const MaskT<G> *>(t.al)[(size_t)c * t.plane + w] << (G * c);
+template <int G, int NP = EGS_C>
+__device__ __forceinline__ PackedT<G, NP> option_masks(const OptTable &t, size_t w, int C) {
+  PackedT<G, NP> masks = 0;
+  for (int c = 0; c < C; c++) masks |= (PackedT<G, NP>)reinterpret_cast<const MaskT<G> *>(t.al)[(size_t)c * t.plane + w] << (G * c);
   return masks;
 }
 
 // NodeAllocator.Allocate (node.go:87-104) of node w's cached option; one thread.  The entry goes before the Transact
 // (deferred delete, node.go:90-92); the rows changed, so the node's UNFIT memos go too.
-template <int G>
+template <int G, class R>
 __device__ __forceinline__ int allocate_option(const OptTable &t, size_t w, int32_t *core, int32_t *mem, int mem_total,
-                                               const Req &req, uint8_t *all_st, size_t slot_stride, int n_slots,
-                                               PackedT<G> &masks) {
-  masks = option_masks<G>(t, w, req.C);
+                                               const R &req, uint8_t *all_st, size_t slot_stride, int n_slots,
+                                               PackedT<G, R::NC> &masks) {
+  masks = option_masks<G, R::NC>(t, w, req.C);
   t.st[w] = OPT_ABSENT;
   const bool ok = transact_row<G>(core + w * G, mem + w * G, mem_total, req, masks);
   memo_reset(all_st, slot_stride, n_slots, w);
@@ -147,8 +151,8 @@ __device__ __forceinline__ int allocate_option(const OptTable &t, size_t w, int3
 // --------------------------------------------------------------------------------------------
 // At G = 16 a minimum of one block per SM lifts ptxas's default 64-register cap, under which the 16-wide row spills
 // (70 / 80 registers without spills, sm_90a); 0 leaves the 8-wide instantiations exactly as they were.
-template <int G, bool SINGLE>
-__global__ void __launch_bounds__(PASS_THREADS, G > EGS_G ? 1 : 0) k_pass(PassArgs a) {
+template <int G, int NP, bool SINGLE>
+__global__ void __launch_bounds__(PASS_THREADS, G > EGS_G ? 1 : 0) k_pass(PassArgsT<ReqOf<NP>> a) {
   __shared__ Partial sm[PASS_THREADS / 32];
   __shared__ bool is_last;
   const int i = blockIdx.x * PASS_THREADS + threadIdx.x;
@@ -182,14 +186,14 @@ __global__ void __launch_bounds__(PASS_THREADS, G > EGS_G ? 1 : 0) k_pass(PassAr
   if (threadIdx.x == 0) {
     *a.ticket = 0;
     int node = -1, status = EGS_ERR_NOFIT;
-    PackedT<G> masks = 0;
+    PackedT<G, NP> masks = 0;
     if (key != 0) {
       node = (int)key_node(key);
       status = allocate_option<G>(a.t, (size_t)node, a.core_w, a.mem_w, a.mem_total[node], a.req, a.all_st, a.slot_stride,
                                a.n_slots, masks);
       if (status != EGS_OK) masks = 0;
     }
-    write_pod_out<G>(a.out, a.pod, node, status, fit, fd, sd, masks);
+    write_pod_out<G, NP>(a.out, a.pod, node, status, fit, fd, sd, masks);
   }
 }
 
@@ -234,18 +238,19 @@ __global__ void __launch_bounds__(256) k_evaluate(EvalArgs a) {
 // --------------------------------------------------------------------------------------------
 // verbs over an explicit candidate list (ids == nullptr -> identity)
 // --------------------------------------------------------------------------------------------
-struct GatherArgs {
+template <class R>
+struct GatherArgsT {
   const int32_t *core, *mem, *mem_total;
   int n, n_nodes, policy;
-  Req req;
+  R req;
   OptTable t;
   const int32_t *ids;
   uint8_t *out_fit; int32_t *out_score; int *panic_flag;
 };
 
 // Assume per node (node.go:61-73)
-template <int G, bool SINGLE>
-__global__ void __launch_bounds__(256) k_gather_filter(GatherArgs a) {
+template <int G, int NP, bool SINGLE>
+__global__ void __launch_bounds__(256) k_gather_filter(GatherArgsT<ReqOf<NP>> a) {
   const int j = blockIdx.x * 256 + threadIdx.x;
   if (j >= a.n) return;
   const int i = a.ids ? a.ids[j] : j;
@@ -256,8 +261,8 @@ __global__ void __launch_bounds__(256) k_gather_filter(GatherArgs a) {
 
 // Score per node (node.go:75-85): cached score; no entry -> Assume; fails -> 0, succeeds -> the
 // reference dereferences nil (panic) -- flagged.
-template <int G, bool SINGLE>
-__global__ void __launch_bounds__(256) k_gather_score(GatherArgs a) {
+template <int G, int NP, bool SINGLE>
+__global__ void __launch_bounds__(256) k_gather_score(GatherArgsT<ReqOf<NP>> a) {
   const int j = blockIdx.x * 256 + threadIdx.x;
   if (j >= a.n) return;
   const int i = a.ids ? a.ids[j] : j;
@@ -268,26 +273,27 @@ __global__ void __launch_bounds__(256) k_gather_score(GatherArgs a) {
   a.out_score[j] = 0;
 }
 
-struct BindArgs {
+template <class R>
+struct BindArgsT {
   int32_t *core, *mem; const int32_t *mem_total;
-  int node; Req req; OptTable t;
+  int node; R req; OptTable t;
   uint8_t *all_st; size_t slot_stride; int n_slots;
   int skip_transact;          // uid already in the node's podsMap (node.go:149)
   int consume;                // 1: Bind (delete the entry); 0: peek
-  int32_t *result;            // [0] had entry, [1] status, [2] masks (low 32 bits), [3] score, [4] masks >> 32 (G = 16)
+  int32_t *result;            // [0] had entry, [1] status, [2] masks (low 32 bits), [3] score, [4] masks >> 32 (64-bit word)
 };
-template <int G>
-__global__ void k_bind(BindArgs a) {
+template <int G, int NP>
+__global__ void k_bind(BindArgsT<ReqOf<NP>> a) {
   const size_t w = (size_t)a.node;
   const bool had = a.t.st[w] == OPT_CACHED;
-  PackedT<G> masks = 0; int status = EGS_ERR_NO_OPTION, score = 0;
+  PackedT<G, NP> masks = 0; int status = EGS_ERR_NO_OPTION, score = 0;
   if (had) {
     score = a.t.sc[w];
     status = EGS_OK;
     if (a.consume && !a.skip_transact) {
       status = allocate_option<G>(a.t, w, a.core, a.mem, a.mem_total[w], a.req, a.all_st, a.slot_stride, a.n_slots, masks);
     } else {                                     // peek, or Bind of a known uid (node.go:149): the entry goes, rows stay
-      masks = option_masks<G>(a.t, w, a.req.C);
+      masks = option_masks<G, NP>(a.t, w, a.req.C);
       if (a.consume) a.t.st[w] = OPT_ABSENT;
     }
   }
@@ -337,4 +343,107 @@ __global__ void k_node_reset(uint8_t *all_st, size_t slot_stride, int n_slots, i
     uint8_t *p = all_st + (size_t)s * slot_stride + node0 + i;
     if (full || *p == OPT_UNFIT) *p = OPT_ABSENT;
   }
+}
+
+// --------------------------------------------------------------------------------------------
+// Leaf-split Trade (sidecar handles, geometry (8, 8)): the Trade of every node whose option is absent, with the leaf
+// space of each node (trade_leaf_eval: one digit per branching container, `bits` wide) cut into chunks of LEAF_CHUNK
+// leaves spread over the whole GPU.  Three launches on the handle's stream, no host synchronisation:
+//   k_trade_probe  : candidates whose state is OPT_ABSENT go to a miss list (count on the device); with out_score it
+//                    is also Score's read of the cache (cached score, else 0).
+//   k_trade_leaves : grid-strides over (miss, tile of LEAF_THREADS chunks); each thread walks its chunk in leaf order,
+//                    skipping every leaf whose prefix is already infeasible; one 64-bit atomicMax per CTA and miss on
+//                    key = score << 32 | (leaf + 1), so key 0 is "no feasible leaf" and the max over keys is "the last
+//                    maximal leaf wins" (gpu.go:85).  Scores stay below 2^31: each of up to 8 sentinel units adds 1
+//                    to a GPU, so range <= (2^25 + 8 + 2^20 + 8) / 2 < 2^24.1 and range * 100 < 2^30.8.
+//   k_trade_commit : decodes each miss's winning leaf into its masks and caches the option, or memoises OPT_UNFIT.
+// --------------------------------------------------------------------------------------------
+#define LEAF_THREADS 256
+#define LEAF_CHUNK 64
+
+struct LeafArgs {
+  const int32_t *core, *mem, *mem_total;
+  int policy, bits, nbranch, tiles;         // tiles: ceil(nleaf / (LEAF_THREADS * LEAF_CHUNK)) per miss
+  ReqW req;
+  int32_t *miss; unsigned int *n_miss; unsigned long long *keys;
+};
+
+struct ProbeArgs {
+  const uint8_t *st; const int32_t *sc;
+  const int32_t *ids; int n, n_nodes;       // ids == nullptr -> identity
+  int32_t *miss; unsigned int *n_miss; unsigned long long *keys;
+  int32_t *out_score;                       // optional: Score's reads (node.go:75-85)
+};
+
+__global__ void __launch_bounds__(256) k_trade_probe(ProbeArgs a) {
+  const int j = blockIdx.x * 256 + threadIdx.x;
+  const int i = j < a.n ? (a.ids ? a.ids[j] : j) : -1;
+  const bool valid = i >= 0 && i < a.n_nodes;
+  const uint8_t st = valid ? a.st[i] : (uint8_t)OPT_UNFIT;
+  if (a.out_score && j < a.n) a.out_score[j] = st == OPT_CACHED ? a.sc[i] : 0;
+  const bool miss = st == OPT_ABSENT;
+  const unsigned b = __ballot_sync(0xffffffffu, miss);       // one atomic per warp
+  if (!b) return;
+  const int lane = threadIdx.x & 31, lead = __ffs(b) - 1;
+  unsigned base = 0;
+  if (lane == lead) base = atomicAdd(a.n_miss, (unsigned)__popc(b));
+  base = __shfl_sync(0xffffffffu, base, lead);
+  if (miss) {
+    const unsigned m = base + __popc(b & ((1u << lane) - 1u));
+    a.miss[m] = i; a.keys[m] = 0ull;
+  }
+}
+
+__global__ void __launch_bounds__(LEAF_THREADS) k_trade_leaves(LeafArgs a) {
+  __shared__ unsigned long long sm[LEAF_THREADS / 32];
+  const unsigned long long items = (unsigned long long)*a.n_miss * (unsigned)a.tiles;
+  const int nleaf = 1 << (a.bits * a.nbranch);
+  for (unsigned long long t = blockIdx.x; t < items; t += gridDim.x) {
+    const int m = (int)(t / (unsigned)a.tiles), tile = (int)(t % (unsigned)a.tiles);
+    const size_t node = (size_t)a.miss[m];
+    int c[EGS_G], mm[EGS_G];
+    load_row(a.core, a.mem, node, c, mm);
+    const int mt = a.mem_total[node];
+    int leaf = (tile * LEAF_THREADS + (int)threadIdx.x) * LEAF_CHUNK;
+    const int end = EGS_MIN(leaf + LEAF_CHUNK, nleaf);
+    unsigned long long best = 0;
+    while (leaf < end) {
+      uint64_t mk; int fail;
+      const int s = trade_leaf_eval(c, mm, mt, a.req, a.policy, a.bits, a.nbranch, leaf, mk, &fail);
+      if (s >= 0) {
+        const unsigned long long key = ((unsigned long long)(uint32_t)s << 32) | (unsigned)(leaf + 1);
+        best = key > best ? key : best;
+        leaf++;
+      } else {
+        leaf = trade_leaf_next(leaf, fail, a.bits, a.nbranch);
+      }
+    }
+    best = warp_max_u64(best);
+    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = best;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+      best = threadIdx.x < LEAF_THREADS / 32 ? sm[threadIdx.x] : 0ull;
+      best = warp_max_u64(best);
+      if (threadIdx.x == 0 && best) atomicMax(a.keys + m, best);
+    }
+    __syncthreads();
+  }
+}
+
+// One thread per miss.  panic_flag (Score): a node that had no entry and fits is the reference's nil-option panic.
+__global__ void __launch_bounds__(256) k_trade_commit(LeafArgs a, OptTable t, int *panic_flag) {
+  const int m = blockIdx.x * 256 + threadIdx.x;
+  if (m >= (int)*a.n_miss) return;
+  const size_t node = (size_t)a.miss[m];
+  const unsigned long long key = a.keys[m];
+  if (!key) { t.st[node] = OPT_UNFIT; return; }
+  int c[EGS_G], mm[EGS_G];
+  load_row(a.core, a.mem, node, c, mm);
+  uint64_t masks = 0;
+  const int leaf = (int)(uint32_t)key - 1;
+  trade_leaf_eval(c, mm, a.mem_total[node], a.req, a.policy, a.bits, a.nbranch, leaf, masks);
+  t.sc[node] = (int32_t)(key >> 32);
+  for (int k = 0; k < a.req.C; k++) t.al[(size_t)k * t.plane + node] = (uint8_t)(masks >> (EGS_G * k));
+  t.st[node] = OPT_CACHED;
+  if (panic_flag) *panic_flag = 1;
 }

@@ -18,15 +18,16 @@ static const char *ret(HostCtx *c, const std::string &s) { c->buf = s; return c-
 
 extern "C" {
 
-// g_max: the widest node (EGS_MAX_GPUS, or up to EGS_MAX_GPUS_WIDE)
-void *egsh_create(int policy, int max_nodes, int device, int g_max) {
+// g_max: the widest node (EGS_MAX_GPUS, or up to EGS_MAX_GPUS_WIDE); c_max: the widest pod Assume / Score / Bind
+// place (EGS_MAX_CONTAINERS, or up to EGS_MAX_CONTAINERS_APPLY).  The extender routes (egsr_*) use this scheduler.
+void *egsh_create(int policy, int max_nodes, int device, int g_max, int c_max) {
   HostCtx *c = new HostCtx();
   c->sch = new CudaUnitScheduler(policy, max_nodes, device, [c](const std::string &name, NodeInfo *out) -> std::string {
     auto it = c->cluster.find(name);
     if (it == c->cluster.end()) return "nodes \"" + name + "\" not found";
     *out = it->second;
     return "";
-  }, g_max);
+  }, g_max, c_max);
   if (!c->sch->ok()) { delete c->sch; delete c; return nullptr; }
   return c;
 }

@@ -14,9 +14,14 @@ static int64_t requestOf(const Container &c, const char *key) {   // GetGPUCoreF
   return it == c.requests.end() ? 0 : it->second;
 }
 
-CudaUnitScheduler::CudaUnitScheduler(int policy, int max_nodes, int device, NodeProvider provider, int g_max)
-    : max_nodes_(max_nodes), g_max_(g_max), provider_(std::move(provider)) {
-  if (egs_create(policy, max_nodes, g_max, device, &h_) != EGS_OK) h_ = nullptr;
+CudaUnitScheduler::CudaUnitScheduler(int policy, int max_nodes, int device, NodeProvider provider, int g_max, int c_max)
+    : max_nodes_(max_nodes), g_max_(g_max), c_max_(c_max < EGS_MAX_CONTAINERS ? EGS_MAX_CONTAINERS : c_max),
+      provider_(std::move(provider)) {
+  if (egs_create_ex(policy, max_nodes, g_max, c_max, device, &h_) != EGS_OK) h_ = nullptr;
+}
+
+std::string CudaUnitScheduler::tooWide() const {
+  return "libegs: pods with more than " + std::to_string(c_max_) + " containers are not supported by the device path";
 }
 
 // The GPU ids of container c's mask (EGS_MASK_BYTES(g_max) little-endian bytes at masks[c * EGS_MASK_BYTES]), joined.
@@ -38,7 +43,7 @@ bool CudaUnitScheduler::Handles(const Pod &pod) {
   return false;
 }
 
-// max_containers: EGS_MAX_CONTAINERS for the verbs that Trade (Assume / Score / Bind), EGS_MAX_CONTAINERS_APPLY for the
+// max_containers: c_max for the verbs that Trade (Assume / Score / Bind), EGS_MAX_CONTAINERS_APPLY for the
 // ones that only account a pod somebody placed (AddPod / ForgetPod / replay)
 bool CudaUnitScheduler::RequestOf(const Pod &pod, std::vector<egs_unit> *out, size_t max_containers) {
   out->clear();
@@ -117,7 +122,7 @@ std::string CudaUnitScheduler::Assume(const std::vector<std::string> &nodes, con
   filtered->clear();
   failed->clear();
   std::vector<egs_unit> req;
-  if (!RequestOf(pod, &req)) return "libegs: pods with more than 4 containers are not supported by the device path";
+  if (!RequestOf(pod, &req, c_max_)) return tooWide();
   std::vector<int32_t> ids(nodes.size(), -1);
   std::vector<std::string> load_err(nodes.size());
   for (size_t i = 0; i < nodes.size(); i++) ids[i] = getNodeInfo(nodes[i], &load_err[i]);   // scheduler.go:119-127
@@ -135,7 +140,7 @@ std::string CudaUnitScheduler::Assume(const std::vector<std::string> &nodes, con
 std::vector<int64_t> CudaUnitScheduler::Score(const std::vector<std::string> &nodes, const Pod &pod) {
   std::vector<int64_t> out(nodes.size(), 0);
   std::vector<egs_unit> req;
-  if (!RequestOf(pod, &req)) return out;
+  if (!RequestOf(pod, &req, c_max_)) return out;
   std::vector<int32_t> ids(nodes.size(), -1), sc(nodes.size() + 1, 0);
   std::string err;
   for (size_t i = 0; i < nodes.size(); i++) ids[i] = getNodeInfo(nodes[i], &err);            // error -> ScoreMin (scheduler.go:176-179)
@@ -161,10 +166,10 @@ std::string CudaUnitScheduler::Bind(const std::string &node, Pod *pod) {
   int id = getNodeInfo(node, &err);
   if (id < 0) return err;                                                                     // scheduler.go:190-193
   std::vector<egs_unit> req;
-  if (!RequestOf(*pod, &req)) return "libegs: pods with more than 4 containers are not supported by the device path";
-  uint8_t masks[2 * EGS_MAX_CONTAINERS] = {};                  // room for EGS_MASK_BYTES <= 2
+  if (!RequestOf(*pod, &req, c_max_)) return tooWide();
+  uint8_t masks[2 * EGS_MAX_CONTAINERS_APPLY] = {};            // room for EGS_MASKS_PER_POD <= 8 masks of EGS_MASK_BYTES <= 2
   // option text for the Transact error has to be read before the entry is consumed
-  int32_t valid = 0, score = 0; uint8_t pm[2 * EGS_MAX_CONTAINERS] = {};
+  int32_t valid = 0, score = 0; uint8_t pm[2 * EGS_MAX_CONTAINERS_APPLY] = {};
   egs_option_peek(h_, id, (int)req.size(), req.data(), &valid, &score, pm);
   const std::string gpus_before = gpusJson(id);
   int st = egs_bind(h_, id, (int)req.size(), req.data(), uidOf(pod->uid), masks);

@@ -57,8 +57,11 @@ class ResourceScheduler {                // scheduler.go:30-39 (errors are "" fo
 class CudaUnitScheduler : public ResourceScheduler {
  public:
   // policy: EGS_BINPACK / EGS_SPREAD (cmd/main.go:45-54); max_nodes bounds the dense node-id space; g_max is the widest
-  // node (egs_create): EGS_MAX_GPUS, or up to EGS_MAX_GPUS_WIDE for servers with more GPUs
-  CudaUnitScheduler(int policy, int max_nodes, int device, NodeProvider provider, int g_max = EGS_MAX_GPUS);
+  // node (egs_create): EGS_MAX_GPUS, or up to EGS_MAX_GPUS_WIDE for servers with more GPUs; c_max is the widest pod
+  // Assume / Score / Bind place (egs_create_ex): EGS_MAX_CONTAINERS, or up to EGS_MAX_CONTAINERS_APPLY for pods with
+  // sidecars (g_max <= EGS_MAX_GPUS then)
+  CudaUnitScheduler(int policy, int max_nodes, int device, NodeProvider provider, int g_max = EGS_MAX_GPUS,
+                    int c_max = EGS_MAX_CONTAINERS);
   ~CudaUnitScheduler() override;
   bool ok() const { return h_ != nullptr; }
 
@@ -84,11 +87,13 @@ class CudaUnitScheduler : public ResourceScheduler {
   static uint64_t uidOf(const std::string &uid);
   std::string gpusJson(int node_id);                            // GPUs.String (gpu.go:60-63)
   std::string gpuList(const uint8_t *masks, size_t c, const char *sep) const;   // GPU ids of container c's mask
+  std::string tooWide() const;                                  // the error of a pod wider than c_max
   static void optionFromPod(const Pod &pod, std::vector<int32_t> *off, std::vector<int32_t> *idx);  // allocate.go:75-93
 
   egs_handle *h_ = nullptr;
   int max_nodes_;
   int g_max_;
+  int c_max_;                                                   // widest pod the Trade verbs take
   NodeProvider provider_;
   std::unordered_map<std::string, int> node_ids_;
   std::vector<std::string> node_names_;

@@ -3,6 +3,8 @@
 // source the GPU runs against the oracle (tests/test_device_arith_host.py).  Not part of libegs.
 #include "../egs_device.cuh"
 
+#include <vector>
+
 template <int G>
 static void rows(const int32_t *core, const int32_t *mem, int (&c)[G], int (&m)[G]) {
   for (int g = 0; g < G; g++) { c[g] = core[g]; m[g] = mem[g]; }
@@ -94,6 +96,73 @@ int egsdh_apply(int32_t *core, int32_t *mem, int mem_total, int C, const egs_uni
 int egsdh_apply16(int32_t *core, int32_t *mem, int mem_total, int C, const egs_unit *units, const int32_t *n_idx,
                   const int32_t *idx, int cancel) {
   return apply_w<16>(core, mem, mem_total, C, units, n_idx, idx, cancel);
+}
+// The general DFS Trade at geometry (8, 8) -- a sidecar handle's one-thread Trade -- for C <= 8 containers: masks
+// are 8 x u8.  path as in egsdh_trade.
+int egsdh_trade8c(const int32_t *core, const int32_t *mem, int mem_total, int C, const egs_unit *units, int policy,
+                  int path, int32_t *score, uint64_t *masks) {
+  int c[EGS_G], m[EGS_G];
+  rows(core, mem, c, m);
+  const ReqW r = make_req<ReqW>(C, units);
+  const bool single = path == 0 && C == 1 && r.cnt[0] == 0 && r.core[0] >= 0 && r.mem[0] >= 0;
+  int sc = 0; PackedT<EGS_G, EGS_CA> mk = 0;
+  const bool ok = trade_any(c, m, mem_total, r, single, policy, sc, mk);
+  *score = sc; *masks = mk;
+  return ok ? 1 : 0;
+}
+// The leaf-split Trade's reduction (k_trade_leaves + k_trade_commit) for C <= 8 containers, serially: the leaf space
+// of digit width `bits` is cut into chunks of `chunk` leaves, the chunks are walked in the order of a Fisher-Yates
+// shuffle drawn from `seed`, each chunk in leaf order with the kernel's pruning, and the 64-bit keys are max-reduced;
+// the winner is decoded as the commit decodes it.  *n_eval: leaves evaluated (pruned ones are not).
+int egsdh_trade_split(const int32_t *core, const int32_t *mem, int mem_total, int C, const egs_unit *units, int policy,
+                      int bits, int chunk, uint64_t seed, int32_t *score, uint64_t *masks, int64_t *n_eval) {
+  int c[EGS_G], m[EGS_G];
+  rows(core, mem, c, m);
+  const ReqW r = make_req<ReqW>(C, units);
+  int nbranch = 0;
+  for (int i = 0; i < C; i++) nbranch += r.cnt[i] > 0 ? 0 : 1;
+  const int nleaf = 1 << (bits * nbranch), nchunk = (nleaf + chunk - 1) / chunk;
+  std::vector<int> order(nchunk);
+  for (int k = 0; k < nchunk; k++) order[k] = k;
+  for (int k = nchunk - 1; k > 0; k--) std::swap(order[k], order[mix64(seed ^ (uint64_t)k) % (uint64_t)(k + 1)]);
+  unsigned long long best = 0; int64_t ev = 0;
+  for (int k : order) {
+    int leaf = k * chunk;
+    const int end = std::min(leaf + chunk, nleaf);
+    while (leaf < end) {
+      uint64_t mk; int fail;
+      const int s = trade_leaf_eval(c, m, mem_total, r, policy, bits, nbranch, leaf, mk, &fail);
+      ev++;
+      if (s >= 0) {
+        const unsigned long long key = ((unsigned long long)(uint32_t)s << 32) | (unsigned)(leaf + 1);
+        best = std::max(best, key);
+        leaf++;
+      } else {
+        leaf = trade_leaf_next(leaf, fail, bits, nbranch);
+      }
+    }
+  }
+  *n_eval = ev;
+  if (!best) return 0;
+  uint64_t mk = 0;
+  trade_leaf_eval(c, m, mem_total, r, policy, bits, nbranch, (int)(uint32_t)best - 1, mk);
+  *score = (int32_t)(best >> 32); *masks = mk;
+  return 1;
+}
+// One leaf through both leaf evaluations: the resolver's (Req, 32-bit masks) and the leaf-split Trade's template (ReqW,
+// 64-bit masks), for C <= EGS_MAX_CONTAINERS.  The two are separate definitions and must agree leaf for leaf.
+void egsdh_leaf_eval_both(const int32_t *core, const int32_t *mem, int mem_total, int C, const egs_unit *units,
+                          int policy, int bits, int leaf, int32_t *s4, uint32_t *m4, int32_t *s8, uint64_t *m8) {
+  int c[EGS_G], m[EGS_G];
+  rows(core, mem, c, m);
+  const Req r = make_req(C, units);
+  const ReqW rw = make_req<ReqW>(C, units);
+  int nbranch = 0;
+  for (int i = 0; i < C; i++) nbranch += r.cnt[i] > 0 ? 0 : 1;
+  uint32_t a = 0; uint64_t b = 0;
+  *s4 = trade_leaf_eval(c, m, mem_total, r, policy, bits, nbranch, leaf, a);
+  *s8 = trade_leaf_eval(c, m, mem_total, rw, policy, bits, nbranch, leaf, b);
+  *m4 = *s4 >= 0 ? a : 0; *m8 = *s8 >= 0 ? b : 0;
 }
 int egsdh_is_single(int C, const egs_unit *units) { const Req r = make_req(C, units); return req_is_single(r) ? 1 : 0; }
 unsigned long long egsdh_cand_key(int32_t score, uint32_t node) { return cand_key(score, node); }

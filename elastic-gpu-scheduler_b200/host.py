@@ -6,7 +6,7 @@ import ctypes as C
 from typing import Dict, List, Optional, Sequence, Tuple
 
 from . import _build
-from .capi import EGS_MAX_GPUS
+from .capi import EGS_MAX_CONTAINERS, EGS_MAX_GPUS
 
 _lib = None
 
@@ -16,7 +16,7 @@ def _load():
     if _lib is None:
         L = C.CDLL(_build.build_host())
         vp, cp, i64 = C.c_void_p, C.c_char_p, C.c_int64
-        L.egsh_create.restype = vp; L.egsh_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
+        L.egsh_create.restype = vp; L.egsh_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
         L.egsh_destroy.argtypes = [vp]
         L.egsh_register_node.argtypes = [vp, cp, i64, i64]
         L.egsh_register_assumed_pod.argtypes = [vp, cp, vp]
@@ -67,10 +67,12 @@ class Pod:
 
 
 class CudaUnitScheduler:
-    def __init__(self, policy: int, max_nodes: int = 1024, device: int = 0, g_max: int = EGS_MAX_GPUS):
-        """g_max: the widest node; above EGS_MAX_GPUS (up to 16) the handle is wide."""
+    def __init__(self, policy: int, max_nodes: int = 1024, device: int = 0, g_max: int = EGS_MAX_GPUS,
+                 c_max: int = EGS_MAX_CONTAINERS):
+        """g_max: the widest node; above EGS_MAX_GPUS (up to 16) the handle is wide.  c_max: the widest pod Assume /
+        Score / Bind place; above EGS_MAX_CONTAINERS (up to 8, with g_max <= 8) the handle is a sidecar handle."""
         self.L = _load()
-        self.h = self.L.egsh_create(policy, max_nodes, device, g_max)
+        self.h = self.L.egsh_create(policy, max_nodes, device, g_max, c_max)
         if not self.h:
             raise RuntimeError("egsh_create failed (no CUDA device?)")
 

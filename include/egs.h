@@ -23,8 +23,8 @@
  *   free_core[N][W], free_mem[N][W], mem_total[N]      W = EGS_ROW_WIDTH(g_max)
  * (CoreTotal == 100 for every GPU, pkg/utils/types.go:6) plus, per interned
  * request shape s, the per-node option cache of node.go:19
- *   opt_state[s][N] (u8), opt_score[s][N] (i32), opt_alloc[s][c][N] (GPU mask of container c, c < 4,
- *   EGS_MASK_BYTES(g_max) bytes).
+ *   opt_state[s][N] (u8), opt_score[s][N] (i32), opt_alloc[s][c][N] (GPU mask of container c,
+ *   c < EGS_MASKS_PER_POD(c_max), EGS_MASK_BYTES(g_max) bytes).
  *
  * The INTEGRATION.md at the repo root shows the cgo binding.
  */
@@ -39,20 +39,25 @@ extern "C" {
 
 #define EGS_MAX_GPUS        8      /* GPUs per node the SoA row of a handle with g_max <= 8 holds; width of egs_mutation */
 #define EGS_MAX_GPUS_WIDE   16     /* widest node any handle takes (a "wide" handle: 9 <= g_max <= 16)                */
-#define EGS_MAX_CONTAINERS  4      /* containers per pod the filter / score / bind path enumerates */
-#define EGS_MAX_CONTAINERS_APPLY 8 /* containers per pod AddPod / ForgetPod / replay account (sidecars count) */
+#define EGS_MAX_CONTAINERS  4      /* containers per pod filter / score / bind take on a handle of egs_create */
+#define EGS_MAX_CONTAINERS_APPLY 8 /* containers per pod AddPod / ForgetPod / replay account (sidecars count), and
+                                      the largest pod a sidecar handle (egs_create_ex, c_max > 4) schedules */
 #define EGS_CORE_PER_GPU    100    /* utils.GPUCoreEachCard, pkg/utils/types.go:6          */
 #define EGS_MAX_MEM_PER_GPU (1 << 25) /* int32 guard: Range/(k+1)*100 must fit int32 (Go int is 64-bit) */
 #define EGS_MAX_CORE_LOAD   (1 << 20) /* bound for free_core values given to egs_state_load */
 
-/* Layout of a handle created with `g_max` GPUs per node -- the one rule every row and mask buffer below follows:
- *   EGS_ROW_WIDTH(g_max)  int32 cells per node row (egs_state_dump): 8, or 16 on a wide handle;
- *   EGS_MASK_BYTES(g_max) bytes per GPU mask, little endian, bit g = GPU g: 1, or 2 on a wide handle.
+/* Layout of a handle created with `g_max` GPUs per node and pods of up to `c_max` containers (c_max ==
+ * EGS_MAX_CONTAINERS for egs_create) -- the one rule every row and mask buffer below follows:
+ *   EGS_ROW_WIDTH(g_max)     int32 cells per node row (egs_state_dump): 8, or 16 on a wide handle;
+ *   EGS_MASK_BYTES(g_max)    bytes per GPU mask, little endian, bit g = GPU g: 1, or 2 on a wide handle;
+ *   EGS_MASKS_PER_POD(c_max) GPU masks per pod / node: 4, or 8 on a sidecar handle.
  * Every GPU mask output (egs_bind, egs_option_peek, egs_option_dump and out_alloc_mask of the egs_schedule_batch*
- * calls) holds EGS_MAX_CONTAINERS masks per pod / node: element (p, c) starts at byte
- * (p*EGS_MAX_CONTAINERS + c) * EGS_MASK_BYTES(g_max).  For g_max <= 8 this is one u8 per container, as always. */
+ * calls) holds EGS_MASKS_PER_POD(c_max) masks per pod / node, of which the first n_containers are meaningful (the
+ * rest read 0): element (p, c) starts at byte (p*EGS_MASKS_PER_POD(c_max) + c) * EGS_MASK_BYTES(g_max).  On a handle
+ * of egs_create this is EGS_MAX_CONTAINERS masks per pod, of one u8 each for g_max <= 8, as always. */
 #define EGS_ROW_WIDTH(g_max)  ((g_max) > EGS_MAX_GPUS ? EGS_MAX_GPUS_WIDE : EGS_MAX_GPUS)
 #define EGS_MASK_BYTES(g_max) ((g_max) > EGS_MAX_GPUS ? 2 : 1)
+#define EGS_MASKS_PER_POD(c_max) ((c_max) > EGS_MAX_CONTAINERS ? EGS_MAX_CONTAINERS_APPLY : EGS_MAX_CONTAINERS)
 
 /* -priority flag, cmd/main.go:45-54 */
 enum egs_policy { EGS_BINPACK = 0, EGS_SPREAD = 1 };
@@ -87,6 +92,18 @@ typedef struct egs_handle egs_handle;
  *   - a mutation record still lists at most EGS_MAX_GPUS indices per container: a whole-GPU container of more
  *     than 8 GPUs goes through egs_pod_apply / egs_node_replay_pod / egs_pod_cancel, whose lists take up to 16. */
 int egs_create(int policy, int max_nodes, int g_max, int device, egs_handle **out);
+/* egs_create for pods of up to `c_max` containers, 1 <= c_max <= EGS_MAX_CONTAINERS_APPLY (else EGS_ERR_BAD_ARG).
+ * c_max <= EGS_MAX_CONTAINERS gives the handle egs_create gives.  5 <= c_max <= 8 gives a "sidecar" handle: filter,
+ * score, bind, peek and egs_option_dump take 1..c_max containers -- a container without a GPU request is the sentinel
+ * unit {-1,-1,0} and Trade tries it on every GPU, as the reference does -- and every mask output holds 8 masks per
+ * pod (EGS_MASKS_PER_POD).  Its limits, each refused with EGS_ERR_BAD_ARG and an egs_last_error text:
+ *   - its batch engine is the per-pod engine: EGS_MODE_AUTO runs EGS_MODE_RESCAN, EGS_MODE_ROUNDS is refused
+ *     and applies nothing (also no record of egs_schedule_batch_mut);
+ *   - egs_shard_set is refused;
+ *   - egs_profile_evaluate takes at most EGS_MAX_CONTAINERS containers.
+ * g_max > EGS_MAX_GPUS together with c_max > EGS_MAX_CONTAINERS is refused (EGS_ERR_BAD_ARG, no handle).
+ * egs_mutation and the accounting verbs are the same on every handle. */
+int egs_create_ex(int policy, int max_nodes, int g_max, int c_max, int device, egs_handle **out);
 int egs_destroy(egs_handle *h);
 const char *egs_last_error(egs_handle *h);
 const char *egs_status_string(int status);        /* exact reference message where one exists */
@@ -216,7 +233,8 @@ int egs_pod_released(egs_handle *h, uint64_t uid);   /* 1 / 0, scheduler.go:276-
 /* ---- batch decision loop (device resident) ---------------------------------- */
 
 /* Limits of the device path: nodes with at most EGS_MAX_GPUS_WIDE GPUs (more than EGS_MAX_GPUS only on a wide
- * handle, see egs_create), pods with at most EGS_MAX_CONTAINERS containers, per-GPU memory units
+ * handle, see egs_create), pods with at most EGS_MAX_CONTAINERS containers (EGS_MAX_CONTAINERS_APPLY on a sidecar
+ * handle, see egs_create_ex), per-GPU memory units
  * <= EGS_MAX_MEM_PER_GPU (use MiB, not bytes).
  * Anything beyond is refused with EGS_ERR_BAD_ARG / EGS_ERR_OVERFLOW_GUARD -- never computed differently.
  *
@@ -228,7 +246,7 @@ int egs_pod_released(egs_handle *h, uint64_t uid);   /* 1 / 0, scheduler.go:276-
  * Outputs (host pointers, any may be NULL):
  *   out_node[p]        winner node id, -1 when no node fits
  *   out_status[p]      EGS_OK / EGS_ERR_NOFIT / EGS_ERR_TRANSACT
- *   out_alloc_mask     mask (p, c) at byte (p*EGS_MAX_CONTAINERS + c) * EGS_MASK_BYTES(g_max)
+ *   out_alloc_mask     mask (p, c) at byte (p*EGS_MASKS_PER_POD(c_max) + c) * EGS_MASK_BYTES(g_max)
  *   out_fit_count[p]   number of fit nodes
  *   out_fit_digest[p]  sum over fit nodes of egs_mix64(2*node+1)                       (mod 2^64)
  *   out_score_digest[p] sum over fit nodes of egs_mix64(2*node+2) * (2*(u64)(u32)score + 1)             (mod 2^64)
@@ -238,8 +256,8 @@ int egs_pod_released(egs_handle *h, uint64_t uid);   /* 1 / 0, scheduler.go:276-
  * podsMap); otherwise they must be pairwise distinct and not yet known (EGS_ERR_BAD_ARG).  A bind that
  * reaches NodeAllocator.Add records the uid in that node's podsMap even when Transact fails (node.go:150);
  * only a successful bind enters podMaps (scheduler.go:224) -- visible through egs_pod_known.
- * EGS_MODE_AUTO == EGS_MODE_ROUNDS on a handle with g_max <= EGS_MAX_GPUS, EGS_MODE_RESCAN on a wide handle
- * (which refuses EGS_MODE_ROUNDS).  Both modes produce identical outputs; RESCAN is the literal
+ * EGS_MODE_AUTO == EGS_MODE_ROUNDS on a handle of egs_create with g_max <= EGS_MAX_GPUS, EGS_MODE_RESCAN on a
+ * wide or sidecar handle (which refuse EGS_MODE_ROUNDS).  Both modes produce identical outputs; RESCAN is the literal
  * one-pass-per-pod form (single shard only), ROUNDS the fast exact form (DESIGN.md 3).
  */
 enum egs_batch_mode {
@@ -263,8 +281,8 @@ int egs_schedule_batch_vec(egs_handle *h, int n_pods, const int32_t *c_off, cons
 
 /* Same loop with every buffer already in device memory (bench `value` leg):
  * d_* are device pointers on the handle's device, laid out as above.  Each pod's masks are stored as one word of
- * EGS_MAX_CONTAINERS * EGS_MASK_BYTES(g_max) bytes, so d_out_alloc_mask must be aligned to that size (4 bytes, or 8 on
- * a wide handle; cudaMalloc memory always is): EGS_ERR_BAD_ARG otherwise. */
+ * EGS_MASKS_PER_POD(c_max) * EGS_MASK_BYTES(g_max) bytes, so d_out_alloc_mask must be aligned to that size (4 bytes,
+ * or 8 on a wide or sidecar handle; cudaMalloc memory always is): EGS_ERR_BAD_ARG otherwise. */
 int egs_schedule_batch_device(egs_handle *h, int mode, int n_pods, const int32_t *h_c_off,
                               const egs_unit *h_units,
                               int32_t *d_out_node, int32_t *d_out_status, uint8_t *d_out_alloc_mask,

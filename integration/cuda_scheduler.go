@@ -57,13 +57,16 @@ type CudaUnitScheduler struct {
 	nodeErr  map[string]error // nodes whose NodeAllocator could not be built (node.go:28-30)
 	maxNodes int
 	gMax     int // widest node the handle takes (egs_create's g_max): rows and masks are laid out for it
+	cMax     int // widest pod Assume / Score / Bind place (egs_create_ex's c_max)
 }
 
 // NewCudaUnitScheduler mirrors NewGPUUnitScheduler (scheduler.go:86-106): nodes that already carry assumed pods are
 // loaded up front, every other node on first use.  gMax is the widest node of the cluster, C.EGS_MAX_GPUS for 8-GPU
 // servers, up to C.EGS_MAX_GPUS_WIDE (a wide handle: 16-wide rows, two mask bytes per container, per-pod engine).
+// cMax is the widest pod Assume / Score / Bind place: C.EGS_MAX_CONTAINERS, or up to C.EGS_MAX_CONTAINERS_APPLY for
+// pods with sidecars (a sidecar handle: 8 masks per pod, per-pod engine, gMax <= C.EGS_MAX_GPUS).
 func NewCudaUnitScheduler(config ElasticSchedulerConfig, coreName v1.ResourceName, memName v1.ResourceName,
-	maxNodes int, device int, gMax int) (ResourceScheduler, error) {
+	maxNodes int, device int, gMax int, cMax int) (ResourceScheduler, error) {
 	policy := C.int(C.EGS_BINPACK)
 	if _, ok := config.Rater.(*Spread); ok {
 		policy = C.int(C.EGS_SPREAD)
@@ -74,9 +77,13 @@ func NewCudaUnitScheduler(config ElasticSchedulerConfig, coreName v1.ResourceNam
 		nodeErr:       map[string]error{},
 		maxNodes:      maxNodes,
 		gMax:          gMax,
+		cMax:          cMax,
 	}
-	if st := C.egs_create(policy, C.int(maxNodes), C.int(gMax), C.int(device), &d.h); st != C.EGS_OK {
-		return nil, fmt.Errorf("egs_create failed: status %d (no CUDA device?)", int(st))
+	if d.cMax < C.EGS_MAX_CONTAINERS {
+		d.cMax = C.EGS_MAX_CONTAINERS
+	}
+	if st := C.egs_create_ex(policy, C.int(maxNodes), C.int(gMax), C.int(cMax), C.int(device), &d.h); st != C.EGS_OK {
+		return nil, fmt.Errorf("egs_create_ex failed: status %d (no CUDA device, or gMax / cMax out of range)", int(st))
 	}
 	pods, err := d.Clientset.CoreV1().Pods(metav1.NamespaceAll).List(context.Background(), metav1.ListOptions{
 		LabelSelector: fmt.Sprintf("%s=%s", schetypes.EGPUAssumed, "true"),
@@ -104,7 +111,7 @@ func uidKey(uid types.UID) C.uint64_t {
 }
 
 // requestOf == NewGPURequest (allocate.go:35-58) through egs_unit_from_requests.
-// maxContainers: EGS_MAX_CONTAINERS for the verbs that Trade (Assume / Score / Bind), EGS_MAX_CONTAINERS_APPLY for the
+// maxContainers: cMax for the verbs that Trade (Assume / Score / Bind), EGS_MAX_CONTAINERS_APPLY for the
 // ones that only account a pod somebody placed (AddPod / ForgetPod / replay at node load).
 func (d *CudaUnitScheduler) requestOf(pod *v1.Pod, maxContainers int) ([]C.egs_unit, error) {
 	if len(pod.Spec.Containers) > maxContainers {
@@ -191,7 +198,7 @@ func (d *CudaUnitScheduler) Assume(nodes []string, pod *v1.Pod) ([]string, map[s
 	defer d.lock.Unlock()
 	filteredNodes := []string{}
 	failedNodes := map[string]string{}
-	units, err := d.requestOf(pod, C.EGS_MAX_CONTAINERS)
+	units, err := d.requestOf(pod, d.cMax)
 	if err != nil {
 		return nil, nil, err
 	}
@@ -235,7 +242,7 @@ func (d *CudaUnitScheduler) Score(nodes []string, pod *v1.Pod) []int {
 	d.lock.Lock()
 	defer d.lock.Unlock()
 	scores := make([]int, len(nodes))
-	units, err := d.requestOf(pod, C.EGS_MAX_CONTAINERS)
+	units, err := d.requestOf(pod, d.cMax)
 	if err != nil {
 		return scores
 	}
@@ -291,11 +298,11 @@ func (d *CudaUnitScheduler) Bind(node string, pod *v1.Pod) (err error) {
 	if err != nil {
 		return err
 	}
-	units, err := d.requestOf(pod, C.EGS_MAX_CONTAINERS)
+	units, err := d.requestOf(pod, d.cMax)
 	if err != nil {
 		return err
 	}
-	var masks [2 * C.EGS_MAX_CONTAINERS]C.uint8_t // room for EGS_MASK_BYTES <= 2
+	var masks [2 * C.EGS_MAX_CONTAINERS_APPLY]C.uint8_t // room for EGS_MASKS_PER_POD <= 8 masks of EGS_MASK_BYTES <= 2
 	switch st := C.egs_bind(d.h, C.int(id), C.int(len(units)), &units[0], uidKey(pod.UID), &masks[0]); st {
 	case C.EGS_OK:
 	case C.EGS_ERR_NO_OPTION:
@@ -450,7 +457,7 @@ func BuildResourceSchedulersCuda(modes []string, config ElasticSchedulerConfig) 
 	for _, m := range modes {
 		switch m {
 		case "gpushare-cuda":
-			d, err := NewCudaUnitScheduler(config, v1alpha1.ResourceGPUCore, v1alpha1.ResourceGPUMemory, 1<<20, 0, int(C.EGS_MAX_GPUS))
+			d, err := NewCudaUnitScheduler(config, v1alpha1.ResourceGPUCore, v1alpha1.ResourceGPUMemory, 1<<20, 0, int(C.EGS_MAX_GPUS), int(C.EGS_MAX_CONTAINERS))
 			if err != nil {
 				return nil, err
 			}

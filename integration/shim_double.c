@@ -13,8 +13,9 @@
  *   KNOWN <uid> / RELEASED <uid>                             controller.go:314,322 (answered from the shim's own maps)
  *   STATUS                                                   routes.go:201    -> egs_state_dump
  *
- * argv: [policy [g_max]] -- g_max is the widest node (egs_create), EGS_MAX_GPUS by default; masks are printed as the
- * integer EGS_MASK_BYTES(g_max) little-endian bytes hold, rows are dumped EGS_ROW_WIDTH(g_max) wide.
+ * argv: [policy [g_max [c_max]]] -- g_max is the widest node, EGS_MAX_GPUS by default; c_max the widest pod ASSUME /
+ * SCORE / BIND place, EGS_MAX_CONTAINERS by default (egs_create_ex); masks are printed as the integer
+ * EGS_MASK_BYTES(g_max) little-endian bytes hold, rows are dumped EGS_ROW_WIDTH(g_max) wide.
  */
 #include <stdint.h>
 #include <stdio.h>
@@ -24,7 +25,7 @@
 
 #define MAXN 4096
 static egs_handle *H;
-static int G_MAX = EGS_MAX_GPUS;
+static int G_MAX = EGS_MAX_GPUS, C_MAX = EGS_MAX_CONTAINERS;
 static char names[MAXN][64];
 static int n_nodes = 0;
 static uint64_t known[65536], released[65536];
@@ -71,7 +72,8 @@ static int read_units_alloc(char **tok, egs_unit *u, int32_t *off, int32_t *idx)
 int main(int argc, char **argv) {
   int policy = argc > 1 ? atoi(argv[1]) : 0;
   if (argc > 2) G_MAX = atoi(argv[2]);
-  if (egs_create(policy, MAXN, G_MAX, 0, &H) != EGS_OK) { fprintf(stderr, "egs_create failed\n"); return 2; }
+  if (argc > 3) C_MAX = atoi(argv[3]);
+  if (egs_create_ex(policy, MAXN, G_MAX, C_MAX, 0, &H) != EGS_OK) { fprintf(stderr, "egs_create_ex failed\n"); return 2; }
   static char line[1 << 16];
   setvbuf(stdout, NULL, _IOLBF, 1 << 16);            /* every answer line reaches the driver at once */
   while (fgets(line, sizeof line, stdin)) {
@@ -109,7 +111,7 @@ int main(int argc, char **argv) {
     } else if (!strcmp(cmd, "BIND")) {
       char *uid = strtok_r(NULL, " \n", &tok), *node = strtok_r(NULL, " \n", &tok);
       int C = read_units(&tok, u);
-      uint8_t masks[2 * EGS_MAX_CONTAINERS] = {0};
+      uint8_t masks[2 * EGS_MAX_CONTAINERS_APPLY] = {0};
       int id = node_id(node);
       int st = id < 0 ? EGS_ERR_NO_NODE : egs_bind(H, id, C, u, uid_key(uid), masks);
       if (st == EGS_OK && !has(known, n_known, uid_key(uid))) known[n_known++] = uid_key(uid);   /* d.podMaps[pod.UID] = newPod */
@@ -146,7 +148,7 @@ int main(int argc, char **argv) {
     } else if (!strcmp(cmd, "PEEK")) {                                /* test support: the option Assume cached (GPUIDs) */
       int id = node_id(strtok_r(NULL, " \n", &tok));
       int C = read_units(&tok, u);
-      int32_t valid = 0, score = 0; uint8_t masks[2 * EGS_MAX_CONTAINERS] = {0};
+      int32_t valid = 0, score = 0; uint8_t masks[2 * EGS_MAX_CONTAINERS_APPLY] = {0};
       egs_option_peek(H, id, C, u, &valid, &score, masks);
       printf("PEEK %d %d", valid, score);
       for (int c = 0; c < C; c++) printf(" %d", mask_of(masks, c));
