@@ -42,6 +42,7 @@ SYMBOLS = [
     "egs_state_snapshot", "egs_state_restore", "egs_checkpoint_save", "egs_checkpoint_rollback", "egs_checkpoint_drop",
     "egs_filter", "egs_score", "egs_bind", "egs_option_peek", "egs_option_dump", "egs_pod_apply", "egs_node_replay_pod", "egs_pod_cancel",
     "egs_mutations_apply", "egs_schedule_batch_mut", "egs_pod_known", "egs_pod_released", "egs_schedule_batch", "egs_schedule_batch_vec", "egs_schedule_batch_device",
+    "egs_schedule_batch_nodes",
     "egs_shard_set", "egs_shard_range", "egs_comm_unique_id", "egs_comm_init", "egs_comm_init_local", "egs_profile_evaluate", "egs_profile_get",
     "egs_profile_reset", "egs_get_stream", "egs_rounds_stats", "egs_mix64",
 ]
@@ -103,6 +104,7 @@ def load(build: bool = True):
     L.egs_schedule_batch.argtypes = [vp, i32, i32, vp, vp, vp] + [vp] * 6
     L.egs_schedule_batch_vec.argtypes = [vp, i32, vp, vp, vp, i32, vp, vp] + [vp] * 6
     L.egs_schedule_batch_device.argtypes = [vp, i32, i32, vp, vp] + [vp] * 6
+    L.egs_schedule_batch_nodes.argtypes = [vp, i32, i32, vp, vp, vp, i32, vp, vp] + [vp] * 6
     L.egs_shard_set.argtypes = [vp, i32, i32]
     L.egs_shard_range.argtypes = [i32, i32, i32, C.POINTER(i32), C.POINTER(i32)]
     L.egs_comm_unique_id.argtypes = [vp]
@@ -152,6 +154,29 @@ def units_array(req: Sequence[Tuple[int, int, int]]) -> np.ndarray:
 def masks_to_lists(masks, n_containers: int):
     """GPU index lists of the first n_containers masks (up to 8 planes of up to 16 GPUs)."""
     return [[g for g in range(EGS_MAX_GPUS_WIDE) if (int(masks[c]) >> g) & 1] for c in range(n_containers)]
+
+
+def node_set_words(max_nodes: int) -> int:
+    """EGS_NODE_SET_WORDS: 64-bit words of one node set bitmap of a handle with `max_nodes` nodes."""
+    return (max_nodes + 63) // 64
+
+
+def node_sets_array(sets, max_nodes: int) -> np.ndarray:
+    """Node sets -> the [n_sets][EGS_NODE_SET_WORDS] uint64 bitmaps of egs_schedule_batch_nodes.  Each set is a bool
+    array of max_nodes entries or a list of node ids (bit n & 63 of word n >> 6 admits node n)."""
+    out = np.zeros((max(1, len(sets)), node_set_words(max_nodes)), np.uint64)
+    for k, s in enumerate(sets):
+        a = np.asarray(s)
+        if a.dtype == np.bool_:
+            if a.shape != (max_nodes,):
+                raise ValueError(f"node set {k}: a bool set has max_nodes = {max_nodes} entries, not {a.shape}")
+            ids = np.flatnonzero(a)
+        else:
+            ids = a.astype(np.int64).ravel()
+        bits = np.zeros(out.shape[1] * 64, np.uint8)
+        bits[ids] = 1                                    # ids at or beyond max_nodes set bits the library refuses
+        out[k] = np.packbits(bits, bitorder="little").view("<u8")
+    return out
 
 
 def _alloc_arrays(alloc):
@@ -323,6 +348,29 @@ class Egs:
         self._ck(self.L.egs_schedule_batch(self.h, mode, P, _p(c_off), _p(units), _p(u), _p(out["node"]),
                                            _p(out["status"]), _p(out["alloc_mask"]), _p(out["fit_count"]),
                                            _p(out["fit_digest"]), _p(out["score_digest"])), "egs_schedule_batch")
+        return out
+
+    def schedule_batch_nodes(self, c_off: np.ndarray, units: np.ndarray, sets, pod_set=None,
+                             uids: Optional[np.ndarray] = None, mode: int = EGS_MODE_AUTO):
+        """schedule_batch with a candidate node set per pod (egs_schedule_batch_nodes).  sets: bool arrays of
+        max_nodes entries or node-id lists (node_sets_array), or the packed uint64 bitmaps; pod_set: the set of each
+        pod (None: every pod uses set 0)."""
+        P = len(c_off) - 1
+        c_off = np.ascontiguousarray(c_off, np.int32)
+        units = np.ascontiguousarray(units, np.int32)
+        if isinstance(sets, np.ndarray) and sets.dtype == np.uint64 and sets.ndim == 2:
+            bm = np.ascontiguousarray(sets)
+        else:
+            bm = node_sets_array(sets, self.max_nodes)
+        ps = None if pod_set is None else np.ascontiguousarray(pod_set, np.int32)
+        out = dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
+                   alloc_mask=np.zeros((P, self.n_masks), self.mask_dtype), fit_count=np.zeros(P, np.int32),
+                   fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
+        u = None if uids is None else np.ascontiguousarray(uids, np.uint64)
+        self._ck(self.L.egs_schedule_batch_nodes(self.h, mode, P, _p(c_off), _p(units), _p(u), len(bm), _p(bm), _p(ps),
+                                                 _p(out["node"]), _p(out["status"]), _p(out["alloc_mask"]),
+                                                 _p(out["fit_count"]), _p(out["fit_digest"]), _p(out["score_digest"])),
+                 "egs_schedule_batch_nodes")
         return out
 
     def schedule_batch_vec(self, c_off: np.ndarray, units: np.ndarray, vec_pods: int, uids: Optional[np.ndarray] = None):

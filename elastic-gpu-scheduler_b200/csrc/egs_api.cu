@@ -93,6 +93,7 @@ struct egs_handle {
   DeviceBuf<unsigned long long> d_o_fd, d_o_sd;
   DeviceBuf<char> d_ops; DeviceBuf<int32_t> d_group_off;       // egs_mutations_apply: ApplyOp<row_w>[]
   DeviceBuf<uint8_t> d_vec_fit; DeviceBuf<int32_t> d_vec_score; int vec_pods = 0;   // egs_schedule_batch_vec
+  DeviceBuf<uint64_t> d_set;                                    // egs_schedule_batch_nodes: the running run's node set
   // profiling
   int64_t k_launches[EGS_K_COUNT] = {0}; double k_ms[EGS_K_COUNT] = {0}; int timing = 0;
   RoundsState rounds;
@@ -245,9 +246,9 @@ static bool leaf_split(const egs_handle *h, int C, const egs_unit *u) {
 
 // The leaf-split Trade of every candidate of slot `slot` whose option is absent (k_trade_probe, k_trade_leaves,
 // k_trade_commit; egs_kernels.cuh), enqueued on the stream.  d_ids == nullptr: nodes [0, n).  With d_score the probe is
-// also Score's read of the cache and the commit raises d_panic.
+// also Score's read of the cache and the commit raises d_panic.  With d_set only the nodes of that set are Traded.
 static int trade_misses(egs_handle *h, int slot, int C, const egs_unit *u, const int32_t *d_ids, int n,
-                        int32_t *d_score, int *d_panic) {
+                        int32_t *d_score, int *d_panic, const uint64_t *d_set = nullptr) {
   if (n <= 0) return EGS_OK;
   if ((size_t)n > h->d_miss.cap()) {
     const size_t cap = std::max((size_t)n, (size_t)h->n_pad);
@@ -265,7 +266,8 @@ static int trade_misses(egs_handle *h, int slot, int C, const egs_unit *u, const
   pa.st = t.st; pa.sc = t.sc; pa.ids = d_ids; pa.n = n; pa.n_nodes = h->max_nodes;
   pa.miss = h->d_miss; pa.n_miss = d_n; pa.keys = h->d_keys; pa.out_score = d_score;
   const int grid = (n + 255) / 256;
-  k_trade_probe<<<grid, 256, 0, h->stream>>>(pa);
+  if (d_set) k_trade_probe_nodes<<<grid, 256, 0, h->stream>>>(pa, NodeSet{d_set});
+  else k_trade_probe<<<grid, 256, 0, h->stream>>>(pa);
   LeafArgs la;
   la.core = h->d_core; la.mem = h->d_mem; la.mem_total = h->d_mem_total;
   la.policy = h->policy; la.bits = leaf_bits(h); la.nbranch = n_branch(C, u);
@@ -915,16 +917,16 @@ static int ensure_out(egs_handle *h, int P) {
   return EGS_OK;
 }
 
-// EGS_MODE_RESCAN: one k_pass launch per pod, stream ordered.
+// EGS_MODE_RESCAN: one k_pass launch per pod, stream ordered; k_pass_nodes under a node set d_set.
 static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_unit *units,
-                        const std::vector<int> &slots, PodOut out) {
+                        const std::vector<int> &slots, PodOut out, const uint64_t *d_set) {
   const int grid = (h->max_nodes + PASS_THREADS - 1) / PASS_THREADS;
   for (int p = 0; p < P; p++) h->slot_cold[slots[p]] = 0;
   for (int p = 0; p < P; p++) {
     const int C = c_off[p + 1] - c_off[p];
     const egs_unit *u = units + c_off[p];
     // a shape past the one-thread DFS is Traded on every node without an option first: k_pass then only reads caches
-    if (leaf_split(h, C, u)) TRY(trade_misses(h, slots[p], C, u, nullptr, h->max_nodes, nullptr, nullptr));
+    if (leaf_split(h, C, u)) TRY(trade_misses(h, slots[p], C, u, nullptr, h->max_nodes, nullptr, nullptr, d_set));
     by_geometry(h, [&](auto W) -> int {
       constexpr int G = decltype(W)::G, NP = decltype(W)::NP;
       PassArgsT<ReqOf<NP>> a;
@@ -935,7 +937,9 @@ static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_un
       a.vec_score = p < h->vec_pods ? h->d_vec_score + (size_t)p * h->max_nodes : nullptr;
       a.partials = h->d_partials; a.ticket = h->d_ticket;
       a.pod = p; a.out = out;
-      if (is_single(C, u)) k_pass<G, NP, true><<<grid, PASS_THREADS, 0, h->stream>>>(a);
+      if (d_set && is_single(C, u)) k_pass_nodes<G, NP, true><<<grid, PASS_THREADS, 0, h->stream>>>(a, NodeSet{d_set});
+      else if (d_set) k_pass_nodes<G, NP, false><<<grid, PASS_THREADS, 0, h->stream>>>(a, NodeSet{d_set});
+      else if (is_single(C, u)) k_pass<G, NP, true><<<grid, PASS_THREADS, 0, h->stream>>>(a);
       else k_pass<G, NP, false><<<grid, PASS_THREADS, 0, h->stream>>>(a);
       return EGS_OK;
     });
@@ -956,8 +960,9 @@ static int refuse_wide_rounds(egs_handle *h, int mode) {
   return EGS_OK;
 }
 
+// d_set: the pods' node set on the device (egs_schedule_batch_nodes), nullptr for every node.
 static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, const egs_unit *units,
-                        const uint64_t *uids, PodOut out, bool device_out) {
+                        const uint64_t *uids, PodOut out, bool device_out, const uint64_t *d_set = nullptr) {
   if (P < 0 || (P > 0 && (!c_off || !units))) return EGS_ERR_BAD_ARG;
   TRY(refuse_wide_rounds(h, mode));
   if (P == 0) return EGS_OK;
@@ -987,8 +992,8 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
   }
   if (mode == EGS_MODE_AUTO) mode = per_pod_only(h) ? EGS_MODE_RESCAN : EGS_MODE_ROUNDS;
   int batch_rc = EGS_OK, n_done = P;
-  if (mode == EGS_MODE_RESCAN) TRY(batch_rescan(h, P, c_off, units, slots, dev));
-  else if (mode == EGS_MODE_ROUNDS) batch_rc = batch_rounds(h, P, slots, dev, &n_done);
+  if (mode == EGS_MODE_RESCAN) TRY(batch_rescan(h, P, c_off, units, slots, dev, d_set));
+  else if (mode == EGS_MODE_ROUNDS) batch_rc = batch_rounds(h, P, slots, dev, &n_done, d_set);
   else return EGS_ERR_BAD_ARG;
 
   // lazy uid bookkeeping: async copy of (node, status), applied on the next uid-dependent verb.  A batch that
@@ -1054,17 +1059,18 @@ extern "C" int egs_schedule_batch(egs_handle *h, int mode, int n_pods, const int
   return batch_common(h, mode, n_pods, c_off, units, uids, o, false);
 }
 
-extern "C" int egs_schedule_batch_mut(egs_handle *h, int mode, int n_pods, const int32_t *c_off, const egs_unit *units,
-                                      const uint64_t *uids, int n_mut, const int32_t *mut_at, const egs_mutation *muts,
-                                      int32_t *out_node, int32_t *out_status, uint8_t *out_alloc_mask,
-                                      int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest) {
-  if (!h || n_pods < 0 || n_mut < 0 || (n_mut > 0 && (!mut_at || !muts)) || (n_pods > 0 && (!c_off || !units))) return EGS_ERR_BAD_ARG;
-  for (int j = 0; j < n_mut; j++)
-    if (mut_at[j] < 0 || mut_at[j] > n_pods || (j > 0 && mut_at[j] < mut_at[j - 1])) return EGS_ERR_BAD_ARG;
-  Guard g(h);
-  TRY(refuse_wide_rounds(h, mode));                              // before the first record is applied
-  // segments of pods between mutation points; the lock is held throughout, exactly one "call at a time"
-  int p = 0, j = 0;
+// The one segment driver of the batch entry points.  Pods [0, n_pods) run in segments, each one batch_common call:
+// the mutation records due at pod p (mut_at) are applied, then pods [p, q) run, q being the next mutation point or,
+// under node sets, the first pod of another set.  A set is uploaded when its run starts.  The lock is held
+// throughout, exactly one "call at a time"; an error stops the loop and keeps what earlier segments applied.
+struct NodeSets { const uint64_t *sets = nullptr; const int32_t *pod_set = nullptr; };
+static int run_segments(egs_handle *h, int mode, int n_pods, const int32_t *c_off, const egs_unit *units,
+                        const uint64_t *uids, int n_mut, const int32_t *mut_at, const egs_mutation *muts,
+                        const NodeSets &ns, const PodOut &out) {
+  const size_t words = EGS_NODE_SET_WORDS((size_t)h->max_nodes);
+  auto set_of = [&](int p) { return ns.pod_set ? ns.pod_set[p] : 0; };
+  if (ns.sets && words > h->d_set.cap()) CK(h, grow(h->stream, false, to(h->d_set, words)));
+  int p = 0, j = 0, loaded = -1;
   while (p < n_pods || j < n_mut) {
     int j1 = j;
     while (j1 < n_mut && mut_at[j1] == p) j1++;
@@ -1074,15 +1080,56 @@ extern "C" int egs_schedule_batch_mut(egs_handle *h, int mode, int n_pods, const
       j = j1;
     }
     if (p >= n_pods) break;
-    const int q = j < n_mut ? mut_at[j] : n_pods;                // next mutation point (> p)
-    const PodOut o = pod_out(h, out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest, p);
+    int q = j < n_mut ? mut_at[j] : n_pods;                      // next mutation point (> p)
+    if (ns.sets) {
+      for (int i = p + 1; i < q; i++) if (set_of(i) != set_of(p)) { q = i; break; }
+      if (set_of(p) != loaded) {
+        loaded = set_of(p);
+        CK(h, cudaMemcpyAsync(h->d_set, ns.sets + (size_t)loaded * words, words * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+      }
+    }
+    const PodOut o = pod_out(h, out.node, out.status, out.alloc, out.fit_count, (uint64_t *)out.fit_digest,
+                             (uint64_t *)out.score_digest, p);
     // the segment's pods as a batch of its own: offsets rebased
     std::vector<int32_t> off((size_t)(q - p) + 1);
     for (int i = p; i <= q; i++) off[(size_t)(i - p)] = c_off[i] - c_off[p];
-    TRY(batch_common(h, mode, q - p, off.data(), units + c_off[p], uids ? uids + p : nullptr, o, false));
+    TRY(batch_common(h, mode, q - p, off.data(), units + c_off[p], uids ? uids + p : nullptr, o, false,
+                     ns.sets ? h->d_set.get() : nullptr));
     p = q;
   }
   return EGS_OK;
+}
+
+extern "C" int egs_schedule_batch_mut(egs_handle *h, int mode, int n_pods, const int32_t *c_off, const egs_unit *units,
+                                      const uint64_t *uids, int n_mut, const int32_t *mut_at, const egs_mutation *muts,
+                                      int32_t *out_node, int32_t *out_status, uint8_t *out_alloc_mask,
+                                      int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest) {
+  if (!h || n_pods < 0 || n_mut < 0 || (n_mut > 0 && (!mut_at || !muts)) || (n_pods > 0 && (!c_off || !units))) return EGS_ERR_BAD_ARG;
+  for (int j = 0; j < n_mut; j++)
+    if (mut_at[j] < 0 || mut_at[j] > n_pods || (j > 0 && mut_at[j] < mut_at[j - 1])) return EGS_ERR_BAD_ARG;
+  Guard g(h);
+  TRY(refuse_wide_rounds(h, mode));                              // before the first record is applied
+  const PodOut o = pod_out(h, out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest);
+  return run_segments(h, mode, n_pods, c_off, units, uids, n_mut, mut_at, muts, NodeSets(), o);
+}
+
+extern "C" int egs_schedule_batch_nodes(egs_handle *h, int mode, int n_pods, const int32_t *c_off, const egs_unit *units,
+                                        const uint64_t *uids, int n_sets, const uint64_t *sets, const int32_t *pod_set,
+                                        int32_t *out_node, int32_t *out_status, uint8_t *out_alloc_mask,
+                                        int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest) {
+  if (!h || n_pods < 0 || n_sets < 1 || !sets || (n_pods > 0 && (!c_off || !units))) return EGS_ERR_BAD_ARG;
+  if (pod_set)
+    for (int p = 0; p < n_pods; p++) if (pod_set[p] < 0 || pod_set[p] >= n_sets) return EGS_ERR_BAD_ARG;
+  const size_t words = EGS_NODE_SET_WORDS((size_t)h->max_nodes);
+  if (h->max_nodes % 64) {                                       // no bit at or beyond max_nodes
+    const uint64_t beyond = ~0ull << (h->max_nodes % 64);
+    for (int s = 0; s < n_sets; s++) if (sets[(size_t)s * words + words - 1] & beyond) return EGS_ERR_BAD_ARG;
+  }
+  Guard g(h);
+  TRY(refuse_wide_rounds(h, mode));
+  NodeSets ns; ns.sets = sets; ns.pod_set = pod_set;
+  const PodOut o = pod_out(h, out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest);
+  return run_segments(h, mode, n_pods, c_off, units, uids, 0, nullptr, nullptr, ns, o);
 }
 
 extern "C" int egs_schedule_batch_vec(egs_handle *h, int n_pods, const int32_t *c_off, const egs_unit *units,

@@ -36,6 +36,14 @@ struct PodOut {              // per-pod outputs of the batch loop (device pointe
   unsigned long long *fit_digest, *score_digest;
 };
 
+// A candidate node set of egs_schedule_batch_nodes on the device: bit n & 63 of word n >> 6 admits node n.  The
+// masked kernels (k_pass_nodes, k_evaluate_nodes, k_trade_probe_nodes, k_select_nodes) share their body with the
+// unmasked ones through a MASKED template flag; with MASKED false the set is never read.
+struct NodeSet {
+  const uint64_t *w;
+  __device__ __forceinline__ bool admits(int i) const { return (w[i >> 6] >> (i & 63)) & 1ull; }
+};
+
 // The six per-pod outputs of pod p; `masks` packs the NP alloc masks of the pod (one MaskT<G> per container).
 template <int G, int NP = EGS_C>
 __device__ __forceinline__ void write_pod_out(const PodOut &o, int p, int node, int status, int fit, unsigned long long fd,
@@ -151,14 +159,15 @@ __device__ __forceinline__ int allocate_option(const OptTable &t, size_t w, int3
 // --------------------------------------------------------------------------------------------
 // At G = 16 a minimum of one block per SM lifts ptxas's default 64-register cap, under which the 16-wide row spills
 // (70 / 80 registers without spills, sm_90a); 0 leaves the 8-wide instantiations exactly as they were.
-template <int G, int NP, bool SINGLE>
-__global__ void __launch_bounds__(PASS_THREADS, G > EGS_G ? 1 : 0) k_pass(PassArgsT<ReqOf<NP>> a) {
+// k_pass_nodes: the same for a pod restricted to a node set -- an excluded node takes no Assume and counts nowhere.
+template <int G, int NP, bool SINGLE, bool MASKED>
+__device__ __forceinline__ void pass_body(const PassArgsT<ReqOf<NP>> &a, NodeSet set) {
   __shared__ Partial sm[PASS_THREADS / 32];
   __shared__ bool is_last;
   const int i = blockIdx.x * PASS_THREADS + threadIdx.x;
   unsigned long long key = 0, fd = 0, sd = 0;
   int fit = 0;
-  if (i < a.n) {
+  if (i < a.n && (!MASKED || set.admits(i))) {
     int score = 0;
     if (assume_option<G, SINGLE>(a.t, (size_t)i, a.core, a.mem, a.mem_total, a.req, a.policy, score) == OPT_CACHED) {
       fit = 1; key = cand_key(score, (uint32_t)i); fd = fit_term((uint32_t)i); sd = score_term((uint32_t)i, score);
@@ -196,6 +205,14 @@ __global__ void __launch_bounds__(PASS_THREADS, G > EGS_G ? 1 : 0) k_pass(PassAr
     write_pod_out<G, NP>(a.out, a.pod, node, status, fit, fd, sd, masks);
   }
 }
+template <int G, int NP, bool SINGLE>
+__global__ void __launch_bounds__(PASS_THREADS, G > EGS_G ? 1 : 0) k_pass(PassArgsT<ReqOf<NP>> a) {
+  pass_body<G, NP, SINGLE, false>(a, NodeSet{nullptr});
+}
+template <int G, int NP, bool SINGLE>
+__global__ void __launch_bounds__(PASS_THREADS, G > EGS_G ? 1 : 0) k_pass_nodes(PassArgsT<ReqOf<NP>> a, NodeSet set) {
+  pass_body<G, NP, SINGLE, true>(a, set);
+}
 
 // --------------------------------------------------------------------------------------------
 // k_evaluate: full evaluate of nodes [0,n) for one request, results to flat output planes.
@@ -210,19 +227,20 @@ struct EvalArgs {
   uint8_t v_fit, v_unfit;                                       // byte written for fit / unfit (1/0, or OPT_NEW/OPT_UNFIT
 };                                                              // when the target is an option table)
 
-template <int G, bool SINGLE, int ITEMS>
-__global__ void __launch_bounds__(256) k_evaluate(EvalArgs a) {
+// k_evaluate_nodes (the cold fill of a batch under a node set): an excluded node is neither read nor written.
+template <int G, bool SINGLE, int ITEMS, bool MASKED>
+__device__ __forceinline__ void evaluate_body(const EvalArgs &a, NodeSet set) {
   const int base = blockIdx.x * (256 * ITEMS) + threadIdx.x;
   int c[ITEMS][G], m[ITEMS][G];
 #pragma unroll
   for (int it = 0; it < ITEMS; it++) {
     const int j = base + it * 256;
-    if (j < a.n) load_row(a.core, a.mem, (size_t)(a.lo + j), c[it], m[it]);
+    if (j < a.n && (!MASKED || set.admits(a.lo + j))) load_row(a.core, a.mem, (size_t)(a.lo + j), c[it], m[it]);
   }
 #pragma unroll
   for (int it = 0; it < ITEMS; it++) {
     const int j = base + it * 256;
-    if (j >= a.n) continue;
+    if (j >= a.n || (MASKED && !set.admits(a.lo + j))) continue;
     const int i = a.lo + j;
     int score; PackedT<G> masks;
     const int mt = SINGLE ? 0 : a.mem_total[i];
@@ -234,6 +252,10 @@ __global__ void __launch_bounds__(256) k_evaluate(EvalArgs a) {
     else for (int k = 0; k < a.req.C; k++) gpu[(size_t)k * a.plane + i] = ok ? (MaskT<G>)(masks >> (G * k)) : 0;
   }
 }
+template <int G, bool SINGLE, int ITEMS>
+__global__ void __launch_bounds__(256) k_evaluate(EvalArgs a) { evaluate_body<G, SINGLE, ITEMS, false>(a, NodeSet{nullptr}); }
+template <int G, bool SINGLE, int ITEMS>
+__global__ void __launch_bounds__(256) k_evaluate_nodes(EvalArgs a, NodeSet set) { evaluate_body<G, SINGLE, ITEMS, true>(a, set); }
 
 // --------------------------------------------------------------------------------------------
 // verbs over an explicit candidate list (ids == nullptr -> identity)
@@ -375,13 +397,15 @@ struct ProbeArgs {
   int32_t *out_score;                       // optional: Score's reads (node.go:75-85)
 };
 
-__global__ void __launch_bounds__(256) k_trade_probe(ProbeArgs a) {
+// k_trade_probe_nodes (a batch under a node set): an excluded node is no miss.
+template <bool MASKED>
+__device__ __forceinline__ void probe_body(ProbeArgs a, NodeSet set) {
   const int j = blockIdx.x * 256 + threadIdx.x;
   const int i = j < a.n ? (a.ids ? a.ids[j] : j) : -1;
   const bool valid = i >= 0 && i < a.n_nodes;
   const uint8_t st = valid ? a.st[i] : (uint8_t)OPT_UNFIT;
   if (a.out_score && j < a.n) a.out_score[j] = st == OPT_CACHED ? a.sc[i] : 0;
-  const bool miss = st == OPT_ABSENT;
+  const bool miss = st == OPT_ABSENT && (!MASKED || set.admits(i));
   const unsigned b = __ballot_sync(0xffffffffu, miss);       // one atomic per warp
   if (!b) return;
   const int lane = threadIdx.x & 31, lead = __ffs(b) - 1;
@@ -393,6 +417,8 @@ __global__ void __launch_bounds__(256) k_trade_probe(ProbeArgs a) {
     a.miss[m] = i; a.keys[m] = 0ull;
   }
 }
+__global__ void __launch_bounds__(256) k_trade_probe(ProbeArgs a) { probe_body<false>(a, NodeSet{nullptr}); }
+__global__ void __launch_bounds__(256) k_trade_probe_nodes(ProbeArgs a, NodeSet set) { probe_body<true>(a, set); }
 
 __global__ void __launch_bounds__(LEAF_THREADS) k_trade_leaves(LeafArgs a) {
   __shared__ unsigned long long sm[LEAF_THREADS / 32];

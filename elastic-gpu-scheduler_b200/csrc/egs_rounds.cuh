@@ -195,7 +195,11 @@ __device__ __forceinline__ void merge128(unsigned long long (&A)[RQMAX], const u
 // --------------------------------------------------------------------------------------------
 // k_select
 // --------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(SEL_THREADS) k_select(SelectArgs a) {
+// k_select_nodes (a batch under a node set): an excluded node is skipped whole -- no Trade, no NEW -> CACHED, no fit
+// count, no digest, no list key -- so the candidate lists, and with them every node the resolver tracks, hold only
+// admitted nodes.
+template <bool MASKED>
+__device__ __forceinline__ void select_body(const SelectArgs &a, NodeSet set) {
   __shared__ unsigned long long s_list[SEL_WARPS][32][RK];
   __shared__ AggPart s_agg[SEL_WARPS][32];
   __shared__ Req s_reqs[32];          // the round descriptor is indexed dynamically: stage it in smem
@@ -230,7 +234,8 @@ __global__ void __launch_bounds__(SEL_THREADS) k_select(SelectArgs a) {
 #pragma unroll
         for (int j = 0; j < 4; j++) {
           const int i = base + 32 * j;
-          st[j] = i < a.hi ? stp[i] : (uint8_t)OPT_UNFIT;
+          // an excluded node reads as a node past hi: OPT_UNFIT, which the loop below neither Trades, writes nor counts
+          st[j] = i < a.hi && (!MASKED || set.admits(i)) ? stp[i] : (uint8_t)OPT_UNFIT;
           sc[j] = i < a.hi ? scp[i] : 0;
         }
         unsigned long long key[4], fd = 0, sd = 0;
@@ -287,6 +292,8 @@ __global__ void __launch_bounds__(SEL_THREADS) k_select(SelectArgs a) {
     }
   }
 }
+__global__ void __launch_bounds__(SEL_THREADS) k_select(SelectArgs a) { select_body<false>(a, NodeSet{nullptr}); }
+__global__ void __launch_bounds__(SEL_THREADS) k_select_nodes(SelectArgs a, NodeSet set) { select_body<true>(a, set); }
 
 // --------------------------------------------------------------------------------------------
 // k_merge: one CTA per shape of the round
@@ -1367,8 +1374,9 @@ struct RoundsState {
 };
 
 static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_unit *units,
-                        const std::vector<int> &slots, PodOut out);
-static int batch_rounds(egs_handle *h, int P, const std::vector<int> &slots, PodOut out, int *n_done);
+                        const std::vector<int> &slots, PodOut out, const uint64_t *d_set);
+static int batch_rounds(egs_handle *h, int P, const std::vector<int> &slots, PodOut out, int *n_done,
+                        const uint64_t *d_set);
 static void rounds_free(RoundsState *r);
 static int rounds_comm_unique_id(uint8_t out_id[128]);
 static int rounds_comm_init(egs_handle *h, const uint8_t id[128]);

@@ -126,8 +126,10 @@ static int rounds_ensure(egs_handle *h, int P, const BufLayout &L) {
   return EGS_OK;
 }
 
-// Runs the batch; *n_done = pods resolved (== P unless an error stopped the loop).
-static int batch_rounds(egs_handle *h, int P, const std::vector<int> &slots, PodOut out, int *n_done) {
+// Runs the batch; *n_done = pods resolved (== P unless an error stopped the loop).  Under a node set d_set the cold
+// fill and k_select leave every excluded node alone; the resolver needs no change, since it only tracks list nodes.
+static int batch_rounds(egs_handle *h, int P, const std::vector<int> &slots, PodOut out, int *n_done,
+                        const uint64_t *d_set) {
   RoundsState &R = h->rounds;
   *n_done = 0;
   if (h->world > 1 && !R.comm && !R.local) return fail(h, EGS_ERR_COMM, "sharded handle without egs_comm_init");
@@ -164,7 +166,8 @@ static int batch_rounds(egs_handle *h, int P, const std::vector<int> &slots, Pod
 
   // Cold shapes (option table still all-absent, e.g. a fresh or restored scheduler): ONE full-evaluate launch
   // per shape over this shard's nodes fills the table (OPT_NEW / OPT_UNFIT) -- the HBM-roofline kernel,
-  // N * (8G + 5 + C) bytes each; k_select then finds nothing left to Trade for them.
+  // N * (8G + 5 + C) bytes each; k_select then finds nothing left to Trade for them.  Under a node set the excluded
+  // nodes stay OPT_ABSENT: k_select Trades them in a later batch whose set admits them.
   if (h->hi > h->lo) {
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     int cold = 0;
@@ -178,8 +181,14 @@ static int batch_rounds(egs_handle *h, int P, const std::vector<int> &slots, Pod
       ea.policy = h->policy; ea.req = make_req(sh.C, sh.u);
       ea.fit = tb.st + (size_t)slot * tb.n_pad; ea.score = tb.sc + (size_t)slot * tb.n_pad;
       ea.gpu = tb.al + (size_t)slot * EGS_C * tb.n_pad; ea.plane = tb.n_pad; ea.v_fit = OPT_NEW; ea.v_unfit = OPT_UNFIT;
-      if (is_single(sh.C, sh.u)) k_evaluate<EGS_G, true, 2><<<(ea.n + 511) / 512, 256, 0, h->stream>>>(ea);
-      else k_evaluate<EGS_G, false, 1><<<(ea.n + 255) / 256, 256, 0, h->stream>>>(ea);
+      const NodeSet set{d_set};
+      if (is_single(sh.C, sh.u)) {
+        if (d_set) k_evaluate_nodes<EGS_G, true, 2><<<(ea.n + 511) / 512, 256, 0, h->stream>>>(ea, set);
+        else k_evaluate<EGS_G, true, 2><<<(ea.n + 511) / 512, 256, 0, h->stream>>>(ea);
+      } else {
+        if (d_set) k_evaluate_nodes<EGS_G, false, 1><<<(ea.n + 255) / 256, 256, 0, h->stream>>>(ea, set);
+        else k_evaluate<EGS_G, false, 1><<<(ea.n + 255) / 256, 256, 0, h->stream>>>(ea);
+      }
       cold++;
     }
     if (e0) {
@@ -214,7 +223,8 @@ static int batch_rounds(egs_handle *h, int P, const std::vector<int> &slots, Pod
   int ns_round = ns_cfg;                                        // grid of k_merge
   auto launch_round = [&]() -> int {
     if (h->timing) CK(h, cudaEventRecord(ev[0], h->stream));
-    k_select<<<grid, SEL_THREADS, 0, h->stream>>>(sa);
+    if (d_set) k_select_nodes<<<grid, SEL_THREADS, 0, h->stream>>>(sa, NodeSet{d_set});
+    else k_select<<<grid, SEL_THREADS, 0, h->stream>>>(sa);
     if (h->timing) CK(h, cudaEventRecord(ev[1], h->stream));
     TRY(wait_peers_copied());                                   // peers must have copied my previous buffer before k_merge rewrites it
     k_merge<<<ns_round, 256, 0, h->stream>>>(ma);

@@ -289,6 +289,33 @@ int egs_schedule_batch_device(egs_handle *h, int mode, int n_pods, const int32_t
                               int32_t *d_out_fit_count, uint64_t *d_out_fit_digest,
                               uint64_t *d_out_score_digest);
 
+/* egs_schedule_batch with a candidate node set per pod: the node list kube-scheduler passes after its own predicates
+ * (node selectors and affinity, taints, cordoned and NotReady nodes), as GPUUnitScheduler.Assume receives it
+ * (scheduler.go:112-168).  `sets` holds n_sets >= 1 bitmaps of EGS_NODE_SET_WORDS(max_nodes) words each; bit n & 63
+ * of word n >> 6 admits node n.  Pod p uses set pod_set[p] (pod_set NULL: every pod uses set 0).
+ * Pod p is scheduled exactly as the reference schedules it when passed the nodes of its set in ascending id order:
+ * only those are filtered (Traded and cached), the fit ones scored, the first maximal one bound.  A node outside the
+ * pod's set is not Traded, its options (stale ones included), its "known not to fit" memos and its rows stay as they
+ * are, it counts in neither out_fit_count nor a digest, and it cannot win.  An all-ones set gives what
+ * egs_schedule_batch gives; an empty set gives EGS_ERR_NOFIT with fit count 0 and changes nothing.
+ * Outputs, uids, modes and the per-handle limits are those of egs_schedule_batch (EGS_MODE_ROUNDS stays refused on a
+ * wide or sidecar handle, EGS_MODE_RESCAN stays single-shard); on a sharded handle every rank passes the same full
+ * bitmaps.  EGS_ERR_BAD_ARG, before anything is applied: n_sets < 1, sets NULL, pod_set[p] outside [0, n_sets), or
+ * a bit set at or beyond max_nodes.
+ * Each run of consecutive pods with the same pod_set value is one batch of its own, with the library-assigned uids
+ * continuing across runs as in one batch; a run stopped by an error keeps what earlier runs applied.
+ * Cost model: the set is read per node by the kernels that already read that node, so one set costs what
+ * egs_schedule_batch costs (config 4 on one H100 80GB HBM3 at 700 W, one run each: 0.95 M decisions/s without a set,
+ * 0.98 M with an all-ones set, 0.99 M with a 90 % set).  Every run boundary ends a batch -- a host synchronisation, the result copies, the upload of
+ * the next set and at least one round of its own -- about 0.3-0.5 ms at config 4 on that card: two pools alternating
+ * in runs of 10 000 / 1 000 / 100 / 10 pods give 0.96 M / 0.77 M / 0.16 M / 0.024 M decisions/s.  So order the pods
+ * set by set where that keeps each pod's decision (INTEGRATION.md 3). */
+#define EGS_NODE_SET_WORDS(max_nodes) (((max_nodes) + 63) / 64)
+int egs_schedule_batch_nodes(egs_handle *h, int mode, int n_pods, const int32_t *c_off, const egs_unit *units,
+                             const uint64_t *uids, int n_sets, const uint64_t *sets, const int32_t *pod_set,
+                             int32_t *out_node, int32_t *out_status, uint8_t *out_alloc_mask,
+                             int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest);
+
 /* ---- node sharding over several GPUs (one handle per device) ----------------- */
 
 /* This handle owns nodes [lo, hi) of the max_nodes id space; rank/world describe the
