@@ -317,17 +317,8 @@ class Egs:
         return self.L.egs_mutations_apply(self.h, len(records), _p(a))
 
     def schedule_batch_mut(self, c_off, units, mut_at, records, uids=None, mode: int = EGS_MODE_AUTO):
-        P = len(c_off) - 1
-        c_off = np.ascontiguousarray(c_off, np.int32); units = np.ascontiguousarray(units, np.int32)
         at = np.ascontiguousarray(mut_at, np.int32); a = mutations_array(records)
-        out = dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
-                   alloc_mask=np.zeros((P, self.n_masks), self.mask_dtype), fit_count=np.zeros(P, np.int32),
-                   fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
-        u = None if uids is None else np.ascontiguousarray(uids, np.uint64)
-        self._ck(self.L.egs_schedule_batch_mut(self.h, mode, P, _p(c_off), _p(units), _p(u), len(records), _p(at), _p(a),
-                                               _p(out["node"]), _p(out["status"]), _p(out["alloc_mask"]), _p(out["fit_count"]),
-                                               _p(out["fit_digest"]), _p(out["score_digest"])), "egs_schedule_batch_mut")
-        return out
+        return self._batch_call("egs_schedule_batch_mut", (mode,), c_off, units, uids, (len(records), _p(at), _p(a)))
 
     def pod_known(self, uid: int) -> bool:
         return bool(self.L.egs_pod_known(self.h, uid))
@@ -336,59 +327,47 @@ class Egs:
         return bool(self.L.egs_pod_released(self.h, uid))
 
     # ---- batch
-    def schedule_batch(self, c_off: np.ndarray, units: np.ndarray, uids: Optional[np.ndarray] = None,
-                       mode: int = EGS_MODE_AUTO):
-        P = len(c_off) - 1
+    def _batch_out(self, P: int) -> dict:
+        """The six per-pod outputs of a batch of P pods, at the handle's mask dtype and plane count."""
+        return dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
+                    alloc_mask=np.zeros((P, self.n_masks), self.mask_dtype), fit_count=np.zeros(P, np.int32),
+                    fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
+
+    def _batch_call(self, fn: str, lead, c_off, units, uids, extra=(), out: Optional[dict] = None) -> dict:
+        """fn(handle, *lead, P, c_off, units, uids, *extra, the six outputs), its status checked.  Returns the outputs:
+        `out`, or the six arrays of _batch_out."""
+        out = self._batch_out(len(c_off) - 1) if out is None else out
         c_off = np.ascontiguousarray(c_off, np.int32)
         units = np.ascontiguousarray(units, np.int32)
-        out = dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
-                   alloc_mask=np.zeros((P, self.n_masks), self.mask_dtype), fit_count=np.zeros(P, np.int32),
-                   fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
         u = None if uids is None else np.ascontiguousarray(uids, np.uint64)
-        self._ck(self.L.egs_schedule_batch(self.h, mode, P, _p(c_off), _p(units), _p(u), _p(out["node"]),
-                                           _p(out["status"]), _p(out["alloc_mask"]), _p(out["fit_count"]),
-                                           _p(out["fit_digest"]), _p(out["score_digest"])), "egs_schedule_batch")
+        outs = [_p(out[k]) for k in ("node", "status", "alloc_mask", "fit_count", "fit_digest", "score_digest")]
+        self._ck(getattr(self.L, fn)(self.h, *lead, len(c_off) - 1, _p(c_off), _p(units), _p(u), *extra, *outs), fn)
         return out
+
+    def schedule_batch(self, c_off: np.ndarray, units: np.ndarray, uids: Optional[np.ndarray] = None,
+                       mode: int = EGS_MODE_AUTO):
+        return self._batch_call("egs_schedule_batch", (mode,), c_off, units, uids)
 
     def schedule_batch_nodes(self, c_off: np.ndarray, units: np.ndarray, sets, pod_set=None,
                              uids: Optional[np.ndarray] = None, mode: int = EGS_MODE_AUTO):
         """schedule_batch with a candidate node set per pod (egs_schedule_batch_nodes).  sets: bool arrays of
         max_nodes entries or node-id lists (node_sets_array), or the packed uint64 bitmaps; pod_set: the set of each
         pod (None: every pod uses set 0)."""
-        P = len(c_off) - 1
-        c_off = np.ascontiguousarray(c_off, np.int32)
-        units = np.ascontiguousarray(units, np.int32)
         if isinstance(sets, np.ndarray) and sets.dtype == np.uint64 and sets.ndim == 2:
             bm = np.ascontiguousarray(sets)
         else:
             bm = node_sets_array(sets, self.max_nodes)
         ps = None if pod_set is None else np.ascontiguousarray(pod_set, np.int32)
-        out = dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
-                   alloc_mask=np.zeros((P, self.n_masks), self.mask_dtype), fit_count=np.zeros(P, np.int32),
-                   fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
-        u = None if uids is None else np.ascontiguousarray(uids, np.uint64)
-        self._ck(self.L.egs_schedule_batch_nodes(self.h, mode, P, _p(c_off), _p(units), _p(u), len(bm), _p(bm), _p(ps),
-                                                 _p(out["node"]), _p(out["status"]), _p(out["alloc_mask"]),
-                                                 _p(out["fit_count"]), _p(out["fit_digest"]), _p(out["score_digest"])),
-                 "egs_schedule_batch_nodes")
-        return out
+        return self._batch_call("egs_schedule_batch_nodes", (mode,), c_off, units, uids, (len(bm), _p(bm), _p(ps)))
 
     def schedule_batch_vec(self, c_off: np.ndarray, units: np.ndarray, vec_pods: int, uids: Optional[np.ndarray] = None):
         """schedule_batch + the full fit / score vectors of the first `vec_pods` pods ([vec_pods, N] each)."""
-        P = len(c_off) - 1
-        c_off = np.ascontiguousarray(c_off, np.int32)
-        units = np.ascontiguousarray(units, np.int32)
-        vec_pods = min(vec_pods, P)
-        out = dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
-                   alloc_mask=np.zeros((P, self.n_masks), self.mask_dtype), fit_count=np.zeros(P, np.int32),
-                   fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64),
-                   vec_fit=np.zeros((max(vec_pods, 1), self.max_nodes), np.uint8),
-                   vec_score=np.zeros((max(vec_pods, 1), self.max_nodes), np.int32))
-        u = None if uids is None else np.ascontiguousarray(uids, np.uint64)
-        self._ck(self.L.egs_schedule_batch_vec(self.h, P, _p(c_off), _p(units), _p(u), vec_pods, _p(out["vec_fit"]),
-                                               _p(out["vec_score"]), _p(out["node"]), _p(out["status"]),
-                                               _p(out["alloc_mask"]), _p(out["fit_count"]), _p(out["fit_digest"]),
-                                               _p(out["score_digest"])), "egs_schedule_batch_vec")
+        vec_pods = min(vec_pods, len(c_off) - 1)
+        out = self._batch_out(len(c_off) - 1)
+        out["vec_fit"] = np.zeros((max(vec_pods, 1), self.max_nodes), np.uint8)
+        out["vec_score"] = np.zeros((max(vec_pods, 1), self.max_nodes), np.int32)
+        self._batch_call("egs_schedule_batch_vec", (), c_off, units, uids,
+                         (vec_pods, _p(out["vec_fit"]), _p(out["vec_score"])), out)
         out["vec_fit"], out["vec_score"] = out["vec_fit"][:vec_pods], out["vec_score"][:vec_pods]
         return out
 

@@ -92,7 +92,7 @@ struct egs_handle {
   DeviceBuf<int32_t> d_o_node, d_o_status, d_o_fit; DeviceBuf<uint8_t> d_o_alloc;
   DeviceBuf<unsigned long long> d_o_fd, d_o_sd;
   DeviceBuf<char> d_ops; DeviceBuf<int32_t> d_group_off;       // egs_mutations_apply: ApplyOp<row_w>[]
-  DeviceBuf<uint8_t> d_vec_fit; DeviceBuf<int32_t> d_vec_score; int vec_pods = 0;   // egs_schedule_batch_vec
+  DeviceBuf<uint8_t> d_vec_fit; DeviceBuf<int32_t> d_vec_score;              // egs_schedule_batch_vec
   DeviceBuf<uint64_t> d_set;                                    // egs_schedule_batch_nodes: the running run's node set
   // profiling
   int64_t k_launches[EGS_K_COUNT] = {0}; double k_ms[EGS_K_COUNT] = {0}; int timing = 0;
@@ -909,6 +909,28 @@ extern "C" int egs_pod_released(egs_handle *h, uint64_t uid) {
 }
 
 // ------------------------------------------------------------------------------- batch loop
+// The caller's outputs of one batch call: the six per-pod arrays, device pointers when `device` and host pointers
+// otherwise, each of which may be null; and egs_schedule_batch_vec's full fit / score vectors, [vec_pods][max_nodes]
+// on the device, read only for pods below vec_pods.
+struct BatchOut {
+  PodOut pod; bool device;
+  uint8_t *vec_fit = nullptr; int32_t *vec_score = nullptr; int vec_pods = 0;
+  BatchOut(int32_t *node, int32_t *status, uint8_t *alloc, int32_t *fit_count, uint64_t *fit_digest,
+           uint64_t *score_digest, bool device)
+      : pod{node, status, fit_count, alloc, (unsigned long long *)fit_digest, (unsigned long long *)score_digest},
+        device(device) {}
+};
+
+// The outputs of pods [p, ...) of a batch whose outputs are `o`: every pointer advanced by p pods.
+static BatchOut out_from(const egs_handle *h, BatchOut o, int p) {
+  auto at = [p](auto *&a, size_t per_pod) { if (a) a += (size_t)p * per_pod; };
+  at(o.pod.node, 1); at(o.pod.status, 1); at(o.pod.fit_count, 1); at(o.pod.fit_digest, 1); at(o.pod.score_digest, 1);
+  at(o.pod.alloc, (size_t)h->planes * h->mask_b);
+  o.vec_pods = std::max(o.vec_pods - p, 0);
+  if (o.vec_pods) { at(o.vec_fit, h->max_nodes); at(o.vec_score, h->max_nodes); }
+  return o;
+}
+
 static int ensure_out(egs_handle *h, int P) {
   if ((size_t)P <= h->d_o_node.cap()) return EGS_OK;
   const size_t cap = (size_t)std::max(P, 1024);
@@ -917,9 +939,9 @@ static int ensure_out(egs_handle *h, int P) {
   return EGS_OK;
 }
 
-// EGS_MODE_RESCAN: one k_pass launch per pod, stream ordered; k_pass_nodes under a node set d_set.
+// EGS_MODE_RESCAN: one k_pass launch per pod into the device outputs `out`, stream ordered; k_pass_nodes under d_set.
 static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_unit *units,
-                        const std::vector<int> &slots, PodOut out, const uint64_t *d_set) {
+                        const std::vector<int> &slots, const BatchOut &out, const uint64_t *d_set) {
   const int grid = (h->max_nodes + PASS_THREADS - 1) / PASS_THREADS;
   for (int p = 0; p < P; p++) h->slot_cold[slots[p]] = 0;
   for (int p = 0; p < P; p++) {
@@ -933,10 +955,10 @@ static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_un
       a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total; a.core_w = h->d_core; a.mem_w = h->d_mem;
       a.n = h->max_nodes; a.policy = h->policy; a.req = make_req<ReqOf<NP>>(C, u); a.t = table(h, slots[p]);
       a.all_st = h->tables.st; a.slot_stride = (size_t)h->n_pad; a.n_slots = (int)h->shapes.size();
-      a.vec_fit = p < h->vec_pods ? h->d_vec_fit + (size_t)p * h->max_nodes : nullptr;
-      a.vec_score = p < h->vec_pods ? h->d_vec_score + (size_t)p * h->max_nodes : nullptr;
+      a.vec_fit = p < out.vec_pods ? out.vec_fit + (size_t)p * h->max_nodes : nullptr;
+      a.vec_score = p < out.vec_pods ? out.vec_score + (size_t)p * h->max_nodes : nullptr;
       a.partials = h->d_partials; a.ticket = h->d_ticket;
-      a.pod = p; a.out = out;
+      a.pod = p; a.out = out.pod;
       if (d_set && is_single(C, u)) k_pass_nodes<G, NP, true><<<grid, PASS_THREADS, 0, h->stream>>>(a, NodeSet{d_set});
       else if (d_set) k_pass_nodes<G, NP, false><<<grid, PASS_THREADS, 0, h->stream>>>(a, NodeSet{d_set});
       else if (is_single(C, u)) k_pass<G, NP, true><<<grid, PASS_THREADS, 0, h->stream>>>(a);
@@ -950,22 +972,21 @@ static int batch_rescan(egs_handle *h, int P, const int32_t *c_off, const egs_un
   return EGS_OK;
 }
 
-// Wide and sidecar handles have no rounds engine: EGS_MODE_ROUNDS is refused before the batch touches anything, and
-// EGS_MODE_AUTO runs the per-pod engine there.
+// Wide and sidecar handles have no rounds engine: EGS_MODE_AUTO runs the per-pod engine there.
 static bool per_pod_only(const egs_handle *h) { return is_wide(h) || is_sidecar(h); }
-static int refuse_wide_rounds(egs_handle *h, int mode) {
-  if (mode != EGS_MODE_ROUNDS) return EGS_OK;
-  if (is_wide(h)) return fail(h, EGS_ERR_BAD_ARG, "EGS_MODE_ROUNDS needs g_max <= EGS_MAX_GPUS");
-  if (is_sidecar(h)) return fail(h, EGS_ERR_BAD_ARG, "EGS_MODE_ROUNDS needs c_max <= EGS_MAX_CONTAINERS");
+
+// The argument checks every batch entry point makes, under the lock, before it applies or allocates anything.
+static int check_batch(egs_handle *h, int mode, int n_pods, const int32_t *c_off, const egs_unit *units) {
+  if (n_pods < 0 || (n_pods > 0 && (!c_off || !units))) return EGS_ERR_BAD_ARG;
+  if (mode == EGS_MODE_ROUNDS && is_wide(h)) return fail(h, EGS_ERR_BAD_ARG, "EGS_MODE_ROUNDS needs g_max <= EGS_MAX_GPUS");
+  if (mode == EGS_MODE_ROUNDS && is_sidecar(h)) return fail(h, EGS_ERR_BAD_ARG, "EGS_MODE_ROUNDS needs c_max <= EGS_MAX_CONTAINERS");
   return EGS_OK;
 }
 
-// d_set: the pods' node set on the device (egs_schedule_batch_nodes), nullptr for every node.
+// Pods [0, P) of one segment, P > 0.  c_off[p] is the offset of pod p's units from `units`; out: the segment's
+// outputs.  d_set: the pods' node set on the device (egs_schedule_batch_nodes), nullptr for every node.
 static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, const egs_unit *units,
-                        const uint64_t *uids, PodOut out, bool device_out, const uint64_t *d_set = nullptr) {
-  if (P < 0 || (P > 0 && (!c_off || !units))) return EGS_ERR_BAD_ARG;
-  TRY(refuse_wide_rounds(h, mode));
-  if (P == 0) return EGS_OK;
+                        const uint64_t *uids, const BatchOut &out, const uint64_t *d_set) {
   if (h->world > 1 && mode == EGS_MODE_RESCAN) return fail(h, EGS_ERR_BAD_ARG, "EGS_MODE_RESCAN is single-shard");
   std::vector<int> slots((size_t)P);
   for (int p = 0; p < P; p++) {
@@ -980,20 +1001,15 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
       if (!seen.insert(uids[p]).second || h->book.in_pod_maps(uids[p])) return fail(h, EGS_ERR_BAD_ARG, "duplicate or known uid");
     }
   }
-  PodOut dev = out;
-  if (!device_out) {
-    TRY(ensure_out(h, P));
-    dev.node = h->d_o_node; dev.status = h->d_o_status; dev.fit_count = h->d_o_fit; dev.alloc = h->d_o_alloc;
-    dev.fit_digest = h->d_o_fd; dev.score_digest = h->d_o_sd;
-  } else {
-    TRY(ensure_out(h, P));
-    if (!dev.node) dev.node = h->d_o_node;          // uid bookkeeping needs node + status
-    if (!dev.status) dev.status = h->d_o_status;
-  }
+  TRY(ensure_out(h, P));
+  BatchOut dev = out;                            // the kernels' outputs: the handle's buffers stand in for host ones
+  if (!out.device) dev.pod = PodOut{h->d_o_node, h->d_o_status, h->d_o_fit, h->d_o_alloc, h->d_o_fd, h->d_o_sd};
+  if (!dev.pod.node) dev.pod.node = h->d_o_node;          // uid bookkeeping needs node + status
+  if (!dev.pod.status) dev.pod.status = h->d_o_status;
   if (mode == EGS_MODE_AUTO) mode = per_pod_only(h) ? EGS_MODE_RESCAN : EGS_MODE_ROUNDS;
   int batch_rc = EGS_OK, n_done = P;
   if (mode == EGS_MODE_RESCAN) TRY(batch_rescan(h, P, c_off, units, slots, dev, d_set));
-  else if (mode == EGS_MODE_ROUNDS) batch_rc = batch_rounds(h, P, slots, dev, &n_done, d_set);
+  else if (mode == EGS_MODE_ROUNDS) batch_rc = batch_rounds(h, P, slots, dev.pod, &n_done, d_set);
   else return EGS_ERR_BAD_ARG;
 
   // lazy uid bookkeeping: async copy of (node, status), applied on the next uid-dependent verb.  A batch that
@@ -1003,70 +1019,46 @@ static int batch_common(egs_handle *h, int mode, int P, const int32_t *c_off, co
     if (uids) pb.uids.assign(uids, uids + n_done); else h->next_uid += (uint64_t)n_done;
     TRY(pin_get(h, 2 * (size_t)n_done, &pb.buf));
     pb.h_node = pb.buf; pb.h_status = pb.buf + n_done;
-    CK(h, cudaMemcpyAsync(pb.h_node, dev.node, sizeof(int32_t) * (size_t)n_done, cudaMemcpyDeviceToHost, h->stream));
-    CK(h, cudaMemcpyAsync(pb.h_status, dev.status, sizeof(int32_t) * (size_t)n_done, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaMemcpyAsync(pb.h_node, dev.pod.node, sizeof(int32_t) * (size_t)n_done, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaMemcpyAsync(pb.h_status, dev.pod.status, sizeof(int32_t) * (size_t)n_done, cudaMemcpyDeviceToHost, h->stream));
     CK(h, cudaEventCreateWithFlags(&pb.done, cudaEventDisableTiming));
     CK(h, cudaEventRecord(pb.done, h->stream));
     h->pending.push_back(std::move(pb));
   }
   if (batch_rc != EGS_OK) { cudaStreamSynchronize(h->stream); return batch_rc; }
 
-  if (!device_out) {
-    size_t sp = (size_t)P;
-    const size_t ab = (size_t)h->planes * h->mask_b;   // alloc bytes per pod
-    TRY(ensure_stage(h, sp * (4 + 4 + 4 + ab + 8 + 8)));
-    char *s = h->h_stage.get();
-    int32_t *hn = (int32_t *)s, *hs = hn + sp, *hf = hs + sp;
-    unsigned long long *hfd = (unsigned long long *)(hf + sp), *hsd = hfd + sp;
-    uint8_t *ha = (uint8_t *)(hsd + sp);
-    if (out.node) CK(h, cudaMemcpyAsync(hn, dev.node, 4 * sp, cudaMemcpyDeviceToHost, h->stream));
-    if (out.status) CK(h, cudaMemcpyAsync(hs, dev.status, 4 * sp, cudaMemcpyDeviceToHost, h->stream));
-    if (out.fit_count) CK(h, cudaMemcpyAsync(hf, dev.fit_count, 4 * sp, cudaMemcpyDeviceToHost, h->stream));
-    if (out.fit_digest) CK(h, cudaMemcpyAsync(hfd, dev.fit_digest, 8 * sp, cudaMemcpyDeviceToHost, h->stream));
-    if (out.score_digest) CK(h, cudaMemcpyAsync(hsd, dev.score_digest, 8 * sp, cudaMemcpyDeviceToHost, h->stream));
-    if (out.alloc) CK(h, cudaMemcpyAsync(ha, dev.alloc, ab * sp, cudaMemcpyDeviceToHost, h->stream));
-    CK(h, cudaStreamSynchronize(h->stream));
-    if (out.node) memcpy(out.node, hn, 4 * sp);
-    if (out.status) memcpy(out.status, hs, 4 * sp);
-    if (out.fit_count) memcpy(out.fit_count, hf, 4 * sp);
-    if (out.fit_digest) memcpy(out.fit_digest, hfd, 8 * sp);
-    if (out.score_digest) memcpy(out.score_digest, hsd, 8 * sp);
-    if (out.alloc) memcpy(out.alloc, ha, ab * sp);
-  } else {
-    CK(h, cudaStreamSynchronize(h->stream));
+  if (out.device) { CK(h, cudaStreamSynchronize(h->stream)); return EGS_OK; }
+
+  // host outputs: each requested array is staged through pinned memory
+  const PodOut &o = out.pod, &d = dev.pod;
+  const size_t sp = (size_t)P, ab = (size_t)h->planes * h->mask_b;   // alloc bytes per pod
+  const struct { void *to; const void *from; size_t bytes; } arrays[] = {
+      {o.node, d.node, 4 * sp}, {o.status, d.status, 4 * sp}, {o.fit_count, d.fit_count, 4 * sp},
+      {o.fit_digest, d.fit_digest, 8 * sp}, {o.score_digest, d.score_digest, 8 * sp}, {o.alloc, d.alloc, ab * sp}};
+  TRY(ensure_stage(h, sp * (4 + 4 + 4 + 8 + 8 + ab)));
+  char *s = h->h_stage.get();
+  for (const auto &x : arrays) {
+    if (x.to) CK(h, cudaMemcpyAsync(s, x.from, x.bytes, cudaMemcpyDeviceToHost, h->stream));
+    s += x.bytes;
+  }
+  CK(h, cudaStreamSynchronize(h->stream));
+  s = h->h_stage.get();
+  for (const auto &x : arrays) {
+    if (x.to) memcpy(x.to, s, x.bytes);
+    s += x.bytes;
   }
   return EGS_OK;
 }
 
-// The caller's six per-pod outputs from pod p on; each may be null.
-static PodOut pod_out(const egs_handle *h, int32_t *node, int32_t *status, uint8_t *alloc, int32_t *fit_count,
-                      uint64_t *fit_digest, uint64_t *score_digest, int p = 0) {
-  PodOut o;
-  o.node = node ? node + p : nullptr; o.status = status ? status + p : nullptr;
-  o.alloc = alloc ? alloc + (size_t)p * h->planes * h->mask_b : nullptr; o.fit_count = fit_count ? fit_count + p : nullptr;
-  o.fit_digest = fit_digest ? (unsigned long long *)fit_digest + p : nullptr;
-  o.score_digest = score_digest ? (unsigned long long *)score_digest + p : nullptr;
-  return o;
-}
-
-extern "C" int egs_schedule_batch(egs_handle *h, int mode, int n_pods, const int32_t *c_off, const egs_unit *units,
-                                  const uint64_t *uids, int32_t *out_node, int32_t *out_status,
-                                  uint8_t *out_alloc_mask, int32_t *out_fit_count, uint64_t *out_fit_digest,
-                                  uint64_t *out_score_digest) {
-  if (!h) return EGS_ERR_BAD_ARG;
-  Guard g(h);
-  const PodOut o = pod_out(h, out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest);
-  return batch_common(h, mode, n_pods, c_off, units, uids, o, false);
-}
-
-// The one segment driver of the batch entry points.  Pods [0, n_pods) run in segments, each one batch_common call:
-// the mutation records due at pod p (mut_at) are applied, then pods [p, q) run, q being the next mutation point or,
-// under node sets, the first pod of another set.  A set is uploaded when its run starts.  The lock is held
-// throughout, exactly one "call at a time"; an error stops the loop and keeps what earlier segments applied.
+// The one driver of the batch entry points.  Pods [0, n_pods) run in segments, each one batch_common call: the
+// mutation records due at pod p (mut_at) are applied, then pods [p, q) run, q being the next mutation point or,
+// under node sets, the first pod of another set.  A set is uploaded when its run starts.  Without records or sets
+// the batch is one segment.  The lock is held throughout, exactly one "call at a time"; an error stops the loop and
+// keeps what earlier segments applied.
 struct NodeSets { const uint64_t *sets = nullptr; const int32_t *pod_set = nullptr; };
 static int run_segments(egs_handle *h, int mode, int n_pods, const int32_t *c_off, const egs_unit *units,
-                        const uint64_t *uids, int n_mut, const int32_t *mut_at, const egs_mutation *muts,
-                        const NodeSets &ns, const PodOut &out) {
+                        const uint64_t *uids, const BatchOut &out, int n_mut = 0, const int32_t *mut_at = nullptr,
+                        const egs_mutation *muts = nullptr, const NodeSets &ns = NodeSets()) {
   const size_t words = EGS_NODE_SET_WORDS((size_t)h->max_nodes);
   auto set_of = [&](int p) { return ns.pod_set ? ns.pod_set[p] : 0; };
   if (ns.sets && words > h->d_set.cap()) CK(h, grow(h->stream, false, to(h->d_set, words)));
@@ -1088,36 +1080,42 @@ static int run_segments(egs_handle *h, int mode, int n_pods, const int32_t *c_of
         CK(h, cudaMemcpyAsync(h->d_set, ns.sets + (size_t)loaded * words, words * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
       }
     }
-    const PodOut o = pod_out(h, out.node, out.status, out.alloc, out.fit_count, (uint64_t *)out.fit_digest,
-                             (uint64_t *)out.score_digest, p);
-    // the segment's pods as a batch of its own: offsets rebased
-    std::vector<int32_t> off((size_t)(q - p) + 1);
-    for (int i = p; i <= q; i++) off[(size_t)(i - p)] = c_off[i] - c_off[p];
-    TRY(batch_common(h, mode, q - p, off.data(), units + c_off[p], uids ? uids + p : nullptr, o, false,
+    TRY(batch_common(h, mode, q - p, c_off + p, units, uids ? uids + p : nullptr, out_from(h, out, p),
                      ns.sets ? h->d_set.get() : nullptr));
     p = q;
   }
   return EGS_OK;
 }
 
+extern "C" int egs_schedule_batch(egs_handle *h, int mode, int n_pods, const int32_t *c_off, const egs_unit *units,
+                                  const uint64_t *uids, int32_t *out_node, int32_t *out_status,
+                                  uint8_t *out_alloc_mask, int32_t *out_fit_count, uint64_t *out_fit_digest,
+                                  uint64_t *out_score_digest) {
+  if (!h) return EGS_ERR_BAD_ARG;
+  Guard g(h);
+  TRY(check_batch(h, mode, n_pods, c_off, units));
+  const BatchOut o(out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest, false);
+  return run_segments(h, mode, n_pods, c_off, units, uids, o);
+}
+
 extern "C" int egs_schedule_batch_mut(egs_handle *h, int mode, int n_pods, const int32_t *c_off, const egs_unit *units,
                                       const uint64_t *uids, int n_mut, const int32_t *mut_at, const egs_mutation *muts,
                                       int32_t *out_node, int32_t *out_status, uint8_t *out_alloc_mask,
                                       int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest) {
-  if (!h || n_pods < 0 || n_mut < 0 || (n_mut > 0 && (!mut_at || !muts)) || (n_pods > 0 && (!c_off || !units))) return EGS_ERR_BAD_ARG;
+  if (!h || n_mut < 0 || (n_mut > 0 && (!mut_at || !muts))) return EGS_ERR_BAD_ARG;
   for (int j = 0; j < n_mut; j++)
     if (mut_at[j] < 0 || mut_at[j] > n_pods || (j > 0 && mut_at[j] < mut_at[j - 1])) return EGS_ERR_BAD_ARG;
   Guard g(h);
-  TRY(refuse_wide_rounds(h, mode));                              // before the first record is applied
-  const PodOut o = pod_out(h, out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest);
-  return run_segments(h, mode, n_pods, c_off, units, uids, n_mut, mut_at, muts, NodeSets(), o);
+  TRY(check_batch(h, mode, n_pods, c_off, units));               // before the first record is applied
+  const BatchOut o(out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest, false);
+  return run_segments(h, mode, n_pods, c_off, units, uids, o, n_mut, mut_at, muts);
 }
 
 extern "C" int egs_schedule_batch_nodes(egs_handle *h, int mode, int n_pods, const int32_t *c_off, const egs_unit *units,
                                         const uint64_t *uids, int n_sets, const uint64_t *sets, const int32_t *pod_set,
                                         int32_t *out_node, int32_t *out_status, uint8_t *out_alloc_mask,
                                         int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest) {
-  if (!h || n_pods < 0 || n_sets < 1 || !sets || (n_pods > 0 && (!c_off || !units))) return EGS_ERR_BAD_ARG;
+  if (!h || n_sets < 1 || !sets) return EGS_ERR_BAD_ARG;
   if (pod_set)
     for (int p = 0; p < n_pods; p++) if (pod_set[p] < 0 || pod_set[p] >= n_sets) return EGS_ERR_BAD_ARG;
   const size_t words = EGS_NODE_SET_WORDS((size_t)h->max_nodes);
@@ -1126,10 +1124,10 @@ extern "C" int egs_schedule_batch_nodes(egs_handle *h, int mode, int n_pods, con
     for (int s = 0; s < n_sets; s++) if (sets[(size_t)s * words + words - 1] & beyond) return EGS_ERR_BAD_ARG;
   }
   Guard g(h);
-  TRY(refuse_wide_rounds(h, mode));
+  TRY(check_batch(h, mode, n_pods, c_off, units));
   NodeSets ns; ns.sets = sets; ns.pod_set = pod_set;
-  const PodOut o = pod_out(h, out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest);
-  return run_segments(h, mode, n_pods, c_off, units, uids, 0, nullptr, nullptr, ns, o);
+  const BatchOut o(out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest, false);
+  return run_segments(h, mode, n_pods, c_off, units, uids, o, 0, nullptr, nullptr, ns);
 }
 
 extern "C" int egs_schedule_batch_vec(egs_handle *h, int n_pods, const int32_t *c_off, const egs_unit *units,
@@ -1138,18 +1136,18 @@ extern "C" int egs_schedule_batch_vec(egs_handle *h, int n_pods, const int32_t *
                                       int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest) {
   if (!h || vec_pods < 0 || (vec_pods > 0 && (!out_vec_fit || !out_vec_score))) return EGS_ERR_BAD_ARG;
   Guard g(h);
+  TRY(check_batch(h, EGS_MODE_RESCAN, n_pods, c_off, units));
   if (h->world > 1) return fail(h, EGS_ERR_BAD_ARG, "egs_schedule_batch_vec is single-shard");
-  vec_pods = std::min(vec_pods, n_pods);
-  const size_t cells = (size_t)vec_pods * h->max_nodes;
+  BatchOut o(out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest, false);
+  o.vec_pods = std::min(vec_pods, n_pods);
+  const size_t cells = (size_t)o.vec_pods * h->max_nodes;
   if (cells > h->d_vec_fit.cap()) CK(h, grow(h->stream, false, to(h->d_vec_fit, cells), to(h->d_vec_score, cells)));
-  const PodOut o = pod_out(h, out_node, out_status, out_alloc_mask, out_fit_count, out_fit_digest, out_score_digest);
-  h->vec_pods = vec_pods;
-  const int rc = batch_common(h, EGS_MODE_RESCAN, n_pods, c_off, units, uids, o, false);
-  h->vec_pods = 0;
-  if (rc != EGS_OK) return rc;
+  o.vec_fit = h->d_vec_fit; o.vec_score = h->d_vec_score;
+  TRY(run_segments(h, EGS_MODE_RESCAN, n_pods, c_off, units, uids, o));
   if (cells) {
-    CK(h, cudaMemcpy(out_vec_fit, h->d_vec_fit, cells, cudaMemcpyDeviceToHost));
-    CK(h, cudaMemcpy(out_vec_score, h->d_vec_score, cells * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CK(h, cudaMemcpyAsync(out_vec_fit, h->d_vec_fit, cells, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaMemcpyAsync(out_vec_score, h->d_vec_score, cells * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
   }
   return EGS_OK;
 }
@@ -1162,8 +1160,9 @@ extern "C" int egs_schedule_batch_device(egs_handle *h, int mode, int n_pods, co
   Guard g(h);
   if ((uintptr_t)d_out_alloc_mask % ((uintptr_t)h->planes * h->mask_b))     // one packed word per pod (write_pod_out)
     return fail(h, EGS_ERR_BAD_ARG, "d_out_alloc_mask must be aligned to EGS_MASKS_PER_POD(c_max) * EGS_MASK_BYTES(g_max)");
-  const PodOut o = pod_out(h, d_out_node, d_out_status, d_out_alloc_mask, d_out_fit_count, d_out_fit_digest, d_out_score_digest);
-  return batch_common(h, mode, n_pods, h_c_off, h_units, nullptr, o, true);
+  TRY(check_batch(h, mode, n_pods, h_c_off, h_units));
+  const BatchOut o(d_out_node, d_out_status, d_out_alloc_mask, d_out_fit_count, d_out_fit_digest, d_out_score_digest, true);
+  return run_segments(h, mode, n_pods, h_c_off, h_units, nullptr, o);
 }
 
 // ------------------------------------------------------------------------------- sharding

@@ -198,15 +198,15 @@ class OracleC:
             return None
         return _alloc_lists(off, idx, len(req)), sc.value
 
-    def peek_many(self, node_ids, req):
-        """The cached option of `req` on each of `node_ids`: (present bool [n], score int64 [n], GPU masks u16 [n, 4],
-        one per container, up to 16 GPUs)."""
+    def peek_many(self, node_ids, req, planes: int = 4):
+        """The cached option of `req` on each of `node_ids`: (present bool [n], score int64 [n], GPU masks u16
+        [n, planes], one per container, up to 16 GPUs)."""
         units, nc = _units(req), len(req)
         off, idx, sc = np.zeros(nc + 1, np.int32), np.zeros(16 * nc + 1, np.int32), C.c_int64(0)
         offp, idxp = _ptr(off), _ptr(idx)
         present = np.zeros(len(node_ids), bool)
         score = np.zeros(len(node_ids), np.int64)
-        masks = np.zeros((len(node_ids), 4), np.uint16)
+        masks = np.zeros((len(node_ids), planes), np.uint16)
         for i, n in enumerate(node_ids):
             if self.L.egso_peek(self.h, int(n), nc, units, C.byref(sc), offp, idxp):
                 present[i], score[i] = True, sc.value

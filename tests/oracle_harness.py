@@ -1,6 +1,6 @@
 """One cluster on a library handle and on the C oracle, and the comparisons the GPU tests make between them: the six
-per-pod outputs, node rows, option caches, an in-process shard group against the unsharded run, and a pod-by-pod
-oracle driver whose masks keep all 16 GPUs.
+per-pod outputs, node rows, option caches, an in-process shard group against the unsharded run, and the one pod-by-pod
+oracle driver, whose masks keep all 16 GPUs.
 
 Importing this module loads neither libegs nor a GPU: `egs()` imports the package on first use."""
 import threading
@@ -22,10 +22,10 @@ class Cluster:
     """nodes: [(gpu_count, mem_total per GPU, (core row, mem row) or None)].  The same cluster on a library handle
     (rows through egs_state_load, or egs_state_load_bulk for a workload) and on the oracle.  A cluster of a workload
     (anything with policy, n_nodes, gpus, mem_total and core / mem [n_nodes, gpus]) is loaded in bulk on both sides,
-    and its node list is only built when asked for."""
+    and its node list is only built when asked for.  c_max > 4 makes the handle a sidecar handle."""
 
-    def __init__(self, policy, nodes, g_max=8):
-        self.policy, self._nodes, self.g_max = policy, nodes, g_max
+    def __init__(self, policy, nodes, g_max=8, c_max=4):
+        self.policy, self._nodes, self.g_max, self.c_max = policy, nodes, g_max, c_max
         self.workload = None
 
     @classmethod
@@ -46,7 +46,7 @@ class Cluster:
         return self.workload.n_nodes if self.workload is not None else len(self._nodes)
 
     def handle(self, world=1, rank=0):
-        e = egs().Egs(self.policy, self.n_nodes, self.g_max)
+        e = egs().Egs(self.policy, self.n_nodes, self.g_max, c_max=self.c_max)
         if world > 1:
             e.shard_set(rank, world)
         w = self.workload
@@ -97,15 +97,16 @@ def compare_rows(e, o, nodes):
 
 
 def compare_caches(e, o, shapes, nodes, unfit_check):
-    """Option cache of every shape on `nodes`: presence, score and masks equal the oracle's, at the mask width of the
-    handle's option_dump (u8, or u16 on a wide handle).  With unfit_check, a node the library marks "known not to fit"
-    (option_dump state 2) must not fit in the oracle either."""
+    """Option cache of every shape on `nodes`: presence, score and masks equal the oracle's, at the mask width and
+    plane count of the handle's option_dump (u8, or u16 on a wide handle; 4 planes, or 8 on a sidecar handle).  With
+    unfit_check, a node the library marks "known not to fit" (option_dump state 2) must not fit in the oracle either."""
     nodes = np.asarray(sorted(nodes), np.int64)
     for sh in shapes:
         st, sc, am = e.option_dump(list(sh))
         assert am.dtype == egs().capi.mask_dtype(e.g_max), f"shape {sh}: mask dtype {am.dtype}"
+        assert am.shape[1] == e.n_masks, f"shape {sh}: {am.shape[1]} mask planes"
         st, sc, am = st[nodes], sc[nodes], am[nodes]
-        present, score, masks = o.peek_many(nodes, sh)
+        present, score, masks = o.peek_many(nodes, sh, e.n_masks)
         bad = np.nonzero(present != (st == 1))[0]
         assert bad.size == 0, f"shape {sh}: cache presence differs on nodes {nodes[bad[:5]].tolist()} " \
                               f"(library state {st[bad[:5]].tolist()})"
@@ -214,20 +215,25 @@ def pod_request(units, c_off, p):
     return [tuple(int(x) for x in units[k]) for k in range(int(c_off[p]), int(c_off[p + 1]))]
 
 
-def oracle_batch(o, c_off, units, uids, muts=(), mut_at=()):
-    """The driver rule on the oracle pod by pod with its own verbs -- filter every node, score the fit ones, bind the
-    first maximal -- so the masks keep all 16 GPUs (egso_schedule_batch's hold 8).  Records muts[j] apply right before
-    pod mut_at[j]."""
+def oracle_batch(o, c_off, units, uids, muts=(), mut_at=(), node_ids=None, planes=4):
+    """The driver rule on the oracle pod by pod with its own verbs -- filter the pod's nodes, score the fit ones, bind
+    the first maximal -- so the masks keep all 16 GPUs (egso_schedule_batch's hold 8), in `planes` planes (4, or 8 for
+    a sidecar handle).  Records muts[j] apply right before pod mut_at[j].  node_ids[p] is the ascending node list
+    kube-scheduler passes pod p (egs_schedule_batch_nodes); None: every node."""
     mix = o.L.egso_mix64
     P = len(c_off) - 1
-    out = dict(node=np.full(P, -1, np.int32), status=np.zeros(P, np.int32), alloc_mask=np.zeros((P, 4), np.uint16),
+    out = dict(node=np.full(P, -1, np.int32), status=np.zeros(P, np.int32), alloc_mask=np.zeros((P, planes), np.uint16),
                fit_count=np.zeros(P, np.int32), fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
     j = 0
     for p in range(P):
         while j < len(mut_at) and mut_at[j] == p:
             oracle_mut(o, muts[j]); j += 1
         req = pod_request(units, c_off, p)
-        ids = np.flatnonzero(o.filter(None, req)).astype(np.int32)
+        if node_ids is None:
+            ids = np.flatnonzero(o.filter(None, req)).astype(np.int32)
+        else:
+            cand = np.ascontiguousarray(node_ids[p], np.int32)
+            ids = cand[o.filter(cand, req).astype(bool)] if len(cand) else cand
         out["fit_count"][p] = len(ids)
         if len(ids) == 0:
             out["status"][p] = 1

@@ -28,6 +28,9 @@ def test_guards_and_bad_arguments():
     assert st == 0 and list(sc) == [0, 0]                                     # ScoreMin, scheduler.go:176-179
     assert e.bind(1, [(10, 1, 0)], 1)[0] == cap.EGS_ERR_NO_NODE
     assert e.pod_apply(0, [(0, 0, 1)], [[7]], 5) == cap.EGS_ERR_BAD_ARG       # GPU index out of range (Go would panic)
+    vec_fit, vec_score = np.zeros(8, np.uint8), np.zeros(8, np.int32)
+    assert e.L.egs_schedule_batch_vec(e.h, -1, None, None, None, 1, cap._p(vec_fit), cap._p(vec_score),
+                                      *[None] * 6) == cap.EGS_ERR_BAD_ARG     # n_pods < 0, before any vector is sized
 
 
 def test_whole_gpu_larger_than_node_and_sentinel_only():

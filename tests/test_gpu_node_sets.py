@@ -1,11 +1,10 @@
 """egs_schedule_batch_nodes: candidate node sets per pod, against the oracle driven with the same node lists
-(node_set_oracle.oracle_batch_nodes).  Every case compares the six per-pod outputs, the final rows of every node and the
-option cache of every shape on every node, "known not to fit" marks included."""
+(oracle_harness.oracle_batch with node_ids).  Every case compares the six per-pod outputs, the final rows of every node
+and the option cache of every shape on every node, "known not to fit" marks included."""
 import numpy as np
 import pytest
 
-from node_set_oracle import oracle_batch_nodes
-from oracle_harness import Cluster, compare_caches, compare_outputs, compare_rows, egs
+from oracle_harness import Cluster, compare_caches, compare_outputs, compare_rows, egs, oracle_batch
 from shard_groups import ShardGroup, hetero_nodes, mixed_shapes
 import wave_clusters as wc
 
@@ -20,17 +19,6 @@ def _batch(rng, shapes, n_pods):
     units = np.array([u for p in pick for u in shapes[p]], np.int32).reshape(-1, 3)
     c_off = np.concatenate([[0], np.cumsum([len(shapes[p]) for p in pick])]).astype(np.int32)
     return c_off, units
-
-
-def _handle(cl, c_max=4):
-    if c_max == 4:
-        return cl.handle()
-    e = egs().Egs(cl.policy, cl.n_nodes, cl.g_max, c_max=c_max)
-    for n, (g, mt, rows) in enumerate(cl.nodes):
-        assert e.node_set_allocatable(n, 100 * g, mt * g) == 0
-        if rows is not None:
-            assert e.state_load(n, rows[0], rows[1]) == 0
-    return e
 
 
 def _lists(sets, pod_set, P):
@@ -87,7 +75,7 @@ def test_random_sets_8_wide(kind, run, density):
     pod_set = _runs(P, run or P, len(sets))
     e, o = cl.handle(), cl.oracle()
     got = e.schedule_batch_nodes(c_off, units, sets, pod_set, uids, mode=RESCAN if kind == "rescan" else ROUNDS)
-    ref = oracle_batch_nodes(o, c_off, units, uids, _lists(sets, pod_set, P))
+    ref = oracle_batch(o, c_off, units, uids, node_ids=_lists(sets, pod_set, P))
     _check(e, o, shapes, ref, got, f"{kind} run {run} density {density}")
 
 
@@ -109,7 +97,7 @@ def test_random_sets_wide(run, density):
     pod_set = _runs(P, run or P, 2)
     e, o = cl.handle(), cl.oracle()
     got = e.schedule_batch_nodes(c_off, units, sets, pod_set, uids)
-    ref = oracle_batch_nodes(o, c_off, units, uids, _lists(sets, pod_set, P))
+    ref = oracle_batch(o, c_off, units, uids, node_ids=_lists(sets, pod_set, P))
     _check(e, o, shapes, ref, got, f"wide run {run} density {density}")
 
 
@@ -122,7 +110,7 @@ def test_random_sets_sidecar(run, density):
         g = int(rng.integers(1, 9))
         core = [int(rng.choice([100, 100, 60, 0])) for _ in range(g)]
         nodes.append((g, 32, (core, [32 if c == 100 else int(rng.integers(0, 33)) for c in core])))
-    cl = Cluster(run & 1, nodes)
+    cl = Cluster(run & 1, nodes, c_max=8)
     split = ((10, 2, 0), SENT, SENT, SENT, SENT, (0, 0, 1))         # 5 branching on 8 GPUs: the leaf-split Trade
     shapes = [split, ((20, 4, 0), SENT, SENT), ((0, 0, 1),), ((0, 0, 1), SENT, SENT, SENT, SENT, SENT, (5, 1, 0))]
     P = 120
@@ -130,20 +118,10 @@ def test_random_sets_sidecar(run, density):
     uids = np.arange(1, P + 1, dtype=np.uint64)
     sets = _sets(rng, 2, cl.n_nodes, density)
     pod_set = _runs(P, run or P, 2)
-    e, o = _handle(cl, c_max=8), cl.oracle()
+    e, o = cl.handle(), cl.oracle()
     got = e.schedule_batch_nodes(c_off, units, sets, pod_set, uids)
-    ref = oracle_batch_nodes(o, c_off, units, uids, _lists(sets, pod_set, P))
-    compare_outputs(ref, got, f"sidecar run {run} density {density}")
-    compare_rows(e, o, range(cl.n_nodes))
-    for sh in shapes:                                               # all 8 masks of every cached option
-        st, sc, am = e.option_dump(list(sh))
-        for i in range(cl.n_nodes):
-            want = o.peek(i, list(sh))
-            if want is None:
-                assert st[i] != 1 and (st[i] != 2 or o.trade(i, list(sh)) is None), f"shape {sh} node {i}"
-            else:
-                masks = [sum(1 << g for g in a) for a in want[0]] + [0] * (8 - len(want[0]))
-                assert st[i] == 1 and sc[i] == want[1] and am[i].tolist() == masks, f"shape {sh} node {i}"
+    ref = oracle_batch(o, c_off, units, uids, node_ids=_lists(sets, pod_set, P), planes=8)
+    _check(e, o, shapes, ref, got, f"sidecar run {run} density {density}")
 
 
 # ------------------------------------------------------------------------------------------------ 3. stale caches
@@ -157,14 +135,14 @@ def test_excluded_node_keeps_its_stale_option(mode):
     uids = np.arange(1, 41, dtype=np.uint64)
     every = np.ones(64, bool)
     got = e.schedule_batch_nodes(c_off, units, [every], uids=uids, mode=mode)      # every node caches both shapes
-    compare_outputs(oracle_batch_nodes(o, c_off, units, uids, _lists([every], None, 40)), got, "warm-up")
+    compare_outputs(oracle_batch(o, c_off, units, uids, node_ids=_lists([every], None, 40)), got, "warm-up")
     before = [e.option_dump(list(sh)) for sh in shapes]
     X = int(np.flatnonzero((before[0][0] == 1) & (before[1][0] == 1))[0])   # a node caching both shapes
     no_x = every.copy(); no_x[X] = False
     c_off, units = _batch(rng, shapes, 60)
     uids = np.arange(100, 160, dtype=np.uint64)
     got = e.schedule_batch_nodes(c_off, units, [no_x], uids=uids, mode=mode)
-    compare_outputs(oracle_batch_nodes(o, c_off, units, uids, _lists([no_x], None, 60)), got, "X excluded")
+    compare_outputs(oracle_batch(o, c_off, units, uids, node_ids=_lists([no_x], None, 60)), got, "X excluded")
     for sh, b in zip(shapes, before):
         for x, y in zip(b, e.option_dump(list(sh))):
             assert np.array_equal(x[X], y[X]), f"shape {sh}: the option of the excluded node changed"
@@ -174,7 +152,7 @@ def test_excluded_node_keeps_its_stale_option(mode):
     c_off, units = _batch(rng, shapes, 60)
     uids = np.arange(200, 260, dtype=np.uint64)
     got = e.schedule_batch_nodes(c_off, units, [every], uids=uids, mode=mode)
-    ref = oracle_batch_nodes(o, c_off, units, uids, _lists([every], None, 60))
+    ref = oracle_batch(o, c_off, units, uids, node_ids=_lists([every], None, 60))
     _check(e, o, shapes, ref, got, "X admitted again")
 
 
@@ -192,7 +170,7 @@ def test_cold_shapes_leave_excluded_nodes_absent():
     c_off, units = _batch(rng, shapes, 200)
     uids = np.arange(1, 201, dtype=np.uint64)
     got = e.schedule_batch_nodes(c_off, units, [s], uids=uids, mode=ROUNDS)
-    ref = oracle_batch_nodes(o, c_off, units, uids, _lists([s], None, 200))
+    ref = oracle_batch(o, c_off, units, uids, node_ids=_lists([s], None, 200))
     _check(e, o, shapes, ref, got, "cold shapes")
     for sh in shapes:
         st = e.option_dump(list(sh))[0]
@@ -217,7 +195,7 @@ def test_shard_group(world):
     pod_set = _runs(P, 13, 3)
     e, o = cl.handle(), cl.oracle()
     twin = e.schedule_batch_nodes(c_off, units, sets, pod_set, uids, mode=ROUNDS)
-    ref = oracle_batch_nodes(o, c_off, units, uids, _lists(sets, pod_set, P))
+    ref = oracle_batch(o, c_off, units, uids, node_ids=_lists(sets, pod_set, P))
     _check(e, o, shapes, ref, twin, f"world {world}, unsharded")
     with ShardGroup(cl, world) as g:
         outs = g.each(lambda r, h: h.schedule_batch_nodes(c_off, units, sets, pod_set, uids, mode=ROUNDS))
@@ -256,7 +234,7 @@ def test_wave_cluster_chunk_edges():
     pod_set = _runs(P, 50, 3)
     e, o = cl.handle(), cl.oracle()
     got = e.schedule_batch_nodes(c_off, units, sets, pod_set, uids, mode=ROUNDS)
-    ref = oracle_batch_nodes(o, c_off, units, uids, _lists(sets, pod_set, P))
+    ref = oracle_batch(o, c_off, units, uids, node_ids=_lists(sets, pod_set, P))
     compare_outputs(ref, got, "wave cluster")
     touched = set(int(x) for x in ref["node"] if x >= 0) | set(range(0, n, 97))
     compare_rows(e, o, touched)
@@ -327,5 +305,5 @@ def test_checkpoint_rollback_and_library_uids():
     again = e.schedule_batch_nodes(c_off, units, sets, pod_set, mode=ROUNDS)
     compare_outputs(first, again, "rerun after rollback")
     o = cl.oracle()
-    ref = oracle_batch_nodes(o, c_off, units, np.arange(base, base + P, dtype=np.uint64), _lists(sets, pod_set, P))
+    ref = oracle_batch(o, c_off, units, np.arange(base, base + P, dtype=np.uint64), node_ids=_lists(sets, pod_set, P))
     _check(e, o, shapes, ref, again, "checkpoint rerun")

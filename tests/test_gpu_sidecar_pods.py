@@ -1,90 +1,23 @@
 """Sidecar handles (egs_create_ex with c_max > 4): pods of 5..8 containers through filter, score, bind, peek,
 option_dump and the per-pod batch engine, against the C oracle, on both sides of the one-thread DFS / leaf-split
-threshold.  The oracle's own verbs are driven pod by pod here, so that all 8 masks of a pod are compared."""
+threshold.  The oracle's own verbs are driven pod by pod (oracle_batch with 8 planes), so that all 8 masks of a pod
+are compared."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
-import oracle_c as oc
-from oracle_harness import FIELDS, M64, egs
+from oracle_harness import FIELDS, Cluster, compare_caches, compare_outputs, compare_rows, egs, oracle_batch
 
 pytestmark = pytest.mark.gpu
 
 SENT = (-1, -1, 0)
 
 
-def _pair(policy, nodes, c_max=8, g_max=8):
+def _pair(policy, nodes, g_max=8):
     """nodes: [(gpus, mem_total, rows or None)] on a sidecar handle and on the oracle."""
-    e = egs().Egs(policy, len(nodes), g_max, c_max=c_max)
-    o = oc.OracleC(policy)
-    for i, (g, mt, rows) in enumerate(nodes):
-        assert e.node_set(i, g, mt) == 0 and o.add_node(100 * g, mt * g) == i
-        if rows is not None:
-            assert e.state_load(i, rows[0], rows[1]) == 0
-            o.set_rows(i, rows[0], rows[1])
-    return e, o
-
-
-def _masks(alloc, n=8):
-    m = np.zeros(n, np.uint8)
-    for c, a in enumerate(alloc or []):
-        m[c] = sum(1 << g for g in a)
-    return m
-
-
-def _rows_equal(e, o, n):
-    for i in range(n):
-        assert e.rows(i) == o.rows(i), f"rows of node {i}"
-
-
-def _caches_equal(e, o, shapes, n):
-    for sh in shapes:
-        st, sc, am = e.option_dump(list(sh))
-        assert am.shape[1] == 8
-        for i in range(n):
-            want = o.peek(i, list(sh))
-            if want is None:
-                assert st[i] != 1, f"shape {sh} node {i}: cached, the oracle has no entry"
-                if st[i] == 2:
-                    assert o.trade(i, list(sh)) is None
-            else:
-                assert st[i] == 1 and sc[i] == want[1], f"shape {sh} node {i}"
-                assert np.array_equal(am[i], _masks(want[0])), f"shape {sh} node {i}: masks"
-
-
-def oracle_batch8(o, c_off, units, uids):
-    """The driver rule on the oracle with its own verbs, masks of all 8 containers kept."""
-    mix = o.L.egso_mix64
-    P = len(c_off) - 1
-    out = dict(node=np.full(P, -1, np.int32), status=np.zeros(P, np.int32), alloc_mask=np.zeros((P, 8), np.uint8),
-               fit_count=np.zeros(P, np.int32), fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
-    for p in range(P):
-        req = [tuple(int(x) for x in units[k]) for k in range(int(c_off[p]), int(c_off[p + 1]))]
-        ids = np.flatnonzero(o.filter(None, req)).astype(np.int32)
-        out["fit_count"][p] = len(ids)
-        if len(ids) == 0:
-            out["status"][p] = 1
-            continue
-        st, sc = o.score(ids, req)
-        assert st == 0
-        fd = sd = 0
-        for i, s in zip(ids, sc):
-            fd = (fd + mix(2 * int(i) + 1)) & M64
-            sd = (sd + mix(2 * int(i) + 2) * (2 * int(s) + 1)) & M64
-        out["fit_digest"][p], out["score_digest"][p] = fd, sd
-        w = int(ids[int(np.argmax(sc))])
-        st, alloc = o.bind(w, req, int(uids[p]))
-        out["node"][p], out["status"][p] = w, st
-        if st == 0:
-            out["alloc_mask"][p] = _masks(alloc)
-    return out
-
-
-def _compare(ref, got, what):
-    for f in FIELDS:
-        bad = np.nonzero(ref[f] != got[f])[0]
-        assert bad.size == 0, f"{what}: {f} differs first at pod {bad[:3].tolist()}"
+    cl = Cluster(policy, nodes, g_max, c_max=8)
+    return cl.handle(), cl.oracle()
 
 
 def _batch(pods):
@@ -165,7 +98,7 @@ def test_device_masks_need_8_byte_alignment():
         e.schedule_batch_device(c_off, units, [0, 0, buf.data_ptr() + 4, 0, 0, 0])
     e.schedule_batch_device(c_off, units, [0, 0, buf.data_ptr() + 8, 0, 0, 0])
     torch.cuda.synchronize()
-    ref = oracle_batch8(o, c_off, units, np.arange(2) + 1000000)
+    ref = oracle_batch(o, c_off, units, np.arange(2) + 1000000, planes=8)
     assert np.array_equal(buf[8:24].cpu().numpy().reshape(2, 8), ref["alloc_mask"])
 
 
@@ -179,7 +112,7 @@ def test_last_maximal_leaf_under_ties(policy, n_sent):
     assert list(e.filter(None, req)) == list(o.filter(None, req))
     for i in range(2):
         assert e.peek(i, req) == o.peek(i, req)
-    _caches_equal(e, o, [req], 2)
+    compare_caches(e, o, [req], range(2), unfit_check=True)
 
 
 def test_sentinel_makes_a_whole_gpu_container_skip_a_gpu():
@@ -189,7 +122,7 @@ def test_sentinel_makes_a_whole_gpu_container_skip_a_gpu():
     assert list(e.filter(None, req)) == list(o.filter(None, req)) == [1]
     assert e.peek(0, req) == o.peek(0, req)
     assert e.bind(0, req, 5) == o.bind(0, req, 5)
-    _rows_equal(e, o, 1)
+    compare_rows(e, o, range(1))
 
 
 def test_stale_option_fails_in_transact():
@@ -200,8 +133,8 @@ def test_stale_option_fails_in_transact():
     assert e.pod_apply(0, other, alloc, 9) == 0 and o.add_pod(0, other, alloc, 9) == 0
     got = e.bind(0, req, 10)
     assert got == o.bind(0, req, 10) and got[0] == egs().capi.EGS_ERR_TRANSACT
-    _rows_equal(e, o, 2)
-    _caches_equal(e, o, [req], 2)
+    compare_rows(e, o, range(2))
+    compare_caches(e, o, [req], range(2), unfit_check=True)
 
 
 @pytest.mark.parametrize("policy", [0, 1])
@@ -209,13 +142,13 @@ def test_two_bit_digits_on_a_four_gpu_sidecar_handle(policy):
     """g_max = 4: digits are 2 bits wide, so 7 branching containers (2^14 leaves) take the leaf-split kernels, and a
     node with fewer GPUs meets digits that name absent GPUs."""
     rows = ([100, 37, 100], [32, 9, 32])
-    e, o = _pair(policy, [(4, 32, None), (3, 32, rows), (1, 32, None), (2, 32, ([60, 0], [20, 0]))], g_max=4)
+    e, o = _pair(policy, [(4, 32, None), (3, 32, rows), (1, 32, None), (2, 32, ([60, 0], [20, 0]))], 4)
     for req in ([(10, 4, 0)] + [SENT] * 6, [SENT, (0, 0, 1), SENT, (20, 5, 0)] + [SENT] * 4, [SENT] * 6):
         assert list(e.filter(None, req)) == list(o.filter(None, req)), req
-        _caches_equal(e, o, [req], 4)
+        compare_caches(e, o, [req], range(4), unfit_check=True)
         for i in range(4):
             assert e.bind(i, req, 40 + i) == o.bind(i, req, 40 + i)
-        _rows_equal(e, o, 4)
+        compare_rows(e, o, range(4))
 
 
 @pytest.mark.parametrize("req", [[SENT] * 5, [SENT] * 4 + [(0, 0, 1)]])
@@ -226,7 +159,7 @@ def test_score_without_filter_is_the_reference_panic(req):
     st, sc = e.score([0, 1, 2], req)
     ost, osc = o.score([0, 1, 2], req)
     assert st == ost == egs().capi.EGS_ERR_PANIC and list(sc) == list(osc)
-    _caches_equal(e, o, [req], 3)
+    compare_caches(e, o, [req], range(3), unfit_check=True)
 
 
 @pytest.mark.parametrize("policy", [0, 1])
@@ -238,7 +171,7 @@ def test_one_node_with_2_24_leaves(policy):
     assert list(e.filter(None, req)) == list(o.filter(None, req)) == [1]
     assert e.peek(0, req) == o.peek(0, req)
     assert e.bind(0, req, 1) == o.bind(0, req, 1)
-    _rows_equal(e, o, 1)
+    compare_rows(e, o, range(1))
 
 
 # ------------------------------------------------------------------------------------------------ sequences
@@ -268,8 +201,8 @@ def test_verb_sequences_against_the_oracle(policy, seed):
             rec = [(5, 2, 0), (0, 0, 1)]
             alloc = [[int(rng.integers(0, g))], [int(rng.integers(0, g))]]
             assert e.pod_apply(w, rec, alloc, uid) == o.add_pod(w, rec, alloc, uid)
-        _rows_equal(e, o, n)
-        _caches_equal(e, o, shapes, n)
+        compare_rows(e, o, range(n))
+        compare_caches(e, o, shapes, range(n), unfit_check=True)
 
 
 @pytest.mark.parametrize("policy", [0, 1])
@@ -279,7 +212,7 @@ def test_batches_against_the_oracle_driver(policy):
     nodes = _cluster(rng, 40)
     pods = [_pod(rng, 5 if p % 3 else 3) for p in range(30)] + [[(10, 4, 0)], [(0, 0, 2), SENT]]
     c_off, units = _batch(pods)
-    ref = oracle_batch8(_pair(policy, nodes)[1], c_off, units, np.arange(len(pods)) + 1000000)
+    ref = oracle_batch(Cluster(policy, nodes).oracle(), c_off, units, np.arange(len(pods)) + 1000000, planes=8)
     for call in ("batch", "mut", "vec", "device"):
         e, o = _pair(policy, nodes)
         if call == "batch":
@@ -299,22 +232,22 @@ def test_batches_against_the_oracle_driver(policy):
             got = {f: t[f].cpu().numpy() for f in FIELDS}
             got["alloc_mask"] = got["alloc_mask"].reshape(P, 8)
             got["fit_digest"] = got["fit_digest"].view(np.uint64); got["score_digest"] = got["score_digest"].view(np.uint64)
-        _compare(ref, got, call)
+        compare_outputs(ref, got, call)
         if call == "batch":
-            oracle_batch8(o, c_off, units, np.arange(len(pods)) + 1000000)
-            _rows_equal(e, o, len(nodes))
-            _caches_equal(e, o, [tuple(p) for p in pods[:6]], len(nodes))
+            oracle_batch(o, c_off, units, np.arange(len(pods)) + 1000000, planes=8)
+            compare_rows(e, o, range(len(nodes)))
+            compare_caches(e, o, [tuple(p) for p in pods[:6]], range(len(nodes)), unfit_check=True)
 
 
 def test_oracle_driver_equals_egso_schedule_batch():
-    """Pins the driver above to the oracle's own batch on pods of up to 4 containers."""
+    """Pins the harness driver's 8-plane mode to the oracle's own batch on pods of up to 4 containers."""
     rng = np.random.default_rng(11)
     nodes = _cluster(rng, 30)
     pods = [[(int(rng.integers(5, 60)), int(rng.integers(1, 12)), 0)] + [SENT] * int(rng.integers(0, 3)) for _ in range(25)]
     c_off, units = _batch(pods)
     uids = np.arange(len(pods), dtype=np.uint64) + 5
-    a = oracle_batch8(_pair(0, nodes)[1], c_off, units, uids)
-    b = _pair(0, nodes)[1].schedule_batch(c_off, units.astype(np.int64), uids)
+    a = oracle_batch(Cluster(0, nodes).oracle(), c_off, units, uids, planes=8)
+    b = Cluster(0, nodes).oracle().schedule_batch(c_off, units.astype(np.int64), uids)
     for f in FIELDS:
         x = a[f][:, :4] if f == "alloc_mask" else a[f]
         assert np.array_equal(x, b[f]), f
@@ -337,7 +270,7 @@ def test_checkpoint_rollback_with_8_plane_tables():
         assert np.array_equal(st, st2) and np.array_equal(sc[st == 1], sc2[st == 1]) and np.array_equal(am[st == 1], am2[st == 1])
     assert all(np.array_equal(x, y) for x, y in zip(rows, e.state_dump()))
     b = e.schedule_batch(*_batch(pods[4:]))
-    _compare(a, b, "after rollback")
+    compare_outputs(a, b, "after rollback")
 
 
 @pytest.mark.parametrize("mode", [1, 2])

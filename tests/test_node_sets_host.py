@@ -1,11 +1,10 @@
 """Candidate node sets on the CPU: the oracle driver with per-pod node lists, and the bitmap packing of the binding.
-With every node listed, oracle_batch_nodes (tests/node_set_oracle.py) is egso_schedule_batch and oracle_batch; a pod's
-list keeps it off every other node."""
+With every node listed, oracle_batch(node_ids=...) is egso_schedule_batch and oracle_batch without lists; a pod's list
+keeps it off every other node."""
 import numpy as np
 import pytest
 
 import oracle_c as oc
-from node_set_oracle import oracle_batch_nodes
 from oracle_harness import Cluster, compare_outputs, compare_rows, egs, oracle_batch
 
 PODS = [((30, 4, 0),), ((0, 0, 1),), ((10, 2, 0), (-1, -1, 0)), ((0, 0, 2),)]
@@ -30,7 +29,7 @@ def test_all_nodes_listed_is_the_batch(seed):
     o_ref, o = cl.oracle(), cl.oracle()
     ref = o_ref.schedule_batch(c_off, units.astype(np.int64), uids)
     every = [np.arange(cl.n_nodes, dtype=np.int32)] * (len(c_off) - 1)
-    got = oracle_batch_nodes(o, c_off, units, uids, every)
+    got = oracle_batch(o, c_off, units, uids, node_ids=every)
     assert (got["alloc_mask"] < 256).all()                      # 8-GPU nodes: the masks fit egso's bytes
     got["alloc_mask"] = got["alloc_mask"].astype(np.uint8)
     compare_outputs(ref, got, f"seed {seed}")
@@ -45,7 +44,7 @@ def test_lists_keep_pods_on_their_nodes():
     rng = np.random.default_rng(3)
     lists = [np.sort(rng.choice(cl.n_nodes, int(rng.integers(0, cl.n_nodes)), replace=False)).astype(np.int32)
              for _ in range(P)]
-    out = oracle_batch_nodes(cl.oracle(), c_off, units, uids, lists)
+    out = oracle_batch(cl.oracle(), c_off, units, uids, node_ids=lists)
     for p in range(P):
         assert out["node"][p] == -1 or out["node"][p] in lists[p]
         assert out["fit_count"][p] <= len(lists[p])

@@ -16,7 +16,7 @@ class Dump:
 
     def __init__(self, o, g_max):
         cap = egs().capi
-        self.g_max, n = g_max, o.n_nodes
+        self.g_max, self.n_masks, n = g_max, 4, o.n_nodes
         self.core = np.full((n, cap.row_width(g_max)), cap.EGS_PAD, np.int32)
         self.mem, self.gc = self.core.copy(), np.zeros(n, np.int32)
         for i in range(n):
@@ -79,7 +79,7 @@ def _node(lib, want):
     return int(i[0])
 
 
-CHANGES = ["row", "pad", "presence", "score", "mask", "unfit", "rank_output", "shard_row"] + [f"output_{f}" for f in FIELDS]
+CHANGES = ["row", "pad", "presence", "score", "mask", "planes", "unfit", "rank_output", "shard_row"] + [f"output_{f}" for f in FIELDS]
 
 
 @pytest.mark.parametrize("g_max", [8, 16])
@@ -107,6 +107,8 @@ def test_single_cell_change_fails(g_max, change):
         sc[_node(lib, 1)] += 1
     elif change == "mask":
         am[_node(lib, 1), 2] ^= 1 << (8 * am.itemsize - 1)          # the top GPU of container 2
+    elif change == "planes":
+        lib.n_masks = 8                                               # 4 planes dumped by an 8-plane handle
     elif change == "unfit":
         st[_node(lib, 0)] = 2                                         # a node that fits, marked "does not fit"
     elif change.startswith("output_"):

@@ -98,7 +98,7 @@ class _Dump:
 
     def __init__(self, o, shapes):
         cap = egs().capi
-        self.g_max, n = 8, o.n_nodes
+        self.g_max, self.n_masks, n = 8, 4, o.n_nodes
         self.core = np.full((n, cap.row_width(8)), cap.EGS_PAD, np.int32)
         self.mem, self.gc = self.core.copy(), np.zeros(n, np.int32)
         for i in range(n):
