@@ -22,7 +22,8 @@ class Cluster:
     """nodes: [(gpu_count, mem_total per GPU, (core row, mem row) or None)].  The same cluster on a library handle
     (rows through egs_state_load, or egs_state_load_bulk for a workload) and on the oracle.  A cluster of a workload
     (anything with policy, n_nodes, gpus, mem_total and core / mem [n_nodes, gpus]) is loaded in bulk on both sides,
-    and its node list is only built when asked for.  c_max > 4 makes the handle a sidecar handle."""
+    and its node list is only built when asked for.  c_max > 4 makes the handle a sidecar handle.  A None node is an id
+    never set on the handle; the oracle, whose ids are dense, holds a 1-GPU placeholder there that a test never lists."""
 
     def __init__(self, policy, nodes, g_max=8, c_max=4):
         self.policy, self._nodes, self.g_max, self.c_max = policy, nodes, g_max, c_max
@@ -53,7 +54,10 @@ class Cluster:
         if w is not None:
             e.state_load_bulk(0, w.gpus, w.mem_total, w.core, w.mem)
             return e
-        for n, (g, mt, rows) in enumerate(self.nodes):
+        for n, nd in enumerate(self.nodes):
+            if nd is None:
+                continue
+            g, mt, rows = nd
             assert e.node_set_allocatable(n, 100 * g, mt * g) == 0
             if rows is not None:
                 assert e.state_load(n, rows[0], rows[1]) == 0
@@ -65,7 +69,8 @@ class Cluster:
         if w is not None:
             assert o.add_nodes(w.gpus, w.mem_total * w.gpus, w.core, w.mem) == 0
             return o
-        for n, (g, mt, rows) in enumerate(self.nodes):
+        for n, nd in enumerate(self.nodes):
+            g, mt, rows = nd or (1, 1, None)
             assert o.add_node(100 * g, mt * g) == n
             if rows is not None:
                 o.set_rows(n, rows[0], rows[1])
