@@ -19,6 +19,7 @@ EGS_BINPACK, EGS_SPREAD = 0, 1
 EGS_MODE_AUTO, EGS_MODE_RESCAN, EGS_MODE_ROUNDS = 0, 1, 2
 EGS_K_EVALUATE, EGS_K_PASS, EGS_K_SELECT, EGS_K_RESOLVE = 0, 1, 2, 3
 EGS_PAD = -(1 << 31)
+EGS_HEADROOM_MAX_LIMIT = 1 << 18
 
 
 def row_width(g_max: int) -> int:
@@ -42,7 +43,7 @@ SYMBOLS = [
     "egs_state_snapshot", "egs_state_restore", "egs_checkpoint_save", "egs_checkpoint_rollback", "egs_checkpoint_drop",
     "egs_filter", "egs_score", "egs_bind", "egs_option_peek", "egs_option_dump", "egs_pod_apply", "egs_node_replay_pod", "egs_pod_cancel",
     "egs_mutations_apply", "egs_schedule_batch_mut", "egs_pod_known", "egs_pod_released", "egs_schedule_batch", "egs_schedule_batch_vec", "egs_schedule_batch_device",
-    "egs_schedule_batch_nodes",
+    "egs_schedule_batch_nodes", "egs_headroom",
     "egs_shard_set", "egs_shard_range", "egs_comm_unique_id", "egs_comm_init", "egs_comm_init_local", "egs_profile_evaluate", "egs_profile_get",
     "egs_profile_reset", "egs_get_stream", "egs_rounds_stats", "egs_mix64",
 ]
@@ -105,6 +106,7 @@ def load(build: bool = True):
     L.egs_schedule_batch_vec.argtypes = [vp, i32, vp, vp, vp, i32, vp, vp] + [vp] * 6
     L.egs_schedule_batch_device.argtypes = [vp, i32, i32, vp, vp] + [vp] * 6
     L.egs_schedule_batch_nodes.argtypes = [vp, i32, i32, vp, vp, vp, i32, vp, vp] + [vp] * 6
+    L.egs_headroom.argtypes = [vp, i32, vp, vp, i32, i32, vp, i32, vp, vp, vp]
     L.egs_shard_set.argtypes = [vp, i32, i32]
     L.egs_shard_range.argtypes = [i32, i32, i32, C.POINTER(i32), C.POINTER(i32)]
     L.egs_comm_unique_id.argtypes = [vp]
@@ -380,6 +382,26 @@ class Egs:
         args = [C.c_void_p(int(p)) if p else None for p in dptrs]
         self._ck(self.L.egs_schedule_batch_device(self.h, mode, P, _p(c_off), _p(units), *args),
                  "egs_schedule_batch_device")
+
+    # ---- capacity
+    def headroom(self, shapes, node0: int = 0, n: Optional[int] = None, node_set=None, limit: int = 1 << 16):
+        """How many more pods of each shape every node of [node0, node0+n) takes (egs_headroom): per shape a list of
+        (core, mem, count) units.  node_set: a bool array of max_nodes entries, a node-id list or one packed bitmap
+        (node_sets_array), None for every node.  Returns (count [n_shapes, n] i32, failed [n_shapes, n] i32,
+        summary [n_shapes, 4] i64: binds, nodes with a bind, failed binds, nodes stopped by `limit`)."""
+        n = self.max_nodes - node0 if n is None else n
+        S = len(shapes)
+        c_off = np.concatenate([[0], np.cumsum([len(sh) for sh in shapes])]).astype(np.int32)
+        units = units_array([u for sh in shapes for u in sh])
+        bm = None
+        if node_set is not None:
+            a = np.asarray(node_set)
+            bm = np.ascontiguousarray(a if a.dtype == np.uint64 else node_sets_array([a], self.max_nodes)[0], np.uint64)
+        count = np.zeros((S, max(n, 1)), np.int32); failed = np.zeros((S, max(n, 1)), np.int32)
+        summary = np.zeros((max(S, 1), 4), np.int64)
+        self._ck(self.L.egs_headroom(self.h, S, _p(c_off), _p(units), node0, n, _p(bm), limit, _p(count), _p(failed),
+                                     _p(summary)), "egs_headroom")
+        return count[:, :n], failed[:, :n], summary[:S]
 
     # ---- sharding / instrumentation
     def shard_set(self, rank: int, world: int):

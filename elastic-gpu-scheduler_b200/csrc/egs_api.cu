@@ -94,6 +94,7 @@ struct egs_handle {
   DeviceBuf<char> d_ops; DeviceBuf<int32_t> d_group_off;       // egs_mutations_apply: ApplyOp<row_w>[]
   DeviceBuf<uint8_t> d_vec_fit; DeviceBuf<int32_t> d_vec_score;              // egs_schedule_batch_vec
   DeviceBuf<uint64_t> d_set;                                    // egs_schedule_batch_nodes: the running run's node set
+  DeviceBuf<int32_t> d_hr; DeviceBuf<unsigned long long> d_hr_sum;   // egs_headroom: count | failed, summaries
   // profiling
   int64_t k_launches[EGS_K_COUNT] = {0}; double k_ms[EGS_K_COUNT] = {0}; int timing = 0;
   RoundsState rounds;
@@ -1163,6 +1164,75 @@ extern "C" int egs_schedule_batch_device(egs_handle *h, int mode, int n_pods, co
   TRY(check_batch(h, mode, n_pods, h_c_off, h_units));
   const BatchOut o(d_out_node, d_out_status, d_out_alloc_mask, d_out_fit_count, d_out_fit_digest, d_out_score_digest, true);
   return run_segments(h, mode, n_pods, h_c_off, h_units, nullptr, o);
+}
+
+// ------------------------------------------------------------------------------- capacity
+// Every argument is checked before a shape is interned or anything is launched.  One k_headroom launch per shape,
+// all on the stream after whatever batch is still in flight, and one synchronisation for the copies back.
+extern "C" int egs_headroom(egs_handle *h, int n_shapes, const int32_t *c_off, const egs_unit *units, int node0, int n,
+                            const uint64_t *set, int32_t limit, int32_t *out_count, int32_t *out_failed,
+                            int64_t *out_summary) {
+  if (!h) return EGS_ERR_BAD_ARG;
+  Guard g(h);
+  if (n_shapes < 1 || !c_off || !units) return fail(h, EGS_ERR_BAD_ARG, "egs_headroom: n_shapes >= 1 shapes in c_off / units");
+  if (!out_count && !out_failed && !out_summary) return fail(h, EGS_ERR_BAD_ARG, "egs_headroom: no output");
+  if (limit < 1 || limit > EGS_HEADROOM_MAX_LIMIT) return fail(h, EGS_ERR_BAD_ARG, "egs_headroom: limit outside [1, EGS_HEADROOM_MAX_LIMIT]");
+  if (node0 < 0 || n < 0 || node0 > h->max_nodes - n) return fail(h, EGS_ERR_BAD_ARG, "egs_headroom: node range outside [0, max_nodes)");
+  if (h->world > 1 && (node0 < h->lo || node0 + n > h->hi))
+    return fail(h, EGS_ERR_BAD_ARG, "egs_headroom: on a sharded handle the range must lie inside the rank's egs_shard_range");
+  const size_t words = EGS_NODE_SET_WORDS((size_t)h->max_nodes);
+  if (set && h->max_nodes % 64 && (set[words - 1] & (~0ull << (h->max_nodes % 64))))
+    return fail(h, EGS_ERR_BAD_ARG, "egs_headroom: node set bit at or beyond max_nodes");
+  for (int s = 0; s < n_shapes; s++) {
+    const int C = c_off[s + 1] - c_off[s];
+    if (c_off[s] < 0 || C < 1 || C > h->c_max) return fail(h, EGS_ERR_BAD_ARG, "egs_headroom: shape with 0 or more than c_max containers");
+    const int rc = check_units(C, units + c_off[s], h->c_max);
+    if (rc != EGS_OK) return fail(h, rc, "egs_headroom: malformed unit");
+    if (leaf_split(h, C, units + c_off[s]))
+      return fail(h, EGS_ERR_BAD_ARG, "egs_headroom: shapes Traded by the leaf-split kernels (more than 2^12 leaves) are not served");
+  }
+  std::vector<int> slots((size_t)n_shapes);
+  for (int s = 0; s < n_shapes; s++) TRY(intern(h, c_off[s + 1] - c_off[s], units + c_off[s], &slots[s]));
+  const size_t cells = (size_t)n_shapes * n;
+  if (2 * cells > h->d_hr.cap()) CK(h, grow(h->stream, false, to(h->d_hr, std::max(2 * cells, (size_t)h->n_pad))));
+  if ((size_t)n_shapes * 4 > h->d_hr_sum.cap()) CK(h, grow(h->stream, false, to(h->d_hr_sum, (size_t)n_shapes * 4)));
+  CK(h, cudaMemsetAsync(h->d_hr_sum, 0, (size_t)n_shapes * 4 * sizeof(unsigned long long), h->stream));
+  if (set) {
+    if (words > h->d_set.cap()) CK(h, grow(h->stream, false, to(h->d_set, words)));
+    CK(h, cudaMemcpyAsync(h->d_set, set, words * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+  }
+  int32_t *d_count = h->d_hr, *d_failed = d_count + cells;
+  const int grid = (n + HEADROOM_THREADS - 1) / HEADROOM_THREADS;
+  for (int s = 0; s < n_shapes && n > 0; s++) {
+    const int C = c_off[s + 1] - c_off[s];
+    const egs_unit *u = units + c_off[s];
+    by_geometry(h, [&](auto W) -> int {
+      constexpr int G = decltype(W)::G, NP = decltype(W)::NP;
+      HeadroomArgsT<ReqOf<NP>> a;
+      a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total;
+      a.node0 = node0; a.n = n; a.policy = h->policy; a.limit = limit;
+      a.req = make_req<ReqOf<NP>>(C, u); a.t = table(h, slots[s]);
+      a.count = d_count + (size_t)s * n; a.failed = d_failed + (size_t)s * n; a.summary = h->d_hr_sum + (size_t)s * 4;
+      const NodeSet ns{set ? h->d_set.get() : nullptr};
+      const bool single = is_single(C, u);
+      if (set && single) k_headroom<G, NP, true, true><<<grid, HEADROOM_THREADS, 0, h->stream>>>(a, ns);
+      else if (set) k_headroom<G, NP, false, true><<<grid, HEADROOM_THREADS, 0, h->stream>>>(a, ns);
+      else if (single) k_headroom<G, NP, true, false><<<grid, HEADROOM_THREADS, 0, h->stream>>>(a, ns);
+      else k_headroom<G, NP, false, false><<<grid, HEADROOM_THREADS, 0, h->stream>>>(a, ns);
+      return EGS_OK;
+    });
+    CK(h, cudaGetLastError());
+  }
+  TRY(ensure_stage(h, 2 * cells * sizeof(int32_t) + (size_t)n_shapes * 4 * sizeof(int64_t)));
+  int64_t *s_sum = (int64_t *)h->h_stage.get();
+  int32_t *s_cells = (int32_t *)(s_sum + (size_t)n_shapes * 4);
+  CK(h, cudaMemcpyAsync(s_sum, h->d_hr_sum, (size_t)n_shapes * 4 * sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream));
+  if (cells) CK(h, cudaMemcpyAsync(s_cells, d_count, 2 * cells * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+  CK(h, cudaStreamSynchronize(h->stream));
+  if (out_summary) memcpy(out_summary, s_sum, (size_t)n_shapes * 4 * sizeof(int64_t));
+  if (out_count) memcpy(out_count, s_cells, cells * sizeof(int32_t));
+  if (out_failed) memcpy(out_failed, s_cells + cells, cells * sizeof(int32_t));
+  return EGS_OK;
 }
 
 // ------------------------------------------------------------------------------- sharding

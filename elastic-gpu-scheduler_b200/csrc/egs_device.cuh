@@ -448,6 +448,36 @@ EGS_HD bool transact_row(int32_t *core, int32_t *mem, int mem_total, const R &r,
   return true;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Headroom of one node for one shape (egs_headroom): the binds a dry run of identical pods makes on the node.  Under
+// a stream of pods of one shape a node's Assume (node.go:61-73) and Allocate (node.go:87-104) read and write only
+// that node's rows and option entry, so its binds are these, in this order, whatever the other nodes do:
+//   1. state OPT_CACHED: the cached masks are Transacted, stale or not (a failure keeps its Adds, gpu.go:153-175);
+//      OPT_UNFIT: Trade fails on these rows, nothing binds; OPT_ABSENT: straight to 2;
+//   2. Trade on the current rows, Transact, and again, until Trade fails.
+// The row is a copy: the caller's is not written.  At most `limit` binds (successful or failed) are made; `capped`
+// says the node still had an option when the limit stopped it.
+// ---------------------------------------------------------------------------------------------
+struct Headroom { int ok, failed, capped; };
+
+template <int G, class R>
+EGS_HD Headroom headroom_node(const int (&c0)[G], const int (&m0)[G], int mem_total, const R &r, bool single,
+                              int policy, int state, PackedT<G, R::NC> masks, int limit) {
+  Headroom h = {0, 0, 0};
+  if (state == OPT_UNFIT) return h;
+  int c[G], m[G];
+#pragma unroll
+  for (int g = 0; g < G; g++) { c[g] = c0[g]; m[g] = m0[g]; }
+  int score;
+  bool have = state == OPT_CACHED || trade_any(c, m, mem_total, r, single, policy, score, masks);
+  while (have) {
+    if (h.ok + h.failed >= limit) { h.capped = 1; break; }
+    if (transact_row<G>(c, m, mem_total, r, masks)) h.ok++; else h.failed++;
+    have = trade_any(c, m, mem_total, r, single, policy, score, masks);
+  }
+  return h;
+}
+
 // One AddPod / ForgetPod row update with the option rebuilt from annotations (allocate.go:75-93): explicit index
 // lists; a fractional container uses its first index only.  A whole-GPU container lists up to G indices.
 template <int G>

@@ -11,6 +11,7 @@
 //                ForgetPod in one launch.
 // Each reference step these kernels share is written once: Assume (assume_option), Allocate
 // (allocate_option), and the AddPod / ForgetPod row update (apply_op, egs_device.cuh).
+//   k_headroom : egs_headroom, per node of a range the binds a stream of pods of one shape would make (read-only).
 //   k_trade_probe / k_trade_leaves / k_trade_commit : the leaf-split Trade of a sidecar handle (c_max > 4) for shapes
 //                whose leaf space is larger than one thread should walk; the kernels above then only read caches.
 // Every kernel here is a template on the geometry: row width G (8, or 16 on a handle with g_max > 8) and, where masks
@@ -364,6 +365,57 @@ __global__ void k_node_reset(uint8_t *all_st, size_t slot_stride, int n_slots, i
   for (int s = 0; s < n_slots; s++) {
     uint8_t *p = all_st + (size_t)s * slot_stride + node0 + i;
     if (full || *p == OPT_UNFIT) *p = OPT_ABSENT;
+  }
+}
+
+// --------------------------------------------------------------------------------------------
+// k_headroom (egs_headroom): nodes [node0, node0 + n) against one shape, one thread per node running headroom_node on
+// a copy of its row and its option entry; nothing is written but the outputs.  Per node count[j] / failed[j]; the four
+// sums of summary (binds, nodes with a bind, failed binds, nodes stopped by the limit) are folded per block and added
+// with one 64-bit atomicAdd per block and value: integer sums, so the result does not depend on the block order.
+// MASKED: a node outside the set is not read and counts 0; with MASKED false the set is never read.
+// --------------------------------------------------------------------------------------------
+#define HEADROOM_THREADS 256
+template <class R>
+struct HeadroomArgsT {
+  const int32_t *core, *mem, *mem_total;
+  int node0, n, policy, limit;
+  R req;
+  OptTable t;
+  int32_t *count, *failed;                  // [n] each, may be null
+  unsigned long long *summary;              // [4]
+};
+// At G = 16 a minimum of one block per SM lifts ptxas's default register cap, as for k_pass.
+template <int G, int NP, bool SINGLE, bool MASKED>
+__global__ void __launch_bounds__(HEADROOM_THREADS, G > EGS_G ? 1 : 0) k_headroom(HeadroomArgsT<ReqOf<NP>> a, NodeSet set) {
+  __shared__ unsigned long long sm[4][HEADROOM_THREADS / 32];
+  const int j = blockIdx.x * HEADROOM_THREADS + threadIdx.x;
+  Headroom r = {0, 0, 0};
+  if (j < a.n) {
+    const int i = a.node0 + j;
+    const uint8_t st = (!MASKED || set.admits(i)) ? a.t.st[i] : (uint8_t)OPT_UNFIT;
+    if (st != OPT_UNFIT) {
+      int c[G], m[G];
+      load_row(a.core, a.mem, (size_t)i, c, m);
+      const PackedT<G, NP> masks = st == OPT_CACHED ? option_masks<G, NP>(a.t, (size_t)i, a.req.C) : 0;
+      r = headroom_node(c, m, SINGLE ? 0 : a.mem_total[i], a.req, SINGLE, a.policy, st, masks, a.limit);
+    }
+    if (a.count) a.count[j] = r.ok;
+    if (a.failed) a.failed[j] = r.failed;
+  }
+  unsigned long long v[4] = {(unsigned long long)r.ok, r.ok > 0 ? 1ull : 0ull, (unsigned long long)r.failed,
+                             (unsigned long long)r.capped};
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    v[k] = warp_sum_u64(v[k]);
+    if (lane == 0) sm[k][w] = v[k];
+  }
+  __syncthreads();
+  if (threadIdx.x < 4) {
+    unsigned long long s = 0;
+    for (int q = 0; q < HEADROOM_THREADS / 32; q++) s += sm[threadIdx.x][q];
+    if (s) atomicAdd(a.summary + threadIdx.x, s);
   }
 }
 

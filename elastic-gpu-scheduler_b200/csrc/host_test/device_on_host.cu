@@ -35,6 +35,19 @@ static int apply_w(int32_t *core, int32_t *mem, int mem_total, int C, const egs_
   return apply_op(core, mem, mem_total, op) ? 1 : 0;
 }
 
+// headroom_node (k_headroom's per-node loop) at geometry (G, NP) = (8, 4), (16, 4) or (8, 8): rows of G cells, the
+// option entry's state (OPT_*) and packed masks, the kernels' Trade dispatch.  out = {ok, failed, capped}.
+template <int G, int NP>
+static void headroom_w(const int32_t *core, const int32_t *mem, int mem_total, int C, const egs_unit *units, int policy,
+                       int state, uint64_t masks, int limit, int32_t *out) {
+  int c[G], m[G];
+  rows(core, mem, c, m);
+  const ReqOf<NP> r = make_req<ReqOf<NP>>(C, units);
+  const bool single = C == 1 && r.cnt[0] == 0 && r.core[0] >= 0 && r.mem[0] >= 0;
+  const Headroom h = headroom_node(c, m, mem_total, r, single, policy, state, (PackedT<G, NP>)masks, limit);
+  out[0] = h.ok; out[1] = h.failed; out[2] = h.capped;
+}
+
 extern "C" {
 // path: 0 = the dispatch the kernels use (fast path when req_is_single), 1 = always the general DFS
 int egsdh_trade(const int32_t *core, const int32_t *mem, int mem_total, int C, const egs_unit *units, int policy,
@@ -163,6 +176,13 @@ void egsdh_leaf_eval_both(const int32_t *core, const int32_t *mem, int mem_total
   *s4 = trade_leaf_eval(c, m, mem_total, r, policy, bits, nbranch, leaf, a);
   *s8 = trade_leaf_eval(c, m, mem_total, rw, policy, bits, nbranch, leaf, b);
   *m4 = *s4 >= 0 ? a : 0; *m8 = *s8 >= 0 ? b : 0;
+}
+// headroom_w at the geometry of a handle: g == 16 a wide handle, planes == 8 a sidecar handle
+void egsdh_headroom(int g, int planes, const int32_t *core, const int32_t *mem, int mem_total, int C,
+                    const egs_unit *units, int policy, int state, uint64_t masks, int limit, int32_t *out) {
+  if (g == 16) headroom_w<16, EGS_C>(core, mem, mem_total, C, units, policy, state, masks, limit, out);
+  else if (planes == EGS_CA) headroom_w<EGS_G, EGS_CA>(core, mem, mem_total, C, units, policy, state, masks, limit, out);
+  else headroom_w<EGS_G, EGS_C>(core, mem, mem_total, C, units, policy, state, masks, limit, out);
 }
 int egsdh_is_single(int C, const egs_unit *units) { const Req r = make_req(C, units); return req_is_single(r) ? 1 : 0; }
 unsigned long long egsdh_cand_key(int32_t score, uint32_t node) { return cand_key(score, node); }

@@ -316,6 +316,51 @@ int egs_schedule_batch_nodes(egs_handle *h, int mode, int n_pods, const int32_t 
                              int32_t *out_node, int32_t *out_status, uint8_t *out_alloc_mask,
                              int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest);
 
+/* ---- capacity: how many more pods of a shape the nodes take ------------------- */
+
+/* Headroom: for each shape s and each node of [node0, node0+n), the number of pods of shape s the node would still
+ * take if only pods of that shape arrived from now on, exactly as the scheduler would place them.
+ *
+ * Definition, and the equality that pins it: under a stream of pods of one shape, a node's Assume (node.go:61-73)
+ * reads only its own rows and its own option entry, and a bind (node.go:87-104) writes only those; the driver rule
+ * keeps binding while any node has an option.  So a dry run -- egs_checkpoint_save, egs_schedule_batch of K >= the
+ * total identical pods, egs_checkpoint_rollback -- makes on every node the same sequence of binds in some order, and
+ * this call counts that sequence node by node without running it:
+ *   1. the shape's cached option on the node, if there is one, is Transacted first, even when stale (a stale option
+ *      can fail its Transact; the Adds it made stay, gpu.go:153-175); a node whose entry says "known not to fit"
+ *      (egs_option_dump state 2) takes nothing; a node without an entry starts at 2;
+ *   2. Trade on the current rows under the handle's policy, Transact, and again, until Trade fails or `limit` binds
+ *      (successful or failed) are made.
+ * Per node, out_count[s*n + i] equals the EGS_OK pods of that dry run on node node0+i and out_failed[s*n + i] its
+ * EGS_ERR_TRANSACT pods (at most 1, from a stale cached option); every pod after them is EGS_ERR_NOFIT.  With `set`
+ * the equality holds against egs_schedule_batch_nodes with that set.
+ * out_summary[s*4 + k]: k = 0 the sum of out_count, 1 the nodes with out_count > 0, 2 the sum of out_failed, 3 the
+ * nodes stopped by `limit` that still had an option.  summary[3] > 0 means the answer is capped and summary[0] a
+ * lower bound (a {0,0} container or a pod of sentinel units alone fits forever).
+ *
+ * Shape s has containers units[c_off[s] .. c_off[s+1]), checked like every request (up to c_max containers).
+ * set: NULL for every node, else one bitmap of EGS_NODE_SET_WORDS(max_nodes) words in the egs_schedule_batch_nodes
+ * layout; a node outside it counts 0 and is not read.  Any output may be NULL, not all three.
+ * Read-only: rows, every option table, the pod maps, the next library-assigned uid and an open checkpoint stay as
+ * they were; an unseen shape is interned as egs_option_dump interns it (its entries read "no entry", the state the
+ * reference starts from).  A batch still in flight is finished first (stream order).
+ * EGS_ERR_BAD_ARG with an egs_last_error text, nothing interned: n_shapes < 1, a shape of 0 or more than c_max
+ * containers, node0 / n outside [0, max_nodes), a set bit at or beyond max_nodes, no output, limit < 1 or
+ * limit > EGS_HEADROOM_MAX_LIMIT; on a sharded handle a range not inside the rank's egs_shard_range (its other rows
+ * are stale after a sharded batch: each rank counts its own range and the host adds the ranks' summaries, no
+ * collective runs); on a sidecar handle a shape the leaf-split kernels Trade (more than 2^12 leaves: not served by
+ * this call).  A malformed unit returns what egs_filter returns for it.
+ *
+ * EGS_HEADROOM_MAX_LIMIT keeps every step of the per-node loop inside the int32 range the guards of egs_state_load
+ * protect (DESIGN.md 1).  Rows start with free core <= 2^20 and free memory <= 2^25 per GPU, and only a sentinel
+ * container raises a row, by 1 per bind: after L binds of a pod of up to 8 containers a GPU holds at most
+ * 2^20 + 8L core and 2^25 + 8L memory, and the Trade of bind L+1 adds up to 8 more.  Binpack's score is
+ * (max_mem + max_core - min_mem - min_core) / 2 / (k+1) * 100 with every row >= 0, so it stays below 2^31 while
+ * (2^25 + 2^20) / 2 + 8(L+1) < 2^31 / 100, that is L + 1 < 521 666; L <= 2^18 leaves a factor of two. */
+#define EGS_HEADROOM_MAX_LIMIT (1 << 18)
+int egs_headroom(egs_handle *h, int n_shapes, const int32_t *c_off, const egs_unit *units, int node0, int n,
+                 const uint64_t *set, int32_t limit, int32_t *out_count, int32_t *out_failed, int64_t *out_summary);
+
 /* ---- node sharding over several GPUs (one handle per device) ----------------- */
 
 /* This handle owns nodes [lo, hi) of the max_nodes id space; rank/world describe the
