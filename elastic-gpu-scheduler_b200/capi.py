@@ -43,7 +43,7 @@ SYMBOLS = [
     "egs_state_snapshot", "egs_state_restore", "egs_checkpoint_save", "egs_checkpoint_rollback", "egs_checkpoint_drop",
     "egs_filter", "egs_score", "egs_bind", "egs_option_peek", "egs_option_dump", "egs_pod_apply", "egs_node_replay_pod", "egs_pod_cancel",
     "egs_mutations_apply", "egs_schedule_batch_mut", "egs_pod_known", "egs_pod_released", "egs_schedule_batch", "egs_schedule_batch_vec", "egs_schedule_batch_device",
-    "egs_schedule_batch_nodes", "egs_headroom",
+    "egs_schedule_batch_nodes", "egs_headroom", "egs_evict_fit",
     "egs_shard_set", "egs_shard_range", "egs_comm_unique_id", "egs_comm_init", "egs_comm_init_local", "egs_profile_evaluate", "egs_profile_get",
     "egs_profile_reset", "egs_get_stream", "egs_rounds_stats", "egs_mix64",
 ]
@@ -107,6 +107,7 @@ def load(build: bool = True):
     L.egs_schedule_batch_device.argtypes = [vp, i32, i32, vp, vp] + [vp] * 6
     L.egs_schedule_batch_nodes.argtypes = [vp, i32, i32, vp, vp, vp, i32, vp, vp] + [vp] * 6
     L.egs_headroom.argtypes = [vp, i32, vp, vp, i32, i32, vp, i32, vp, vp, vp]
+    L.egs_evict_fit.argtypes = [vp, i32, vp, i32, vp, vp, vp, vp, vp, vp]
     L.egs_shard_set.argtypes = [vp, i32, i32]
     L.egs_shard_range.argtypes = [i32, i32, i32, C.POINTER(i32), C.POINTER(i32)]
     L.egs_comm_unique_id.argtypes = [vp]
@@ -402,6 +403,24 @@ class Egs:
         self._ck(self.L.egs_headroom(self.h, S, _p(c_off), _p(units), node0, n, _p(bm), limit, _p(count), _p(failed),
                                      _p(summary)), "egs_headroom")
         return count[:, :n], failed[:, :n], summary[:S]
+
+    # ---- eviction what-if
+    def evict_fit(self, req, node_ids, victims=None):
+        """Whether pod `req` fits on each node of `node_ids` once that node's victims are forgotten (egs_evict_fit).
+        victims: per node a list of (units, alloc, uid) as pod_cancel takes them, None for no victims at all.
+        Returns (status [n] i32, score [n] i32, masks [n, n_masks] of mask_dtype)."""
+        ids = np.ascontiguousarray(node_ids, np.int32)
+        n = len(ids)
+        off = recs = None
+        if victims is not None:
+            off = np.concatenate([[0], np.cumsum([len(v) for v in victims])]).astype(np.int32)
+            recs = mutations_array([(EGS_MUT_FORGET, int(node), u, a, uid)
+                                    for node, vs in zip(ids, victims) for u, a, uid in vs])
+        status = np.zeros(max(n, 1), np.int32); score = np.zeros(max(n, 1), np.int32)
+        masks = np.zeros((max(n, 1), self.n_masks), self.mask_dtype)
+        self._ck(self.L.egs_evict_fit(self.h, len(req), _p(units_array(req)), n, _p(ids), _p(off), _p(recs),
+                                      _p(status), _p(score), _p(masks)), "egs_evict_fit")
+        return status[:n], score[:n], masks[:n]
 
     # ---- sharding / instrumentation
     def shard_set(self, rank: int, world: int):

@@ -827,6 +827,16 @@ extern "C" int egs_pod_cancel(egs_handle *h, int node_id, int n_containers, cons
 // ------------------------------------------------------------------------------- mutation stream
 // caller holds the lock; pending batch bookkeeping already flushed
 template <int G> static int mutations_rows(egs_handle *h, int n, const egs_mutation *ops);
+// A record of a set node (node_id >= 0): its node, units and index lists.
+static int check_record(egs_handle *h, const egs_mutation &m) {
+  TRY(check_node(h, m.node_id));
+  TRY(check_units(m.n_containers, m.units, EGS_MAX_CONTAINERS_APPLY));
+  for (int c = 0; c < m.n_containers; c++) {
+    if (m.n_idx[c] < 0 || m.n_idx[c] > EGS_MAX_GPUS) return fail(h, EGS_ERR_BAD_ARG, "a mutation record holds at most EGS_MAX_GPUS indices per container");
+    for (int j = 0; j < m.n_idx[c]; j++) if (m.idx[c][j] < 0 || m.idx[c][j] >= h->h_gpu_count[m.node_id]) return EGS_ERR_BAD_ARG;
+  }
+  return EGS_OK;
+}
 static int mutations_apply_locked(egs_handle *h, int n, const egs_mutation *ops) {
   if (n < 0 || (n > 0 && !ops)) return EGS_ERR_BAD_ARG;
   if (n == 0) return EGS_OK;
@@ -835,12 +845,7 @@ static int mutations_apply_locked(egs_handle *h, int n, const egs_mutation *ops)
     const egs_mutation &m = ops[i];
     if (m.kind < EGS_MUT_ADD || m.kind > EGS_MUT_REPLAY) return EGS_ERR_BAD_ARG;
     if (m.node_id < 0) { if (m.kind != EGS_MUT_FORGET) return EGS_ERR_BAD_ARG; continue; }
-    TRY(check_node(h, m.node_id));
-    TRY(check_units(m.n_containers, m.units, EGS_MAX_CONTAINERS_APPLY));
-    for (int c = 0; c < m.n_containers; c++) {
-      if (m.n_idx[c] < 0 || m.n_idx[c] > EGS_MAX_GPUS) return fail(h, EGS_ERR_BAD_ARG, "a mutation record holds at most EGS_MAX_GPUS indices per container");
-      for (int j = 0; j < m.n_idx[c]; j++) if (m.idx[c][j] < 0 || m.idx[c][j] >= h->h_gpu_count[m.node_id]) return EGS_ERR_BAD_ARG;
-    }
+    TRY(check_record(h, m));
   }
   return by_geometry(h, [&](auto W) -> int { return mutations_rows<decltype(W)::G>(h, n, ops); });
 }
@@ -854,10 +859,7 @@ static int mutations_rows(egs_handle *h, int n, const egs_mutation *ops) {
   for (int i = 0; i < n; i++) {
     const egs_mutation &m = ops[i];
     TRY(h->book.account(m.kind, m.node_id, m.uid, [&](int cancel) {
-      Op o; memset(&o, 0, sizeof o);
-      o.node = m.node_id; o.cancel = cancel; o.req = make_req<ReqW>(m.n_containers, m.units);
-      for (int c = 0; c < m.n_containers; c++) { o.n_idx[c] = m.n_idx[c]; for (int j = 0; j < m.n_idx[c]; j++) o.idx[c][j] = m.idx[c][j]; }
-      dev.push_back(o);
+      dev.push_back(apply_op_of<G>(m, cancel));
       return EGS_OK;
     }));
   }
@@ -1233,6 +1235,109 @@ extern "C" int egs_headroom(egs_handle *h, int n_shapes, const int32_t *c_off, c
   if (out_count) memcpy(out_count, s_cells, cells * sizeof(int32_t));
   if (out_failed) memcpy(out_failed, s_cells + cells, cells * sizeof(int32_t));
   return EGS_OK;
+}
+
+// ------------------------------------------------------------------------------- eviction what-if
+// Every argument is checked before the shape is interned or anything is staged.  The podsMap decisions are taken on
+// the host, read-only; only the victims that apply reach the device.  One k_evict launch and one synchronisation.
+extern "C" int egs_evict_fit(egs_handle *h, int n_containers, const egs_unit *units, int n, const int32_t *node_ids,
+                             const int32_t *victim_off, const egs_mutation *victims, int32_t *out_status,
+                             int32_t *out_score, uint8_t *out_alloc_mask) {
+  if (!h) return EGS_ERR_BAD_ARG;
+  Guard g(h);
+  if (n < 0 || (n > 0 && (!node_ids || !out_status || !out_score || !out_alloc_mask)))
+    return fail(h, EGS_ERR_BAD_ARG, "egs_evict_fit: n >= 0 candidate nodes, and node_ids and all three outputs");
+  const int urc = check_units(n_containers, units, h->c_max);      // what egs_filter returns for it
+  if (urc != EGS_OK) return fail(h, urc, "egs_evict_fit: malformed pending pod");
+  if (leaf_split(h, n_containers, units))
+    return fail(h, EGS_ERR_BAD_ARG, "egs_evict_fit: shapes Traded by the leaf-split kernels (more than 2^12 leaves) are not served");
+  for (int j = 0; j < n; j++) {
+    const int rc = check_node(h, node_ids[j]);
+    if (rc != EGS_OK) return fail(h, rc, "egs_evict_fit: candidate node out of range or not set");
+    if (h->world > 1 && (node_ids[j] < h->lo || node_ids[j] >= h->hi))
+      return fail(h, EGS_ERR_BAD_ARG, "egs_evict_fit: on a sharded handle every node must lie inside the rank's egs_shard_range");
+  }
+  std::vector<int32_t> sorted(node_ids, node_ids + n);
+  std::sort(sorted.begin(), sorted.end());
+  if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
+    return fail(h, EGS_ERR_BAD_ARG, "egs_evict_fit: a candidate node repeated");
+  if (victim_off) {
+    if (victim_off[0] != 0) return fail(h, EGS_ERR_BAD_ARG, "egs_evict_fit: victim_off[0] != 0");
+    for (int j = 0; j < n; j++)
+      if (victim_off[j + 1] < victim_off[j]) return fail(h, EGS_ERR_BAD_ARG, "egs_evict_fit: victim_off decreases");
+    if (victim_off[n] > 0 && !victims) return fail(h, EGS_ERR_BAD_ARG, "egs_evict_fit: victims missing");
+    for (int j = 0; j < n; j++)
+      for (int k = victim_off[j]; k < victim_off[j + 1]; k++) {
+        const egs_mutation &m = victims[k];
+        if (m.kind != EGS_MUT_FORGET || m.node_id != node_ids[j])
+          return fail(h, EGS_ERR_BAD_ARG, "egs_evict_fit: a victim is an EGS_MUT_FORGET record of its candidate node");
+        const int rc = check_record(h, m);
+        if (rc != EGS_OK) return fail(h, rc, "egs_evict_fit: a victim record egs_mutations_apply refuses");
+      }
+  }
+  int slot;
+  TRY(intern(h, n_containers, units, &slot));
+  if (n == 0) return EGS_OK;
+  TRY(settle_pending(h, true));                   // the podsMap decisions need every batch's binds in the book
+  const size_t sn = (size_t)n, ab = (size_t)h->planes * h->mask_b;   // alloc bytes per node
+  if (sn > h->d_ids.cap()) {
+    const size_t cap = std::max(sn, (size_t)4096);
+    CK(h, grow(h->stream, false, to(h->d_ids, cap), to(h->d_fit, cap), to(h->d_score, cap)));
+  }
+  TRY(ensure_out(h, n));
+  return by_geometry(h, [&](auto W) -> int {
+    constexpr int G = decltype(W)::G, NP = decltype(W)::NP;
+    typedef ApplyOp<G> Op;
+    // the victims that apply: in the node's podsMap and not forgotten by an earlier victim of the same list
+    std::vector<Op> ops;
+    std::vector<int32_t> off(sn + 1, 0);
+    std::vector<uint64_t> gone;
+    for (int j = 0; j < n; j++) {
+      off[j] = (int32_t)ops.size();
+      gone.clear();
+      for (int k = victim_off ? victim_off[j] : 0; victim_off && k < victim_off[j + 1]; k++) {
+        const egs_mutation &m = victims[k];
+        if (!h->book.in_pods_map(m.node_id, m.uid) || std::find(gone.begin(), gone.end(), m.uid) != gone.end()) continue;
+        gone.push_back(m.uid);
+        ops.push_back(apply_op_of<G>(m, 1));
+      }
+    }
+    off[sn] = (int32_t)ops.size();
+    const size_t nd = ops.size();
+    if (nd * sizeof(Op) > h->d_ops.cap() || sn + 1 > h->d_group_off.cap()) {
+      const size_t cap = std::max({nd, sn, (size_t)1024, h->d_ops.cap() / sizeof(Op)});
+      CK(h, grow(h->stream, false, to(h->d_ops, cap * sizeof(Op)), to(h->d_group_off, cap + 1)));
+    }
+    TRY(ensure_stage(h, std::max(nd * sizeof(Op) + (2 * sn + 1) * sizeof(int32_t), sn * (8 + ab))));
+    CK(h, cudaStreamSynchronize(h->stream));     // staging buffer reuse
+    Op *so = (Op *)h->h_stage.get();
+    int32_t *sid = (int32_t *)(so + nd), *soff = sid + sn;
+    std::copy(ops.begin(), ops.end(), so);
+    memcpy(sid, node_ids, sn * sizeof(int32_t));
+    memcpy(soff, off.data(), (sn + 1) * sizeof(int32_t));
+    if (nd) CK(h, cudaMemcpyAsync(h->d_ops, so, nd * sizeof(Op), cudaMemcpyHostToDevice, h->stream));
+    CK(h, cudaMemcpyAsync(h->d_ids, sid, sn * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+    CK(h, cudaMemcpyAsync(h->d_group_off, soff, (sn + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+    EvictArgsT<G, ReqOf<NP>> a;
+    a.core = h->d_core; a.mem = h->d_mem; a.mem_total = h->d_mem_total;
+    a.n = n; a.policy = h->policy; a.req = make_req<ReqOf<NP>>(n_containers, units); a.t = table(h, slot);
+    a.ids = h->d_ids; a.off = h->d_group_off; a.ops = (const Op *)h->d_ops.get();
+    a.status = h->d_o_status; a.score = h->d_score; a.alloc = h->d_o_alloc;
+    const int grid = (n + EVICT_THREADS - 1) / EVICT_THREADS;
+    if (is_single(n_containers, units)) k_evict<G, NP, true><<<grid, EVICT_THREADS, 0, h->stream>>>(a);
+    else k_evict<G, NP, false><<<grid, EVICT_THREADS, 0, h->stream>>>(a);
+    CK(h, cudaGetLastError());
+    // back through the staging buffer, after the copies out of it in stream order
+    char *s = h->h_stage.get();
+    CK(h, cudaMemcpyAsync(s, h->d_o_status, sn * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaMemcpyAsync(s + 4 * sn, h->d_score, sn * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaMemcpyAsync(s + 8 * sn, h->d_o_alloc, sn * ab, cudaMemcpyDeviceToHost, h->stream));
+    CK(h, cudaStreamSynchronize(h->stream));
+    memcpy(out_status, s, sn * sizeof(int32_t));
+    memcpy(out_score, s + 4 * sn, sn * sizeof(int32_t));
+    memcpy(out_alloc_mask, s + 8 * sn, sn * ab);
+    return EGS_OK;
+  });
 }
 
 // ------------------------------------------------------------------------------- sharding

@@ -483,6 +483,19 @@ EGS_HD Headroom headroom_node(const int (&c0)[G], const int (&m0)[G], int mem_to
 template <int G>
 struct ApplyOp { int node, cancel; ReqW req; int n_idx[EGS_CA]; int8_t idx[EGS_CA][G]; };
 
+// The row update of a mutation record (egs_mutation, already validated) in the device's form: cancel 1 is ForgetPod's
+// Cancel, 0 AddPod's Transact.  Host code: the mutation stream and the eviction what-if build their ops with it.
+template <int G>
+inline ApplyOp<G> apply_op_of(const egs_mutation &m, int cancel) {
+  ApplyOp<G> o = {};
+  o.node = m.node_id; o.cancel = cancel; o.req = make_req<ReqW>(m.n_containers, m.units);
+  for (int c = 0; c < m.n_containers; c++) {
+    o.n_idx[c] = m.n_idx[c];
+    for (int j = 0; j < m.n_idx[c]; j++) o.idx[c][j] = m.idx[c][j];
+  }
+  return o;
+}
+
 // The update on the node's rows (one thread): Cancel (gpu.go:177-191, GPU.Sub gpu.go:41-49: a whole-GPU container
 // puts its GPUs back at their totals) or Transact (gpu.go:153-175, CanAllocate + Add: the first failure stops the op,
 // no rollback).  Returns false when a Transact stopped.
@@ -505,4 +518,32 @@ EGS_HD bool apply_op(int32_t *c, int32_t *m, int mt, const ApplyOp<G> &op) {
     }
   }
   return true;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Eviction what-if of one node (egs_evict_fit): would a pending pod fit on the node once its victims are gone?
+// ForgetPod (node.go:129-140) changes only the node's rows and podsMap, not its option entries, and Assume / Score /
+// Allocate (node.go:61-104) read only those rows and the node's entry for the shape, so the answer is the node's own:
+//   1. the GPUs.Cancel of every victim that applies (the host's podsMap decisions: ops[0 .. n_ops)), on a copy of
+//      the row;
+//   2. the option: the cached one, stale or not (ForgetPod keeps it and Assume returns it, node.go:64-66); none when
+//      the entry says "known not to fit" and no victim applied (the rows are those that memo was taken on); else
+//      Trade on the freed row;
+//   3. the bind: Transact of the option's masks on the freed row (gpu.go:153-175).
+// On entry score / masks hold the cached option when state is OPT_CACHED.  Returns EGS_ERR_NOFIT (score and masks 0),
+// EGS_OK, or EGS_ERR_TRANSACT (masks 0, score the option's).
+// ---------------------------------------------------------------------------------------------
+template <int G, class R>
+EGS_HD int evict_node(const int (&c0)[G], const int (&m0)[G], int mem_total, const R &r, bool single, int policy,
+                      int state, const ApplyOp<G> *ops, int n_ops, int &score, PackedT<G, R::NC> &masks) {
+  int c[G], m[G];
+#pragma unroll
+  for (int g = 0; g < G; g++) { c[g] = c0[g]; m[g] = m0[g]; }
+  for (int o = 0; o < n_ops; o++) apply_op<G>(c, m, mem_total, ops[o]);
+  const bool have = state == OPT_CACHED ||
+                    ((state != OPT_UNFIT || n_ops > 0) && trade_any(c, m, mem_total, r, single, policy, score, masks));
+  if (!have) { score = 0; masks = 0; return EGS_ERR_NOFIT; }
+  if (transact_row<G>(c, m, mem_total, r, masks)) return EGS_OK;
+  masks = 0;
+  return EGS_ERR_TRANSACT;
 }

@@ -12,6 +12,8 @@
 // Each reference step these kernels share is written once: Assume (assume_option), Allocate
 // (allocate_option), and the AddPod / ForgetPod row update (apply_op, egs_device.cuh).
 //   k_headroom : egs_headroom, per node of a range the binds a stream of pods of one shape would make (read-only).
+//   k_evict    : egs_evict_fit, per candidate node whether a pending pod fits once the node's victims are gone
+//                (read-only).
 //   k_trade_probe / k_trade_leaves / k_trade_commit : the leaf-split Trade of a sidecar handle (c_max > 4) for shapes
 //                whose leaf space is larger than one thread should walk; the kernels above then only read caches.
 // Every kernel here is a template on the geometry: row width G (8, or 16 on a handle with g_max > 8) and, where masks
@@ -417,6 +419,42 @@ __global__ void __launch_bounds__(HEADROOM_THREADS, G > EGS_G ? 1 : 0) k_headroo
     for (int q = 0; q < HEADROOM_THREADS / 32; q++) s += sm[threadIdx.x][q];
     if (s) atomicAdd(a.summary + threadIdx.x, s);
   }
+}
+
+// --------------------------------------------------------------------------------------------
+// k_evict (egs_evict_fit): one thread per candidate node ids[j], running evict_node on a copy of its row and its option
+// entry with the victims that apply there, ops[off[j] .. off[j+1]) (the host took the podsMap decisions).  Nothing is
+// written but the outputs: status[j], score[j] and the packed masks alloc[j].
+// --------------------------------------------------------------------------------------------
+#define EVICT_THREADS 256
+template <int G, class R>
+struct EvictArgsT {
+  const int32_t *core, *mem, *mem_total;
+  int n, policy;
+  R req;
+  OptTable t;
+  const int32_t *ids, *off;                 // [n] candidate nodes, [n + 1] offsets into ops
+  const ApplyOp<G> *ops;                    // cancel == 1 each
+  int32_t *status, *score;                  // [n]
+  uint8_t *alloc;                           // [n] packed words of NP MaskT<G>
+};
+// At G = 16 a minimum of one block per SM lifts ptxas's default register cap, as for k_pass.
+template <int G, int NP, bool SINGLE>
+__global__ void __launch_bounds__(EVICT_THREADS, G > EGS_G ? 1 : 0) k_evict(EvictArgsT<G, ReqOf<NP>> a) {
+  const int j = blockIdx.x * EVICT_THREADS + threadIdx.x;
+  if (j >= a.n) return;
+  const size_t i = (size_t)a.ids[j];
+  const uint8_t st = a.t.st[i];
+  int c[G], m[G];
+  load_row(a.core, a.mem, i, c, m);
+  int score = st == OPT_CACHED ? a.t.sc[i] : 0;
+  PackedT<G, NP> masks = st == OPT_CACHED ? option_masks<G, NP>(a.t, i, a.req.C) : 0;
+  const int o0 = a.off[j];
+  const int status = evict_node(c, m, a.mem_total[i], a.req, SINGLE, a.policy, st, a.ops + o0, a.off[j + 1] - o0, score,
+                                masks);
+  a.status[j] = status;
+  a.score[j] = score;
+  reinterpret_cast<PackedT<G, NP> *>(a.alloc)[j] = masks;
 }
 
 // --------------------------------------------------------------------------------------------

@@ -48,6 +48,23 @@ static void headroom_w(const int32_t *core, const int32_t *mem, int mem_total, i
   out[0] = h.ok; out[1] = h.failed; out[2] = h.capped;
 }
 
+// evict_node (k_evict's per-node answer) at geometry (G, NP): rows of G cells, the option entry's state, score and
+// packed masks, and the victims that apply as egs_mutation records (converted as egs_evict_fit converts them).
+// out = {status, score}; *masks the masks of a successful bind.
+template <int G, int NP>
+static void evict_w(const int32_t *core, const int32_t *mem, int mem_total, int C, const egs_unit *units, int policy,
+                    int state, int score, uint64_t *masks, int n_victims, const egs_mutation *victims, int32_t *out) {
+  int c[G], m[G];
+  rows(core, mem, c, m);
+  const ReqOf<NP> r = make_req<ReqOf<NP>>(C, units);
+  const bool single = C == 1 && r.cnt[0] == 0 && r.core[0] >= 0 && r.mem[0] >= 0;
+  std::vector<ApplyOp<G>> ops;
+  for (int k = 0; k < n_victims; k++) ops.push_back(apply_op_of<G>(victims[k], 1));
+  PackedT<G, NP> mk = (PackedT<G, NP>)*masks;
+  out[0] = evict_node(c, m, mem_total, r, single, policy, state, ops.data(), n_victims, score, mk);
+  out[1] = score; *masks = mk;
+}
+
 extern "C" {
 // path: 0 = the dispatch the kernels use (fast path when req_is_single), 1 = always the general DFS
 int egsdh_trade(const int32_t *core, const int32_t *mem, int mem_total, int C, const egs_unit *units, int policy,
@@ -183,6 +200,14 @@ void egsdh_headroom(int g, int planes, const int32_t *core, const int32_t *mem, 
   if (g == 16) headroom_w<16, EGS_C>(core, mem, mem_total, C, units, policy, state, masks, limit, out);
   else if (planes == EGS_CA) headroom_w<EGS_G, EGS_CA>(core, mem, mem_total, C, units, policy, state, masks, limit, out);
   else headroom_w<EGS_G, EGS_C>(core, mem, mem_total, C, units, policy, state, masks, limit, out);
+}
+// evict_w at the geometry of a handle: g == 16 a wide handle, planes == 8 a sidecar handle
+void egsdh_evict(int g, int planes, const int32_t *core, const int32_t *mem, int mem_total, int C, const egs_unit *units,
+                 int policy, int state, int score, uint64_t *masks, int n_victims, const egs_mutation *victims,
+                 int32_t *out) {
+  if (g == 16) evict_w<16, EGS_C>(core, mem, mem_total, C, units, policy, state, score, masks, n_victims, victims, out);
+  else if (planes == EGS_CA) evict_w<EGS_G, EGS_CA>(core, mem, mem_total, C, units, policy, state, score, masks, n_victims, victims, out);
+  else evict_w<EGS_G, EGS_C>(core, mem, mem_total, C, units, policy, state, score, masks, n_victims, victims, out);
 }
 int egsdh_is_single(int C, const egs_unit *units) { const Req r = make_req(C, units); return req_is_single(r) ? 1 : 0; }
 unsigned long long egsdh_cand_key(int32_t score, uint32_t node) { return cand_key(score, node); }

@@ -361,6 +361,54 @@ int egs_schedule_batch_nodes(egs_handle *h, int mode, int n_pods, const int32_t 
 int egs_headroom(egs_handle *h, int n_shapes, const int32_t *c_off, const egs_unit *units, int node0, int n,
                  const uint64_t *set, int32_t limit, int32_t *out_count, int32_t *out_failed, int64_t *out_summary);
 
+/* ---- eviction what-if: would a pending pod fit once a node's victims are gone ---- */
+
+/* Eviction what-if: for each candidate node, whether the pending pod units[0 .. n_containers) would fit on it, and
+ * bind with which masks, if the victims listed for that node were forgotten first -- kube-scheduler's preemption
+ * question, asked of every candidate at once, with nothing changed.  Candidate node_ids[i] has the victims
+ * victims[victim_off[i] .. victim_off[i+1]): EGS_MUT_FORGET records of that node, each with the units, index lists
+ * and uid egs_pod_cancel would take (NewGPUOptionFromPod, allocate.go:75-93).  victim_off == NULL: no victims.
+ *
+ * Definition.  ForgetPod on node n (node.go:129-140) changes only n's rows and podsMap, not its option entries, and
+ * Assume / Score / Allocate on n (node.go:61-104) read only n's rows and n's entry for the shape, so each node is
+ * answered on its own, on a copy of its row:
+ *   1. the GPUs.Cancel of every victim, in list order, that applies: its uid is in the node's podsMap and no earlier
+ *      victim of the same list forgot it (the decision egs_pod_cancel takes, node.go:131);
+ *   2. the option: the node's cached option of the shape, even when stale (ForgetPod keeps it, Assume returns it,
+ *      node.go:64-66); none when the entry says "known not to fit" (egs_option_dump state 2) and no victim applied;
+ *      else Trade on the freed row under the handle's policy;
+ *   3. out_status[i]: EGS_ERR_NOFIT without an option, else the Transact of the option's masks on the freed row:
+ *      EGS_OK, or EGS_ERR_TRANSACT when a stale cached option no longer fits (gpu.go:153-175);
+ *      out_score[i]: the option's score (what egs_score returns), 0 for EGS_ERR_NOFIT;
+ *      out_alloc_mask, element (i, c) at byte (i*EGS_MASKS_PER_POD(c_max) + c) * EGS_MASK_BYTES(g_max): the option's
+ *      masks when out_status[i] is EGS_OK, else zeros (what egs_bind returns).
+ * Per-node outputs follow the order of node_ids.
+ *
+ * Equality A, per node: egs_checkpoint_save; egs_pod_cancel of each victim of node_ids[i] in order;
+ * egs_filter({node_ids[i]}), egs_score({node_ids[i]}) and, when it fits, egs_bind(node_ids[i], an unknown uid);
+ * egs_checkpoint_rollback.  Filter says "no fit" exactly when out_status[i] is EGS_ERR_NOFIT; the score equals
+ * out_score[i]; the bind's status and masks equal out_status[i] and the masks.
+ * Equality B, all nodes at once: egs_checkpoint_save; egs_mutations_apply of every victim record of every candidate;
+ * egs_schedule_batch_nodes of the one pending pod with the set of the candidate nodes; rollback.  With "fit" meaning
+ * out_status != EGS_ERR_NOFIT, the batch's node is the lowest id among the fit nodes of maximal out_score (-1 when
+ * none fits), its status and masks are that node's, its fit count is the number of fit nodes, and its digests are the
+ * sums of the fit and score terms over the fit nodes -- whatever the order of node_ids.
+ *
+ * Read-only: rows, option tables, the pod maps, the next library-assigned uid and an open checkpoint stay as they
+ * were; an unseen shape is interned as egs_option_dump interns it.  A batch still in flight is settled first.
+ * Refused before anything is interned, with an egs_last_error text: n < 0, or n > 0 without node_ids or one of the
+ * outputs (EGS_ERR_BAD_ARG); a node id check_node refuses (EGS_ERR_BAD_ARG out of range, EGS_ERR_NO_NODE not set);
+ * a node id repeated (EGS_ERR_BAD_ARG); victim_off[0] != 0 or decreasing, or victims NULL with victim_off[n] > 0
+ * (EGS_ERR_BAD_ARG); a victim of another kind or another node (EGS_ERR_BAD_ARG), or one egs_mutations_apply refuses
+ * (its code: units, n_idx <= EGS_MAX_GPUS, indices below the node's GPU count); on a sidecar handle a pending shape the
+ * leaf-split kernels Trade (EGS_ERR_BAD_ARG, as egs_headroom); on a sharded handle a node outside the rank's
+ * egs_shard_range (EGS_ERR_BAD_ARG: an owner-only verb, like egs_filter).  A malformed pending unit returns what
+ * egs_filter returns for it.  On a wide handle a whole-GPU victim of more than EGS_MAX_GPUS GPUs does not fit in a
+ * record (as for egs_mutations_apply); the checkpoint recipe of equality A covers it. */
+int egs_evict_fit(egs_handle *h, int n_containers, const egs_unit *units,
+                  int n, const int32_t *node_ids, const int32_t *victim_off, const egs_mutation *victims,
+                  int32_t *out_status, int32_t *out_score, uint8_t *out_alloc_mask);
+
 /* ---- node sharding over several GPUs (one handle per device) ----------------- */
 
 /* This handle owns nodes [lo, hi) of the max_nodes id space; rank/world describe the
