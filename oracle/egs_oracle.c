@@ -564,6 +564,21 @@ int egso_peek(egso *o, int node, int C, const egso_unit *units, int64_t *score, 
   opt_export(hit, C, alloc_off, alloc_idx);
   return 1;
 }
+void egso_peek_many(egso *o, int n, const int32_t *node_ids, int C, const egso_unit *units, int planes,
+                    uint8_t *present, int64_t *score, uint16_t *masks) {
+  const uint32_t key = node_key(o, intern(o, C, units), C, units);
+  for (int i = 0; i < n; i++) {
+    const opt_t *hit = cache_find(&o->nodes[node_ids[i]], key);
+    present[i] = hit != NULL;
+    if (!hit) continue;
+    score[i] = hit->score;
+    for (int c = 0; c < C && c < planes; c++) {
+      uint16_t m = 0;
+      for (int j = 0; j < hit->n[c]; j++) m |= (uint16_t)(1u << hit->idx[c][j]);
+      masks[(size_t)i * planes + c] = m;
+    }
+  }
+}
 /* TEST SUPPORT: install cached options of one request shape on nodes [0, n) (node_ids NULL) -- the state of a
  * scheduler that already ran: entry i exists when valid[i] != 0, with option.Score = score[i] and
  * option.Allocated rebuilt from alloc_mask[i][c] (bit g = GPU g of container c; Trade only yields
@@ -620,6 +635,17 @@ int egso_forget_pod(egso *o, int node, int C, const egso_unit *units, const int3
 int egso_known_pod(egso *o, uint64_t uid) { return set_has(&o->pod_maps, uid); }
 int egso_released_pod(egso *o, uint64_t uid) { return set_has(&o->released, uid); }
 
+/* the per-node terms of a pod's fit digest and score digest (sums mod 2^64 over its fit nodes) */
+static inline uint64_t fit_term(int32_t node) { return egso_mix64(2ull * (uint64_t)node + 1); }
+static inline uint64_t score_term(int32_t node, int64_t score) {
+  return egso_mix64(2ull * (uint64_t)node + 2) * (2ull * (uint64_t)(uint32_t)(int32_t)score + 1);
+}
+/* the mask plane of each of the first 4 containers of a bound option (GPUs beyond 8 are not representable) */
+static void alloc_mask_of(int C, const int32_t *off, const int32_t *idx, uint8_t mask[4]) {
+  for (int c = 0; c < C && c < 4; c++)
+    for (int k = off[c]; k < off[c + 1]; k++) if (idx[k] < 8) mask[c] |= (uint8_t)(1u << idx[k]);
+}
+
 int egso_schedule_batch(egso *o, int P, const int32_t *c_off, const egso_unit *units, const uint64_t *uids,
                         int threads, int32_t *out_node, int32_t *out_status, uint8_t *out_alloc_mask,
                         int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest,
@@ -638,8 +664,8 @@ int egso_schedule_batch(egso *o, int P, const int32_t *c_off, const egso_unit *u
     uint64_t fd = 0, sd = 0;
     int w = -1; int64_t best = 0;
     for (int j = 0; j < nf; j++) {
-      fd += egso_mix64(2ull * (uint64_t)ids[j] + 1);
-      sd += egso_mix64(2ull * (uint64_t)ids[j] + 2) * (2ull * (uint64_t)(uint32_t)(int32_t)sc[j] + 1);
+      fd += fit_term(ids[j]);
+      sd += score_term(ids[j], sc[j]);
       if (w < 0 || sc[j] > best) { w = ids[j]; best = sc[j]; }   /* first max */
     }
     if (p < vec_pods) {
@@ -655,9 +681,7 @@ int egso_schedule_batch(egso *o, int P, const int32_t *c_off, const egso_unit *u
     if (w >= 0) {
       int32_t off[EGSO_MAX_C + 1], idx[EGSO_MAX_C * EGSO_MAX_G];
       st = egso_bind(o, w, C, u, uids ? uids[p] : (uint64_t)p, off, idx); /* /scheduler/bind */
-      if (st == ST_OK)
-        for (int c = 0; c < C && c < 4; c++)
-          for (int k = off[c]; k < off[c + 1]; k++) if (idx[k] < 8) mask[c] |= (uint8_t)(1u << idx[k]);
+      if (st == ST_OK) alloc_mask_of(C, off, idx, mask);
     }
     if (out_node) out_node[p] = w;
     if (out_status) out_status[p] = st;
@@ -668,4 +692,130 @@ int egso_schedule_batch(egso *o, int P, const int32_t *c_off, const egso_unit *u
   }
   free(fit); free(ids); free(sc);
   return P;
+}
+
+/* ---------------------------------------------------------------- indexed driver
+ *
+ * egso_schedule_batch Assumes every node for every pod.  Within one call nearly all of those Assumes repeat an
+ * earlier answer, because an Assume of shape s on node n (node_assume) reads only two things:
+ *   - n's cache entry for s's key: a hit returns it untouched (node.go:64-66), stale or not;
+ *   - on a miss, n's rows, which Trade reads (and on success the entry is cached).
+ * During a batch the only event that changes either is a bind (egso_bind): it deletes the bound shape's entry at the
+ * bound node (node.go:90-92) and changes that node's rows (Transact, also when it fails part way: gpu.go:153-175
+ * keeps the earlier Adds).  No other node and no other key changes.  So, for shape s:
+ *   - a node that holds an entry for s keeps it, with the same score, until s itself is bound there;
+ *   - a node without one answers "no fit" again until its rows change, i.e. until it is bound (to any shape).
+ * The driver logs every bound node.  Before a pod of s it Assumes only the nodes logged since s's last pod that hold
+ * no entry for s, so every node then holds exactly the entry the plain driver's Filter would leave, and the nodes
+ * with an entry are exactly the plain driver's fit set.  Per shape it keeps that set in a max segment tree over node
+ * ids, ordered by (score, lower id) -- the plain driver's first max in node order -- and its fit count and digests as
+ * running sums of the same terms.  The first pod of s in a call Assumes every node, so any state the object was left
+ * in between calls (add_pod / forget_pod, cache_load, node_reset, earlier batches) is read afresh.
+ *
+ * Faithful mode keys entries by the 8-hex sha256 prefix: two shapes of one batch with the same prefix share an entry,
+ * so a bind of one would change the other's set, which this driver does not track; it refuses such a batch. */
+typedef struct {
+  uint32_t shape;
+  int C;
+  const egso_unit *u;
+  int64_t cursor;     /* log length at this shape's last pod; -1 before its first pod of the call */
+  int32_t *tree;      /* [2L]: leaf L + n = n when node n holds an entry, else -1; inner = the better child */
+  int64_t *score;     /* [N]: the score of each node's entry */
+  int32_t fit_count;
+  uint64_t fd, sd;
+} ix_shape;
+
+static inline int32_t ix_pick(const ix_shape *s, int32_t lo, int32_t hi) { /* lo's ids are below hi's */
+  if (lo < 0) return hi;
+  if (hi < 0) return lo;
+  return s->score[hi] > s->score[lo] ? hi : lo;
+}
+static void ix_set(ix_shape *s, int L, int32_t node, int32_t leaf) {
+  size_t i = (size_t)L + (size_t)node;
+  s->tree[i] = leaf;
+  for (i >>= 1; i; i >>= 1) s->tree[i] = ix_pick(s, s->tree[2 * i], s->tree[2 * i + 1]);
+}
+static void ix_insert(ix_shape *s, int L, int32_t node, int64_t score) {
+  s->score[node] = score;
+  s->fit_count++; s->fd += fit_term(node); s->sd += score_term(node, score);
+  ix_set(s, L, node, node);
+}
+static void ix_remove(ix_shape *s, int L, int32_t node) {
+  s->fit_count--; s->fd -= fit_term(node); s->sd -= score_term(node, s->score[node]);
+  ix_set(s, L, node, -1);
+}
+
+int egso_schedule_batch_indexed(egso *o, int P, const int32_t *c_off, const egso_unit *units, const uint64_t *uids,
+                                int threads, int32_t *out_node, int32_t *out_status, uint8_t *out_alloc_mask,
+                                int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest) {
+  const int N = o->nn;
+  int L = 1;
+  while (L < N) L *= 2;
+  int32_t *pod_shape = malloc(sizeof(int32_t) * (size_t)(P > 0 ? P : 1));
+  for (int p = 0; p < P; p++) pod_shape[p] = (int32_t)intern(o, c_off[p + 1] - c_off[p], units + c_off[p]);
+  int32_t *local = malloc(sizeof(int32_t) * (size_t)(o->ns > 0 ? o->ns : 1));
+  for (int i = 0; i < o->ns; i++) local[i] = -1;
+  ix_shape *sh = calloc((size_t)(o->ns > 0 ? o->ns : 1), sizeof *sh);
+  int ns = 0;
+  for (int p = 0; p < P; p++) {
+    int32_t g = pod_shape[p];
+    if (local[g] < 0) {
+      ix_shape *s = &sh[ns];
+      s->shape = (uint32_t)g; s->C = c_off[p + 1] - c_off[p]; s->u = units + c_off[p]; s->cursor = -1;
+      local[g] = ns++;
+    }
+    pod_shape[p] = local[g];
+  }
+  int rc = P;
+  if (o->faithful)
+    for (int a = 0; a < ns && rc == P; a++)
+      for (int b = a + 1; b < ns; b++)
+        if (node_key(o, sh[a].shape, sh[a].C, sh[a].u) == node_key(o, sh[b].shape, sh[b].C, sh[b].u)) { rc = -1; break; }
+  int32_t *log = malloc(sizeof(int32_t) * (size_t)(P > 0 ? P : 1));
+  int64_t nlog = 0;
+  int32_t *seen = malloc(sizeof(int32_t) * (size_t)(N > 0 ? N : 1)); /* the last pod that caught a node up */
+  uint8_t *fit = malloc((size_t)(N > 0 ? N : 1));
+  for (int i = 0; i < N; i++) seen[i] = -1;
+  for (int p = 0; p < P && rc == P; p++) {
+    ix_shape *s = &sh[pod_shape[p]];
+    const int C = s->C;
+    const egso_unit *u = units + c_off[p];
+    if (s->cursor < 0) {                                          /* first pod of s: every node */
+      s->tree = malloc(sizeof(int32_t) * 2 * (size_t)L);
+      s->score = calloc((size_t)(N > 0 ? N : 1), sizeof(int64_t));
+      for (size_t i = 0; i < 2 * (size_t)L; i++) s->tree[i] = -1;
+      egso_filter(o, N, NULL, C, u, threads, fit);
+      const uint32_t key = node_key(o, s->shape, C, u);
+      for (int n = 0; n < N; n++)
+        if (fit[n]) ix_insert(s, L, n, cache_find(&o->nodes[n], key)->score);
+    } else {                                                      /* nodes bound since s's last pod */
+      for (int64_t k = s->cursor; k < nlog; k++) {
+        const int32_t n = log[k];
+        if (seen[n] == p || s->tree[(size_t)L + n] >= 0) continue; /* logged twice, or holds an entry */
+        seen[n] = p;
+        const opt_t *op = node_assume(o, &o->nodes[n], s->shape, C, u);
+        if (op) ix_insert(s, L, n, op->score);
+      }
+    }
+    s->cursor = nlog;
+    const int32_t w = s->tree[1];
+    int st = ST_NOFIT;
+    uint8_t mask[4] = {0, 0, 0, 0};
+    if (out_fit_count) out_fit_count[p] = s->fit_count;
+    if (out_fit_digest) out_fit_digest[p] = s->fd;
+    if (out_score_digest) out_score_digest[p] = s->sd;
+    if (w >= 0) {
+      int32_t off[EGSO_MAX_C + 1], idx[EGSO_MAX_C * EGSO_MAX_G];
+      st = egso_bind(o, w, C, u, uids ? uids[p] : (uint64_t)p, off, idx);
+      if (st == ST_OK) alloc_mask_of(C, off, idx, mask);
+      ix_remove(s, L, w);                                         /* egso_bind deleted w's entry whatever st is */
+      log[nlog++] = w;
+    }
+    if (out_node) out_node[p] = w;
+    if (out_status) out_status[p] = st;
+    if (out_alloc_mask) memcpy(out_alloc_mask + 4 * (size_t)p, mask, 4);
+  }
+  for (int i = 0; i < ns; i++) { free(sh[i].tree); free(sh[i].score); }
+  free(sh); free(local); free(pod_shape); free(log); free(seen); free(fit);
+  return rc;
 }

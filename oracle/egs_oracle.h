@@ -66,6 +66,10 @@ int egso_bind(egso *o, int node, int C, const egso_unit *units, uint64_t uid,
               int32_t *alloc_off, int32_t *alloc_idx);
 int egso_peek(egso *o, int node, int C, const egso_unit *units, int64_t *score,
               int32_t *alloc_off, int32_t *alloc_idx);   /* 1 = cached */
+/* egso_peek on node_ids[0..n): present[i], score[i] and masks[i][planes] (one GPU bitmask per container, up to 16
+ * GPUs; planes past C untouched), written only where present. */
+void egso_peek_many(egso *o, int n, const int32_t *node_ids, int C, const egso_unit *units, int planes,
+                    uint8_t *present, int64_t *score, uint16_t *masks);
 int egso_add_pod(egso *o, int node, int C, const egso_unit *units,
                  const int32_t *alloc_off, const int32_t *alloc_idx, uint64_t uid);
 int egso_forget_pod(egso *o, int node, int C, const egso_unit *units,
@@ -85,6 +89,15 @@ int egso_schedule_batch(egso *o, int P, const int32_t *c_off, const egso_unit *u
                         int32_t *out_node, int32_t *out_status, uint8_t *out_alloc_mask,
                         int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest,
                         int vec_pods, uint8_t *vec_fit, int32_t *vec_score);
+
+/* The same decisions and the same six per-pod outputs as egso_schedule_batch (no vec_*), from any state of `o`, in
+ * about O(P * (S + log N)) work for S shapes: each pod Assumes only the nodes bound since its shape's last pod, and the
+ * fit set of each shape is kept indexed (see egs_oracle.c).  threads only parallelises each shape's first sweep over
+ * every node.  Returns P, or -1 (nothing done) in faithful mode when two shapes of the batch share a cache key. */
+int egso_schedule_batch_indexed(egso *o, int P, const int32_t *c_off, const egso_unit *units,
+                                const uint64_t *uids, int threads,
+                                int32_t *out_node, int32_t *out_status, uint8_t *out_alloc_mask,
+                                int32_t *out_fit_count, uint64_t *out_fit_digest, uint64_t *out_score_digest);
 
 uint64_t egso_mix64(uint64_t x);
 void egso_sha256(const uint8_t *msg, uint64_t len, uint8_t out[32]);

@@ -27,6 +27,24 @@ def build(force: bool = False) -> str:
     return _SO
 
 
+FIELDS = ("node", "status", "alloc_mask", "fit_count", "fit_digest", "score_digest")
+
+
+def first_difference(ref: dict, got: dict, fields: Sequence[str] = FIELDS) -> Optional[Tuple[int, str]]:
+    """(pod, field) of the first pod at which two batches' per-pod outputs differ, the field first in `fields` order
+    at that pod; None when they are equal.  Arrays of different lengths differ at the shorter length."""
+    first = None
+    for f in fields:
+        a, b = np.asarray(ref[f]), np.asarray(got[f])
+        n = min(len(a), len(b))
+        ne = a[:n] != b[:n]
+        bad = np.flatnonzero(ne.any(axis=tuple(range(1, ne.ndim))) if ne.ndim > 1 else ne)
+        p = int(bad[0]) if bad.size else (n if len(a) != len(b) else None)
+        if p is not None and (first is None or p < first[0]):
+            first = (p, f)
+    return first
+
+
 class Unit(C.Structure):
     _fields_ = [("core", C.c_int64), ("mem", C.c_int64), ("count", C.c_int64)]
 
@@ -57,6 +75,7 @@ def lib():
         L.egso_score.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         L.egso_bind.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
         L.egso_peek.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.egso_peek_many.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 3
         L.egso_add_pod.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
         L.egso_forget_pod.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
         L.egso_cache_load.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -64,6 +83,8 @@ def lib():
         L.egso_released_pod.argtypes = [C.c_void_p, C.c_uint64]
         L.egso_schedule_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + \
             [C.c_void_p] * 6 + [C.c_int, C.c_void_p, C.c_void_p]
+        L.egso_schedule_batch_indexed.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + \
+            [C.c_void_p] * 6
         L.egso_mix64.restype = C.c_uint64
         L.egso_mix64.argtypes = [C.c_uint64]
         L.egso_sha256.argtypes = [C.c_char_p, C.c_uint64, C.c_void_p]
@@ -201,18 +222,15 @@ class OracleC:
     def peek_many(self, node_ids, req, planes: int = 4):
         """The cached option of `req` on each of `node_ids`: (present bool [n], score int64 [n], GPU masks u16
         [n, planes], one per container, up to 16 GPUs)."""
-        units, nc = _units(req), len(req)
-        off, idx, sc = np.zeros(nc + 1, np.int32), np.zeros(16 * nc + 1, np.int32), C.c_int64(0)
-        offp, idxp = _ptr(off), _ptr(idx)
-        present = np.zeros(len(node_ids), bool)
-        score = np.zeros(len(node_ids), np.int64)
-        masks = np.zeros((len(node_ids), planes), np.uint16)
-        for i, n in enumerate(node_ids):
-            if self.L.egso_peek(self.h, int(n), nc, units, C.byref(sc), offp, idxp):
-                present[i], score[i] = True, sc.value
-                for c in range(nc):
-                    masks[i, c] = sum(1 << int(g) for g in idx[off[c]:off[c + 1]])
-        return present, score, masks
+        ids = np.ascontiguousarray(node_ids, dtype=np.int32)
+        assert ids.size == 0 or (ids.min() >= 0 and ids.max() < self.n_nodes)
+        assert len(req) <= planes
+        present = np.zeros(len(ids), np.uint8)
+        score = np.zeros(len(ids), np.int64)
+        masks = np.zeros((len(ids), planes), np.uint16)
+        self.L.egso_peek_many(self.h, len(ids), _ptr(ids), len(req), _units(req), planes, _ptr(present), _ptr(score),
+                              _ptr(masks))
+        return present.astype(bool), score, masks
 
     def trade_fits(self, node_ids, req) -> np.ndarray:
         """Whether Trade of `req` succeeds on the current rows of each of `node_ids` (no cache effects)."""
@@ -262,6 +280,24 @@ class OracleC:
                                    vec_pods, _ptr(vf), _ptr(vs))
         if vec_pods:
             out["vec_fit"], out["vec_score"] = vf, vs
+        return out
+
+    def schedule_batch_indexed(self, c_off: np.ndarray, units: np.ndarray, uids: Optional[np.ndarray] = None,
+                               threads: int = 1):
+        """schedule_batch's decisions and six outputs through the indexed driver (egso_schedule_batch_indexed)."""
+        P = len(c_off) - 1
+        c_off = np.ascontiguousarray(c_off, dtype=np.int32)
+        units = np.ascontiguousarray(units, dtype=np.int64)
+        out = dict(node=np.zeros(P, np.int32), status=np.zeros(P, np.int32),
+                   alloc_mask=np.zeros((P, 4), np.uint8), fit_count=np.zeros(P, np.int32),
+                   fit_digest=np.zeros(P, np.uint64), score_digest=np.zeros(P, np.uint64))
+        u = None if uids is None else np.ascontiguousarray(uids, dtype=np.uint64)
+        rc = self.L.egso_schedule_batch_indexed(self.h, P, _ptr(c_off), _ptr(units), _ptr(u), threads,
+                                                _ptr(out["node"]), _ptr(out["status"]), _ptr(out["alloc_mask"]),
+                                                _ptr(out["fit_count"]), _ptr(out["fit_digest"]),
+                                                _ptr(out["score_digest"]))
+        if rc < 0:
+            raise ValueError("schedule_batch_indexed: two shapes of the batch share a faithful-mode cache key")
         return out
 
 
