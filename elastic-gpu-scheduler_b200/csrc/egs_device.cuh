@@ -122,8 +122,9 @@ __device__ __forceinline__ void load_row(const int32_t *__restrict__ core, const
 // after the Add on GPU g:
 //   * new value n = row[g] - req <= row[g], so  min' = min(min_all, n)           (no exclusion needed)
 //   * max' = max(max over rows != g, n): prefix/suffix maxima + one 3-input max
-//   * PAD (0x80000000) is the largest UNSIGNED and the smallest SIGNED value: an unsigned min
-//     and a signed max both ignore absent GPUs without any select (valid rows are >= 0).
+//   * PAD (INT32_MIN) is the smallest signed value: a signed max ignores absent GPUs without a select, the min
+//     skips them.  Rows can be negative -- ForgetPod of a sentinel unit takes 1 from a GPU (gpu.go:41-49) -- so the
+//     min is a signed one, as Go's.
 //   * score = Range/(1+1)*100 with Range = x/2, x >= 0  ==  (x >> 2) * 100        (rater.go:49-50)
 //   * candidates are folded as key = q*G + g: one max keeps the last maximal GPU.  q = x >> 2 with
 //     x <= 2*(EGS_MAX_MEM_PER_GPU + EGS_MAX_CORE_LOAD) < 2^26.1, so q < 2^24.1 and the largest key,
@@ -136,16 +137,18 @@ EGS_HD bool trade_single(const int (&c)[G], const int (&m)[G], int rc, int rm,
   constexpr int LG = RowWidth<G>::LG;
   int bestkey = -1;
   if (policy == EGS_BINPACK) {
-    unsigned ucmin = 0xFFFFFFFFu, ummin = 0xFFFFFFFFu;
+    int cmin = INT32_MAX, mmin = INT32_MAX;
     int cpre[G], csuf[G], mpre[G], msuf[G];
     cpre[0] = INT32_MIN; mpre[0] = INT32_MIN; csuf[G - 1] = INT32_MIN; msuf[G - 1] = INT32_MIN;
 #pragma unroll
-    for (int g = 0; g < G; g++) { ucmin = EGS_MIN(ucmin, (unsigned)c[g]); ummin = EGS_MIN(ummin, (unsigned)m[g]); }
+    for (int g = 0; g < G; g++) {
+      const bool real = c[g] != EGS_PAD;
+      cmin = real ? EGS_MIN(cmin, c[g]) : cmin; mmin = real ? EGS_MIN(mmin, m[g]) : mmin;
+    }
 #pragma unroll
     for (int g = 1; g < G; g++) { cpre[g] = EGS_MAX(cpre[g - 1], c[g - 1]); mpre[g] = EGS_MAX(mpre[g - 1], m[g - 1]); }
 #pragma unroll
     for (int g = G - 2; g >= 0; g--) { csuf[g] = EGS_MAX(csuf[g + 1], c[g + 1]); msuf[g] = EGS_MAX(msuf[g + 1], m[g + 1]); }
-    const int cmin = (int)ucmin, mmin = (int)ummin;
 #pragma unroll
     for (int g = 0; g < G; g++) {
       const bool ok = (c[g] >= rc) && (m[g] >= rm);         // CanAllocate gpu.go:55; PAD rows fail
@@ -170,17 +173,18 @@ EGS_HD bool trade_single(const int (&c)[G], const int (&m)[G], int rc, int rm,
 // Returns the lane's folded key -- (x >> 2) * 8 + gl under binpack, gl under spread, -1 when GPU gl does not fit;
 // the max over gl = 0..7 is trade_single's bestkey.  The max over the OTHER GPUs is a masked scan of the row.
 EGS_HD int trade_lane_key(const int (&c)[EGS_G], const int (&m)[EGS_G], int gl, int rq_c, int rq_m, int policy) {
-  unsigned ucmin = 0xFFFFFFFFu, ummin = 0xFFFFFFFFu;
+  int cmin = INT32_MAX, mmin = INT32_MAX;
   int cex = INT32_MIN, mex = INT32_MIN, cg = 0, mg = 0;
 #pragma unroll
   for (int g = 0; g < EGS_G; g++) {
-    ucmin = EGS_MIN(ucmin, (unsigned)c[g]); ummin = EGS_MIN(ummin, (unsigned)m[g]);
+    const bool real = c[g] != EGS_PAD;                           // signed min over the GPUs present (trade_single)
+    cmin = real ? EGS_MIN(cmin, c[g]) : cmin; mmin = real ? EGS_MIN(mmin, m[g]) : mmin;
     cex = EGS_MAX(cex, g == gl ? INT32_MIN : c[g]); mex = EGS_MAX(mex, g == gl ? INT32_MIN : m[g]);
     cg = g == gl ? c[g] : cg; mg = g == gl ? m[g] : mg;
   }
   const bool ok = cg >= rq_c && mg >= rq_m;                      // CanAllocate gpu.go:55; PAD rows fail
   const int nc = cg - rq_c, nm = mg - rq_m;                      // GPU.Add gpu.go:36-37
-  const int x = (EGS_MAX(mex, nm) + EGS_MAX(cex, nc)) - (EGS_MIN((int)ummin, nm) + EGS_MIN((int)ucmin, nc));
+  const int x = (EGS_MAX(mex, nm) + EGS_MAX(cex, nc)) - (EGS_MIN(mmin, nm) + EGS_MIN(cmin, nc));
   return !ok ? -1 : (policy == EGS_BINPACK ? (x >> 2) * 8 + gl : gl);
 }
 

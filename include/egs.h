@@ -17,7 +17,11 @@
  * (cgo rule), no torch types.  Every entry point returns an egs_status and
  * never aborts the process.  A handle serialises its callers with an internal
  * mutex (the reference holds one global lock per verb, scheduler.go:113,171,187)
- * and calls cudaSetDevice on entry, so cgo thread-hopping is fine.
+ * and calls cudaSetDevice on entry, so cgo thread-hopping is fine.  The text
+ * egs_last_error points to is the handle's own and is not guarded past the call
+ * that returns the pointer: the next failing call on the handle, from any thread,
+ * overwrites it.  A handle shared by several threads reads it (and copies it)
+ * only while no other thread can be calling the handle.
  *
  * The device state is an int32 SoA node/GPU cache:
  *   free_core[N][W], free_mem[N][W], mem_total[N]      W = EGS_ROW_WIDTH(g_max)

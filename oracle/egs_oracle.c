@@ -632,6 +632,19 @@ int egso_forget_pod(egso *o, int node, int C, const egso_unit *units, const int3
   if (set_has(&o->pod_maps, uid)) { set_del(&o->pod_maps, uid); set_add(&o->released, uid); }
   return ST_OK;
 }
+/* NodeAllocator.Add alone (node.go:148-160), as NewNodeAllocator replays a node's assumed pods (node.go:52-54): the
+ * node's podsMap and Transact, podMaps untouched. */
+int egso_replay_pod(egso *o, int node, int C, const egso_unit *units, const int32_t *alloc_off,
+                    const int32_t *alloc_idx, uint64_t uid) {
+  if (node < 0 || node >= o->nn || o->nodes[node].G == 0) return ST_BAD_ARG;
+  opt_t op;
+  if (!opt_import(&op, C, alloc_off, alloc_idx, o->nodes[node].G)) return ST_BAD_ARG;
+  node_add(&o->nodes[node], C, units, &op, uid);   /* a failed Transact keeps its Adds and the podsMap entry */
+  return ST_OK;
+}
+int egso_node_has_pod(egso *o, int node, uint64_t uid) {
+  return node >= 0 && node < o->nn && pods_has(&o->nodes[node], uid);
+}
 int egso_known_pod(egso *o, uint64_t uid) { return set_has(&o->pod_maps, uid); }
 int egso_released_pod(egso *o, uint64_t uid) { return set_has(&o->released, uid); }
 

@@ -77,6 +77,12 @@ int egso_forget_pod(egso *o, int node, int C, const egso_unit *units,
 /* TEST SUPPORT: load cached options of one shape (a scheduler that already ran); see egs_oracle.c */
 int egso_cache_load(egso *o, int C, const egso_unit *units, int n, const int32_t *node_ids,
                     const uint8_t *valid, const int64_t *score, const uint8_t *alloc_mask);
+/* NodeAllocator.Add alone (node.go:148-160), the replay of an assumed pod at node load: the node's podsMap and
+ * Transact; the scheduler-level podMaps is not touched.  ST_BAD_ARG for a node or GPU index out of range. */
+int egso_replay_pod(egso *o, int node, int C, const egso_unit *units,
+                    const int32_t *alloc_off, const int32_t *alloc_idx, uint64_t uid);
+/* TEST SUPPORT, read-only: whether node `node`'s podsMap (node.go:20) holds uid; 0 for a node out of range. */
+int egso_node_has_pod(egso *o, int node, uint64_t uid);
 int egso_known_pod(egso *o, uint64_t uid);
 int egso_released_pod(egso *o, uint64_t uid);
 

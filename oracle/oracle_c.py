@@ -79,6 +79,8 @@ def lib():
         L.egso_add_pod.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
         L.egso_forget_pod.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
         L.egso_cache_load.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.egso_replay_pod.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
+        L.egso_node_has_pod.argtypes = [C.c_void_p, C.c_int, C.c_uint64]
         L.egso_known_pod.argtypes = [C.c_void_p, C.c_uint64]
         L.egso_released_pod.argtypes = [C.c_void_p, C.c_uint64]
         L.egso_schedule_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + \
@@ -247,6 +249,15 @@ class OracleC:
     def forget_pod(self, node: int, req, alloc, uid: int) -> int:
         off, idx = _alloc_arrays(alloc)
         return self.L.egso_forget_pod(self.h, node, len(req), _units(req), _ptr(off), _ptr(idx), uid)
+
+    def replay_pod(self, node: int, req, alloc, uid: int) -> int:
+        """NodeAllocator.Add alone (egs_node_replay_pod): the node's podsMap and rows; podMaps stays."""
+        off, idx = _alloc_arrays(alloc)
+        return self.L.egso_replay_pod(self.h, node, len(req), _units(req), _ptr(off), _ptr(idx), uid)
+
+    def node_has_pod(self, node: int, uid: int) -> bool:
+        """Whether node `node`'s podsMap holds uid."""
+        return bool(self.L.egso_node_has_pod(self.h, node, uid))
 
     def cache_load(self, req, valid, score, alloc_mask) -> int:
         """Install cached options of shape `req` on nodes 0..n-1 (state of a scheduler that already ran)."""

@@ -1,5 +1,5 @@
 """The kernels' integer arithmetic -- csrc/egs_device.cuh: the Trade fast path (prefix/suffix maxima,
-unsigned-min PAD trick, packed q*8+g key) and its one-GPU-per-lane form in the resolver, the general DFS Trade,
+signed min over the GPUs present, packed q*8+g key) and its one-GPU-per-lane form in the resolver, the general DFS Trade,
 Transact and the AddPod / ForgetPod row update -- compiled for the host
 (csrc/host_test/device_on_host.cu) and checked against the oracle WITHOUT a GPU.  Same source the kernels
 inline; the device SASS is unaffected by the host build."""
@@ -121,6 +121,21 @@ def test_fast_path_single_container_large_values(DH, rows, core, mem, policy):
     assert DH.egsdh_is_single(1, u.ctypes.data) == 1
     assert _trade(DH, rows, mt, req, policy, 0) == want
     assert _trade_lanes(DH, rows, req, policy) == want
+
+
+@settings(max_examples=600, deadline=None)
+@given(rows=st.lists(st.tuples(st.integers(-3, 101), st.integers(-3, 41)), min_size=1, max_size=8),
+       req=st.lists(unit, min_size=1, max_size=4), policy=st.integers(0, 1), mt=st.integers(1, 40))
+def test_trade_on_rows_below_zero(DH, rows, req, policy, mt):
+    """Rows below zero, which ForgetPod of a sentinel unit reaches (GPU.Sub adds -1, gpu.go:41-49): every Trade
+    path rates with Go's signed minimum over the GPUs present."""
+    g = [po.GPU(c, m, 100, mt) for c, m in rows]
+    opt = po.trade(g, po.RATERS[policy], list(req))
+    want = None if opt is None else (opt.allocated, opt.score)
+    assert _trade(DH, rows, mt, req, policy, 0) == want
+    assert _trade(DH, rows, mt, req, policy, 1) == want
+    if DH.egsdh_is_single(len(req), _units(req).ctypes.data):
+        assert _trade_lanes(DH, rows, req, policy) == want
 
 
 @settings(max_examples=400, deadline=None)
